@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native hot path (contract: see DESIGN.md section 6).
+"""bench.py -- headline benchmark of the CUDA-native (H100, sm_90a) hot path (contract: see DESIGN.md section 6).
 
     python bench.py --gpus 1 --steps K --warmup W            # our arm
     python bench.py --impl reference --steps K --warmup W     # CPU restatement of the reference path
@@ -33,15 +33,14 @@ C2 = dict(slots=26, rows=1_000_000, dim=16, batch=65536, dnn=[256, 32])
 C5 = dict(slots=26, rows=3_846_154, dim=128, batch=65536, dnn=[512, 256])
 
 
-def measured_peaks():
-    try:
-        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
-    except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+def peaks():
+    """NVIDIA's data-sheet HBM3 bandwidth of the H100 SXM: the roofline's denominator.  The line also carries the card's
+    name (`clocks.gpu`): on any other card `frac` is relative to the wrong peak."""
+    return {"hbm_gbs": 3350.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi sampler running during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampler running during the timed region (SM clock, power draw and throttle reasons, so a throttled run can be told apart)."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -49,7 +48,7 @@ class ClockSampler:
     def __enter__(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-             "clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_power_cap,power.limit,name")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits",
                                           "-lms", "100", "-i", str(self.index)],
@@ -88,7 +87,9 @@ class ClockSampler:
         if not sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": [], "samples": 0}
         sm.sort()
-        return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": max(mx), "reasons": sorted(reasons), "samples": len(sm)}
+        return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": max(mx), "reasons": sorted(reasons), "samples": len(sm),
+                "power_limit_w": self.rows[-1][7] if len(self.rows[-1]) > 8 else None,
+                "gpu": self.rows[-1][8] if len(self.rows[-1]) > 8 else None}
 
 
 def run_reference(args):
@@ -142,7 +143,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--no-graph", action="store_true", help="launch the step eagerly (for ncu launch lists)")
+    ap.add_argument("--no-graph", action="store_true", help="launch the step eagerly instead of replaying the CUDA graph")
     ap.add_argument("--workload", default="c2", choices=["c2", "c5"],
                     help="c2 (default, the headline config; weak scaling) or c5 (100M rows x D=128, global batch 65536)")
     ap.add_argument("--ids", default="uniform", choices=["uniform", "zipf"],
@@ -153,12 +154,16 @@ def main():
                     help="N=1: sgd (default, fused row-sparse SGD), adam (TF-exact dense ApplyAdam over the arena), lazy_adam "
                          "(row-sparse, two kernels), adam_rows (row-sparse Adam fused into the backward scatter)")
     ap.add_argument("--embed-fwd", default="ldg", choices=["ldg", "tma"],
-                    help="N=1: forward gather through register loads (default) or staged through TMA tile::gather4 (opt-in, measured slower)")
+                    help="N=1: forward gather through register loads (default) or staged through TMA bulk copies (opt-in)")
     ap.add_argument("--fwd-chunks", type=int, default=1,
                     help="N=1: run the gather and the first tower GEMM as this many alternating launches over slices of the batch")
     ap.add_argument("--dw-first", type=int, default=0, help="N=1: enqueue the layer-0 dW GEMM before the embedding update")
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "nccl"],
                     help="N>1: fused NVLink peer-memory gather/update (p2p) or NCCL all-to-all pipeline (nccl)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (loss, predicted probabilities) and "
+                         "left behind (tower parameters, a seeded sample of embedding rows) as DIR/<name>.npy in float32; same "
+                         "arguments -> same inputs, so two builds can be compared output for output")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
@@ -272,6 +277,18 @@ def main():
     ms = max_over_ranks(e0.elapsed_time(e1))
     value = B * world * args.steps / (ms * 1e-3)
     final_loss = float(trainer.loss.item())
+    if args.dump_outputs:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        suffix = "" if world == 1 else f"_rank{rank}"
+        # what the step returns (loss, probabilities) and what it leaves behind for the next step: the tower parameters
+        # and a fixed, seeded sample of rows of this rank's embedding arena (the update kernels' output)
+        arena = trainer.coll.weight if world == 1 else trainer.emb.weight
+        pick = torch.from_numpy(np.random.default_rng(7).integers(0, arena.shape[0], size=65536)).to(dev)
+        outs = {"loss": trainer.loss, "prob": trainer.prob, "tower": trainer.flat, "embedding_rows_sample": arena.detach()[pick]}
+        for name, out in outs.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}{suffix}.npy"),
+                    out.detach().float().cpu().numpy().reshape(-1))
 
     # ---- end-to-end: host buffers in, loss out, copies inside the timed region --------------------
     # (a) the public epoch loop `trainer.fit_host(batches)`: per step the H2D copy of the batch from pinned host memory, the
@@ -318,16 +335,11 @@ def main():
         return
 
     # ---- roofline of the headline kernel (fused gather+FM forward) ---------------------------------
-    peaks, peak_kind = measured_peaks()
+    peak, peak_kind = peaks()
     # SURVEY 8(d): ids + rows + first-order weights + stacked write + logit (3 644 B / example at C2); the kernel also
     # writes the sum_e side output the backward reads (4 D B / example) -- reported separately, not in `frac`
     alg_bytes = B * (S * (8 + 4 * D + 4) + 4 * S * D + 4)
     alg_bytes_with_sum = alg_bytes + B * 4 * D
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "embed_fwd_traffic.json")))["dram_bytes_per_launch"]
-    except Exception:
-        pass
     # duration of the headline kernel: (a) INSIDE the step -- CUDA events on the launching stream around the kernel in the
     # eager per-kernel pass over the timed region's batches (the L2 / DRAM state the kernel really meets in training);
     # (b) back to back -- the same launch repeated with nothing in between, where every launch also pays for writing back
@@ -339,16 +351,14 @@ def main():
                 "how": f"mean duration of the kernel inside the step (CUDA events on the launching stream before / after it, "
                        f"eager passes over {max(10, args.steps)} steps of the id pool) = kernel_ms.{step_key}; "
                        "back_to_back = the same launch repeated between two events",
-                "achieved": alg_bytes / fwd_s / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": alg_bytes / fwd_s / 1e9 / peaks["hbm_gbs"], "traffic": traffic,
-                "traffic_source": "profiles/embed_fwd_traffic.json (ncu --set full capture of this kernel at this config; "
-                                  "not re-measured inside this run)",
+                "achieved": alg_bytes / fwd_s / 1e9, "peak": peak["hbm_gbs"], "unit": "GB/s",
+                "frac": alg_bytes / fwd_s / 1e9 / peak["hbm_gbs"],
                 "peak_source": peak_kind, "algorithmic_bytes_per_launch": alg_bytes,
                 "bytes_convention": "SURVEY 8(d): S*(8+4D+4) + 4*S*D + 4 per example",
-                "frac_incl_sum_e_output": alg_bytes_with_sum / fwd_s / 1e9 / peaks["hbm_gbs"],
+                "frac_incl_sum_e_output": alg_bytes_with_sum / fwd_s / 1e9 / peak["hbm_gbs"],
                 "us_per_launch": fwd_s * 1e6,
                 "back_to_back": {"us_per_launch": b2b_s * 1e6, "achieved": alg_bytes / b2b_s / 1e9,
-                                 "frac": alg_bytes / b2b_s / 1e9 / peaks["hbm_gbs"]}}
+                                 "frac": alg_bytes / b2b_s / 1e9 / peak["hbm_gbs"]}}
 
     cpu = None
     if not args.no_cpu_baseline and world == 1 and args.workload == "c2":     # CPU arm on rank 0 at N=1 only (torchrun pins OMP threads to 1)
@@ -368,8 +378,8 @@ def main():
             "launches_per_step": int(trainer.launches_per_step), "roofline": roofline, "kernel_ms": shares,
             "cpu_baseline": cpu, "final_loss": final_loss,
             "cuda_graph": trainer.graph is not None,
-            "gemm_core": {0: "ffma", 1: "tcgen05 3xTF32, pre-split planes (tc)",
-                          2: "tcgen05 3xTF32, hi/lo split in kernel (tc2); outputs >= 128 wide on the CTA-pair kernel (cta_group::2)"}[_lib._tc_variant if _lib._tc_enabled and not gemm_note else (1 if gemm_note else 0)],
+            "gemm_core": {0: "ffma", 1: "wgmma 3xTF32, pre-split planes (tc)",
+                          2: "wgmma 3xTF32, hi/lo split in kernel (tc2)"}[_lib._tc_variant if _lib._tc_enabled and not gemm_note else (1 if gemm_note else 0)],
             "exchange": getattr(trainer, "exchange", None) if world > 1 else None,
             "optimizer": args.optimizer if world == 1 else "sgd", "embed_fwd": args.embed_fwd if world == 1 else "ldg",
             "fwd_chunks": args.fwd_chunks if world == 1 else 1, "dw_first": bool(args.dw_first)}

@@ -1,6 +1,6 @@
 """Import alias: ``deep_recommenders.*`` resolves to ``deep_recommenders_b200.*`` so the reference's
 own import lines (``from deep_recommenders.keras.models.ranking import DeepFM`` ...) work
-unchanged against the B200-native implementation."""
+unchanged against the CUDA-native implementation."""
 import importlib
 import importlib.abc
 import importlib.util

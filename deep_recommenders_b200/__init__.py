@@ -1,4 +1,4 @@
-"""deep_recommenders_b200 -- B200-native (sm_100a) implementation of the data-parallel hot path of
+"""deep_recommenders_b200 -- CUDA-native (H100, sm_90a) implementation of the data-parallel hot path of
 LongmaoTeamTf/deep_recommenders: embedding lookup -> FM / DeepFM / DCN Cross, and the two-tower
 in-batch softmax, forward and backward, behind the reference's Keras-layer API.
 

@@ -32,7 +32,6 @@ _SIGS = {
     "dr_tune_get": [C.c_char_p, _p],
     "dr_set_workspace": [_p, C.c_uint64],
     "dr_gemm_plane_cache": [_i],
-    "dr_gemm_prof_read": [_p, _i],
     "dr_debug_gemm": [_p, _p, _p, _i64, _i64, _i64, _i, _i, _p],
     "dr_embed_fm_fwd": [_p, _p, _p, _p, _i, _p, _i64, _i, _i, _i64, _i64, _i, _p, _p, _p, _p],
     "dr_embed_fm_fwd_tma": [_p, _i64, _p, _p, _p, _i, _p, _i64, _i, _i, _i64, _p, _p, _p, _p],
@@ -175,7 +174,7 @@ def set_workspace(nbytes: int, device=None):
 
 
 def enable_tensor_core_gemm(workspace_bytes: int = 0, device=None, variant: int = None) -> None:
-    """Route eligible GEMMs (Dense / Cross / scores) to a tcgen05 3xTF32 kernel: variant 1 = pre-split hi/lo planes
+    """Route eligible GEMMs (Dense / Cross / scores) to the wgmma 3xTF32 kernel: variant 1 = pre-split hi/lo planes
     (needs the registered workspace), variant 2 = split in shared memory inside the GEMM (no workspace).
     Default: the variant selected by DR_GEMM (tc -> 1, tc2 -> 2)."""
     global _tc_enabled, _tc_applied
@@ -192,9 +191,8 @@ def disable_tensor_core_gemm() -> None:
     _tc_enabled = False
 
 
-# DR_GEMM selects the default GEMM core: tc2 (default) = tcgen05 3xTF32 with the hi/lo split inside the kernel
-# (bit-identical outputs to tc, 17-23 % faster at the C2 layer shapes: profiles/check_gemm_insplit_r01.json),
-# tc = tcgen05 3xTF32 on pre-split planes, ffma = FFMA.
+# DR_GEMM selects the default GEMM core: tc2 (default) = wgmma 3xTF32 with the hi/lo split inside the kernel,
+# tc = wgmma 3xTF32 on pre-split planes, ffma = FFMA.
 _tc_enabled = _GEMM_ENV != "ffma"
 _tc_variant = 1 if _GEMM_ENV == "tc" else 2
 _tc_applied = False

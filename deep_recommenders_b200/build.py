@@ -1,7 +1,7 @@
 """Builds libdeeprec_b200.so (the C-ABI library of include/deeprec_b200.h) in-tree with nvcc.
 
-sm_100a only: `-gencode arch=compute_100a,code=sm_100a`.  nvcc cross-compiles without a GPU,
-so this runs on the CPU build box; the resulting .so travels with the tree to the GPU box.
+sm_90a only: `-gencode arch=compute_90a,code=sm_90a`.  nvcc cross-compiles without a GPU,
+so the library can be built on a machine that has none.
 Object files are cached per source under deep_recommenders_b200/lib/obj and rebuilt when the
 source, a header, or the flags change.
 """
@@ -22,7 +22,7 @@ LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libdeeprec_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -47,7 +47,7 @@ def _digest(src: Path, headers: list[Path]) -> str:
 
 
 def build(verbose: bool = False, force: bool = False) -> Path:
-    """Compile every csrc/*.cu for sm_100a and link the shared library. Returns its path."""
+    """Compile every csrc/*.cu for sm_90a and link the shared library. Returns its path."""
     nvcc = _nvcc()
     objdir = LIBDIR / "obj"
     objdir.mkdir(parents=True, exist_ok=True)
@@ -81,7 +81,7 @@ def build(verbose: bool = False, force: bool = False) -> Path:
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(_compile, jobs))
     if jobs or not LIB.exists():
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB), *map(str, objs)]
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB), *map(str, objs)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -15,17 +15,25 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
+int num_sms() {
+  static const int n = [] {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v < 1)
+      v = 132;   // no device visible (host-only callers): the H100 SXM count, never used for a launch
+    return v;
+  }();
+  return n;
+}
 void count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_relaxed); }
 
 extern int g_tune_embed_fwd_unroll, g_tune_embed_bwd_unroll, g_tune_embed_block, g_tune_embed_ctas_per_sm,
     g_tune_embed_bwd_agg, g_tune_embed_bwd_mode, g_tune_embed_fwd_minblocks, g_tune_embed_fwd_linx, g_tune_embed_fwd_linx_shard, g_tune_embed_bwd_linx, g_tune_embed_l2_hints, g_tune_embed_bwd_carveout;
 extern int g_tune_topk_variant;
-extern int g_tune_gemm_prof, g_tune_tc_tma_out, g_tune_tc_stages, g_tune_tc_l2_promo, g_tune_tc_dw_stages, g_tune_tc_dw_share, g_tune_tc_pair;
-extern int g_tune_gemm_variant, g_tune_gemm_splitk, g_tune_gemm_bn, g_tune_tc_mn, g_tune_tc_min_n;
+extern int g_tune_tc_stages, g_tune_tc_l2_promo, g_tune_tc_dw_stages, g_tune_tc_dw_share, g_tune_tc_pair;
+extern int g_tune_gemm_variant, g_tune_gemm_splitk, g_tune_gemm_bn, g_tune_tc_min_n;
 
 }  // namespace dr
 
-namespace dr { int gemm_set_store_hi(int v); }
 extern "C" int dr_version(void) { return 100; /* 0.1.0 */ }
 extern "C" const char* dr_last_error(void) { return dr::g_err; }
 extern "C" uint64_t dr_launch_count(void) { return dr::g_launches.load(std::memory_order_relaxed); }
@@ -65,14 +73,10 @@ extern "C" int dr_tune_set(const char* key, int value) {
   else if (!strcmp(key, "gemm_variant")) g_tune_gemm_variant = value;
   else if (!strcmp(key, "gemm_splitk")) g_tune_gemm_splitk = value;
   else if (!strcmp(key, "gemm_bn")) g_tune_gemm_bn = value;
-  else if (!strcmp(key, "tc_mn")) g_tune_tc_mn = value;
   else if (!strcmp(key, "tc_min_n")) g_tune_tc_min_n = value;
   else if (!strcmp(key, "topk_variant")) g_tune_topk_variant = value;
-  else if (!strcmp(key, "gemm_prof")) g_tune_gemm_prof = value;
-  else if (!strcmp(key, "tc_tma_out")) g_tune_tc_tma_out = value;
   else if (!strcmp(key, "tc_stages")) g_tune_tc_stages = value;
   else if (!strcmp(key, "tc_l2_promo")) g_tune_tc_l2_promo = value;
-  else if (!strcmp(key, "tc_store_hi")) return gemm_set_store_hi(value);
   else if (!strcmp(key, "tc_dw_stages")) g_tune_tc_dw_stages = value;
   else if (!strcmp(key, "tc_dw_share")) g_tune_tc_dw_share = value;
   else if (!strcmp(key, "tc_pair")) g_tune_tc_pair = value;

@@ -125,7 +125,7 @@ extern "C" int dr_embed_bag_fwd(const float* table, int64_t rows, int64_t row_st
   const int group = bag_group(vec ? D / 4 : D);
   const int per_block = 256 / group;
   int64_t ctas = (B + per_block - 1) / per_block;
-  if (ctas > kNumSMs * 16) ctas = kNumSMs * 16;
+  if (ctas > num_sms() * 16) ctas = num_sms() * 16;
   cudaStream_t st = (cudaStream_t)stream;
 #define DR_BAG_FWD(IdT, VEC)                                                                                     \
   embed_bag_fwd_kernel<IdT, VEC><<<(unsigned)ctas, 256, 0, st>>>(table, rows, row_stride, (const IdT*)ids,        \
@@ -148,7 +148,7 @@ extern "C" int dr_embed_bag_bwd(const void* ids, int id_bytes, const int64_t* ro
   const int group = bag_group(vec ? D / 4 : D);
   const int per_block = 256 / group;
   int64_t ctas = (B + per_block - 1) / per_block;
-  if (ctas > kNumSMs * 16) ctas = kNumSMs * 16;
+  if (ctas > num_sms() * 16) ctas = num_sms() * 16;
   cudaStream_t st = (cudaStream_t)stream;
 #define DR_BAG_BWD(IdT, VEC)                                                                                     \
   embed_bag_bwd_kernel<IdT, VEC><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, row_splits, B, D, combiner,     \

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libdeeprec_b200.so (sm_100a only).
+// Shared host/device helpers for libdeeprec_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,12 +7,14 @@
 #include "deeprec_b200.h"
 
 #ifndef __CUDA_ARCH_LIST__
-#define __CUDA_ARCH_LIST__ 1000
+#define __CUDA_ARCH_LIST__ 900
 #endif
 
 namespace dr {
 
-constexpr int kNumSMs = 148;   // B200: 2 dies x 74 SMs
+// SMs of the current device (132 on an H100 SXM, fewer on a PCIe card or a MIG slice): sizes every persistent grid and
+// split-K heuristic.  Queried once per process (api.cu).
+int num_sms();
 
 // ---- error plumbing -------------------------------------------------------------------
 void set_error(const char* fmt, ...);

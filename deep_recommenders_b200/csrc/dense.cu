@@ -42,7 +42,7 @@ __global__ void __launch_bounds__(256) actgrad_colsum_kernel(const float* __rest
 
 // Same, for 16-B aligned rows with N a multiple of 4 and N <= 128 * NV: one warp owns whole rows (float4 per lane, NV per
 // row), four rows in flight per warp, column sums in registers until the end (the generic kernel above walks 32-column
-// strips with one 4-byte load in flight per thread: 45 us for the 65536 x 256 bias gradient of the C2 step, 1.5 TB/s).
+// strips with one 4-byte load in flight per thread).
 template <int NV>
 __global__ void __launch_bounds__(256) actgrad_colsum_v4_kernel(const float* gy, const float* __restrict__ y, int act,
                                                                  int64_t M, int N, float* gz, float* __restrict__ gb) {
@@ -107,7 +107,7 @@ static int launch_actgrad_colsum(const float* gy, const float* y, int act, int64
     const int nv = (int)((N / 4 + 31) / 32);
     const int threads = 256, warps = threads / 32;
     int64_t ctas = (M + warps * 4 - 1) / (warps * 4);
-    if (ctas > (int64_t)kNumSMs * 4) ctas = (int64_t)kNumSMs * 4;
+    if (ctas > (int64_t)num_sms() * 4) ctas = (int64_t)num_sms() * 4;
     if (ctas < 1) ctas = 1;
     const size_t smem = (size_t)warps * N * sizeof(float);
     if (nv <= 1) actgrad_colsum_v4_kernel<1><<<(unsigned)ctas, threads, smem, st>>>(gy, y, act, M, (int)N, gz, gb);
@@ -162,7 +162,7 @@ int g_tune_tc_dw_stages = 0;   // 2: weight-gradient GEMMs use the two-stage rin
 int g_tune_tc_dw_share = 0;    // 1: weight-gradient GEMMs use the co-residency build (capped registers, smaller staging)
 
 static int64_t rows_per_cta_for(int64_t M) {
-  int64_t r = (M + (int64_t)kNumSMs * 4 - 1) / ((int64_t)kNumSMs * 4);
+  int64_t r = (M + (int64_t)num_sms() * 4 - 1) / ((int64_t)num_sms() * 4);
   r = (r + 7) / 8 * 8;
   return r < 8 ? 8 : r;
 }
@@ -172,7 +172,7 @@ static int splitk_for(int64_t Mo, int64_t No, int64_t K) {
   const int64_t bn = No > 64 ? 128 : (No > 16 ? 32 : 16);
   const int64_t bm = No > 16 ? 128 : 256;
   const int64_t tiles = ((Mo + bm - 1) / bm) * ((No + bn - 1) / bn);
-  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
+  int64_t s = (2 * num_sms() + tiles - 1) / tiles;
   const int64_t ktiles = (K + 15) / 16;
   if (s > ktiles / 8) s = ktiles / 8;
   if (s < 1) s = 1;
@@ -211,11 +211,11 @@ int softmax_scores_block(const float* q_blk, const float* c, const float* p, con
 int softmax_grad_block(const float* g_ws, const float* q_blk, const float* c, int64_t rb, int64_t nc, int D, float* gq_blk,
                        float* gc, cudaStream_t st) {
   GemmArgs a = mk(g_ws, c, gq_blk, rb, D, nc, nc, D, D, EPI_STORE);
-  // few query rows (a sharded rank's b x (G b) block): rb / 128 output tiles cannot fill 148 SMs -- split the long
-  // contraction over the candidates instead (partial sums meet through TMA reduce-adds into the zeroed gq block)
+  // few query rows (a sharded rank's b x (G b) block): rb / 128 output tiles cannot fill the SMs -- split the long
+  // contraction over the candidates instead (partial sums meet through global reductions into the zeroed gq block)
   const int64_t tiles = ((rb + 127) / 128) * ((D + 63) / 64);
-  if (tiles < kNumSMs / 2 && nc >= 1024) {
-    int64_t sk = (kNumSMs + tiles - 1) / tiles;
+  if (tiles < num_sms() / 2 && nc >= 1024) {
+    int64_t sk = (num_sms() + tiles - 1) / tiles;
     if (sk > nc / 256) sk = nc / 256;
     if (sk > 1) {
       DR_CUDA_CALL(cudaMemsetAsync(gq_blk, 0, sizeof(float) * (size_t)rb * D, st));

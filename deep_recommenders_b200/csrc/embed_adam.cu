@@ -398,7 +398,7 @@ extern "C" int dr_embed_adam_count(const void* ids, int id_bytes, int64_t B, int
   DR_REQUIRE(ids && rows && slot_offsets && state, DR_EINVAL, "dr_embed_adam_count: null pointer");
   const int64_t n = B * S;
   int64_t ctas = (n + 255) / 256;
-  if (ctas > (int64_t)kNumSMs * 16) ctas = (int64_t)kNumSMs * 16;
+  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
   const int SS = adam_state_stride(D);
   cudaStream_t st = (cudaStream_t)stream;
   if (id_bytes == 8)
@@ -444,7 +444,7 @@ static int embed_fm_bwd_adam_impl(const char* fn, const void* ids, int id_bytes,
   const int threads = 256, warps = threads / 32;
   const size_t smem = (size_t)S * (sizeof(void*) * 2 + sizeof(int64_t) * 2);
   int64_t ctas = (B + warps - 1) / warps;
-  if (ctas > (int64_t)kNumSMs * 8) ctas = (int64_t)kNumSMs * 8;
+  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
   cudaStream_t st = (cudaStream_t)stream;
 #define DR_ADAM2(L, IdT)                                                                                        \
   do {                                                                                                          \
@@ -517,7 +517,7 @@ extern "C" int dr_embed_adam_prepare(const void* ids, int id_bytes, int64_t B, i
   const int lpr = lpr_of(D);
   const int64_t n = B * S;
   int64_t ctas = (n * lpr + 255) / 256;
-  if (ctas > (int64_t)kNumSMs * 16) ctas = (int64_t)kNumSMs * 16;
+  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
   cudaStream_t st = (cudaStream_t)stream;
 #define DR_PREP2(L, IdT)                                                                                               \
   embed_adam_prepare_kernel<L, IdT><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, n, S, D, rows, slot_offsets, table_ptrs, \
@@ -553,7 +553,7 @@ extern "C" int dr_embed_adam_flush(const int64_t* rows, const int64_t* slot_offs
   const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
   const int lpr = lpr_of(D);
   int64_t ctas = (total_rows * lpr + 255) / 256;
-  if (ctas > (int64_t)kNumSMs * 16) ctas = (int64_t)kNumSMs * 16;
+  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
   cudaStream_t st = (cudaStream_t)stream;
 #define DR_FLUSH(L)                                                                                                 \
   embed_adam_flush_kernel<L><<<(unsigned)ctas, 256, 0, st>>>(table_ptrs, lin_in_row ? nullptr : lin_ptrs, rows, slot_offsets, S, \

@@ -26,8 +26,8 @@ int g_tune_embed_block = 256;         // threads per CTA
 int g_tune_embed_ctas_per_sm = 0;     // 0 = as many as fit (2048 threads / SM)
 int g_tune_embed_bwd_agg = 1;         // example-parallel mode: warp-aggregate duplicate ids before the atomics
 int g_tune_embed_bwd_mode = 0;        // 0 = slot-parallel (default), 1 = example-parallel (+ optional aggregation)
-int g_tune_embed_fwd_linx = 1;        // 1 (default) = LINX forward mapping for in-row first-order weights: measured 70.0 us
-                                      // vs 86.0 us at C2 (tools/ab_embed_fwd.py, profiles/ab_embed_fwd_r01.json), bit-identical
+int g_tune_embed_fwd_linx = 1;        // 1 (default) = LINX forward mapping for in-row first-order weights (no idle lanes,
+                                      // twice the rows in flight per warp); 0 = a lane of its own for the weight; bit-identical
 int g_tune_embed_bwd_linx = 0;        // LINX mapping for the slot-parallel backward (in-row weight, D <= 32): unmeasured
 int g_tune_embed_fwd_linx_shard = 0;  // same mapping for the row-sharded (peer-memory) forward: off until measured at N > 1
 int g_tune_embed_l2_hints = 0;        // bit 0: forward row loads L2::evict_first; bit 1: stacked-output stores L2::evict_last;
@@ -571,7 +571,7 @@ static LaunchGeom geom(int64_t B, int S, int LPR, int id_bytes) {
   int64_t ctas = (ntiles + warps - 1) / warps;
   int per_sm = 2048 / lg.threads;
   if (g_tune_embed_ctas_per_sm > 0 && g_tune_embed_ctas_per_sm < per_sm) per_sm = g_tune_embed_ctas_per_sm;
-  const int64_t cap = (int64_t)kNumSMs * per_sm;
+  const int64_t cap = (int64_t)num_sms() * per_sm;
   if (ctas > cap) ctas = cap;
   if (ctas < 1) ctas = 1;
   lg.ctas = (int)ctas;
@@ -604,7 +604,7 @@ static int launch_fwd_u(const EmbedFwdParams& p, cudaStream_t st) {
       if (g_tune_embed_ctas_per_sm > 0 && g_tune_embed_ctas_per_sm < per_sm) per_sm = g_tune_embed_ctas_per_sm;
       const int64_t warps = lg.threads / 32, G = 32 / LPR;
       int64_t ctas = ((p.B + G - 1) / G + warps - 1) / warps;
-      if (ctas > (int64_t)kNumSMs * per_sm) ctas = (int64_t)kNumSMs * per_sm;   // one resident wave
+      if (ctas > (int64_t)num_sms() * per_sm) ctas = (int64_t)num_sms() * per_sm;   // one resident wave
       if (ctas < 1) ctas = 1;
       if (minb >= 4) {
         embed_fm_fwd_kernel<LPR, IdT, UU, false, 4, LINXSEL><<<(unsigned)ctas, lg.threads, lg.smem, st>>>(p);
@@ -681,13 +681,13 @@ static int launch_bwd_sp_u(const EmbedBwdParams& p, cudaStream_t st) {
   const size_t smem = (size_t)p.S * (sizeof(void*) * 2 + sizeof(int64_t) * 2) + kMaxShardWorld * sizeof(void*);
   int64_t ctas = (p.B + warps - 1) / warps;
   int per_sm = g_tune_embed_ctas_per_sm > 0 ? g_tune_embed_ctas_per_sm : 8;
-  if (ctas > (int64_t)kNumSMs * per_sm) ctas = (int64_t)kNumSMs * per_sm;
+  if (ctas > (int64_t)num_sms() * per_sm) ctas = (int64_t)num_sms() * per_sm;
   if (ctas < 1) ctas = 1;
   void (*k)(EmbedBwdParams) = p.shard_world > 0 ? embed_fm_bwd_sp_kernel<LPR, IdT, U, true>
                               : (LINX ? embed_fm_bwd_sp_kernel<LPR, IdT, U, false, LINX>
                                       : embed_fm_bwd_sp_kernel<LPR, IdT, U, false>);
-  // The update runs beside the persistent tcgen05 weight-gradient GEMM, which configures its SMs with the maximum
-  // shared-memory carveout (214+ KB of dynamic shared memory).  A kernel that prefers another L1 / shared split cannot
+  // The update runs beside the persistent wgmma weight-gradient GEMM, which configures its SMs with the maximum
+  // shared-memory carveout (up to 224 KB of dynamic shared memory).  A kernel that prefers another L1 / shared split cannot
   // become resident on an SM in that configuration, so the update asks for the same carveout (it uses 2 KB either way).
   if (g_tune_embed_bwd_carveout)
     DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, g_tune_embed_bwd_carveout));
@@ -833,7 +833,7 @@ extern "C" int dr_gather_fwd(const float* table, int64_t rows, const void* ids, 
   DR_REQUIRE(aligned16(table) && aligned16(out), DR_EALIGN, "dr_gather_fwd: table/out not 16-B aligned");
   const int chunks = D / 4;
   int64_t ctas = (n * chunks + 255) / 256;
-  if (ctas > (int64_t)kNumSMs * 8) ctas = (int64_t)kNumSMs * 8;
+  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
   cudaStream_t st = (cudaStream_t)stream;
   if (id_bytes == 8)
     gather_rows_kernel<int64_t><<<(unsigned)ctas, 256, 0, st>>>(table, rows, (const int64_t*)ids, n, chunks, out);
@@ -852,7 +852,7 @@ extern "C" int dr_scatter_add(float* grad_table, int64_t rows, const void* ids, 
   DR_REQUIRE(aligned16(grad_table) && aligned16(g), DR_EALIGN, "dr_scatter_add: table/g not 16-B aligned");
   const int chunks = D / 4;
   int64_t ctas = (n * chunks + 255) / 256;
-  if (ctas > (int64_t)kNumSMs * 8) ctas = (int64_t)kNumSMs * 8;
+  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
   cudaStream_t st = (cudaStream_t)stream;
   if (id_bytes == 8)
     scatter_add_rows_kernel<int64_t><<<(unsigned)ctas, 256, 0, st>>>(grad_table, rows, (const int64_t*)ids, n, chunks, g, scale);

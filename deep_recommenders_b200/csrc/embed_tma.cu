@@ -1,17 +1,14 @@
-// Opt-in variant of the fused gather + first-order + FM forward (rows E + L + F) that STAGES THE ROWS THROUGH TMA INTO
-// SHARED MEMORY: `cp.async.bulk.tensor.2d ... tile::gather4` (UTMALDG.2D.GATHER4) fetches four table rows by index per
-// instruction into a per-warp tile, completion on an mbarrier, the FM sums are computed from shared memory and the stacked
-// rows leave as one `cp.async.bulk` store per tile.  Same reference lines as embed_fm.cu
-// (keras/models/ranking/fm.py:23-37, deepfm.py:36-46).
+// Opt-in variant of the fused gather + first-order + FM forward (rows E + L + F) that STAGES THE ROWS THROUGH THE TMA
+// UNIT INTO SHARED MEMORY: one `cp.async.bulk.shared::cluster.global` (UBLKCP) per looked-up row copies its D floats into
+// a per-warp tile (Hopper's TMA has no gather-by-index tensor mode, so every row is its own bulk copy), completion on an
+// mbarrier, the FM sums are computed from shared memory and the stacked rows leave as one `cp.async.bulk` store per tile.
+// Same reference lines as embed_fm.cu (keras/models/ranking/fm.py:23-37, deepfm.py:36-46).
 //
-// Why it is NOT the default: measured on B200 at C2 (tools/mb_gather.cu, profiles/mb_gather_r02_*.jsonl and the bench
-// lines of this kernel) the TMA path is slower than register loads for this access pattern -- a gather4 costs the SM's
-// TMA unit ~46 cycles per 4 rows, the register path is bound by the DRAM's random-row rate before that -- and for skewed
-// (Zipf) ids the hot rows are L2 hits already.  It exists so that the comparison is a product measurement, not a claim.
+// It is NOT the default: the register-load kernel of embed_fm.cu is.  This one exists so that the comparison between
+// the two is a product measurement (bench.py --embed-fwd tma), not a claim.
 //
 // Scope: the fused row layout of embedding.py (one 128-B line [emb D | w | pad] per row, all tables in one arena),
 // D = 16, S <= 32.  Everything else uses dr_embed_fm_fwd.
-#include <cuda.h>
 #include "common.cuh"
 
 namespace dr {
@@ -34,11 +31,10 @@ __device__ __forceinline__ void t_mbar_wait(uint32_t bar, uint32_t parity) {
       ::"r"(bar), "r"(parity)
       : "memory");
 }
-__device__ __forceinline__ void t_gather4(uint32_t sdst, const CUtensorMap* tm, int col, int r0, int r1, int r2, int r3,
-                                          uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes"
-               " [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-               ::"r"(sdst), "l"(tm), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(bar) : "memory");
+// one row of `bytes` (multiple of 16) from global to shared memory through the TMA unit
+__device__ __forceinline__ void t_bulk_load(uint32_t sdst, const void* gsrc, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(sdst), "l"(gsrc), "r"(bytes), "r"(bar) : "memory");
 }
 __device__ __forceinline__ void t_bulk_store(void* gdst, uint32_t ssrc, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(ssrc), "r"(bytes) : "memory");
@@ -65,8 +61,7 @@ struct EmbedTmaParams {
 };
 
 template <typename IdT>
-__global__ void __launch_bounds__(TMA_WARPS * 32) embed_fm_fwd_tma_kernel(const EmbedTmaParams p,
-                                                                           const __grid_constant__ CUtensorMap tmap) {
+__global__ void __launch_bounds__(TMA_WARPS * 32) embed_fm_fwd_tma_kernel(const EmbedTmaParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) uint64_t bars[TMA_WARPS * TMA_NBUF];
   __shared__ int64_t s_off[32], s_rows[32];
@@ -83,34 +78,37 @@ __global__ void __launch_bounds__(TMA_WARPS * 32) embed_fm_fwd_tma_kernel(const 
   const int64_t ntiles = (p.B + TMA_EX - 1) / TMA_EX;
   const int64_t w0 = (int64_t)blockIdx.x * TMA_WARPS + warp, nw = (int64_t)gridDim.x * TMA_WARPS;
   const float bias = p.bias ? __ldg(p.bias) : 0.f;
-  const int oob = (int)p.total_rows;               // a row index outside the tensor: TMA fills zeros (OOV id -> zero row)
 
   auto issue = [&](int64_t tile, int buf) {
     unsigned char* tb = mybuf + buf * buf_bytes;
     const uint32_t bar = tsm_u32(&bars[warp * TMA_NBUF + buf]);
     const int64_t b0 = tile * TMA_EX;
     const int n = (int)min((int64_t)LK, (p.B - b0) * S);
-    if (lane == 0) t_mbar_expect_tx(bar, (uint32_t)(LK / 4) * 256u);
-    __syncwarp();
-    for (int m = lane; m < LK / 4; m += 32) {      // quad m = lookups 4m .. 4m+3 of the tile -> one gather4
-      int r[4];
-#pragma unroll
-      for (int x = 0; x < 4; ++x) {
-        const int j = m * 4 + x;
-        r[x] = oob;
-        float w = 0.f;
-        if (j < n) {
-          const int s = j % S;
-          const int64_t id = (int64_t)__ldg(ids + b0 * S + j);
-          if ((uint64_t)id < (uint64_t)s_rows[s]) {
-            r[x] = (int)(s_off[s] + id);
-            w = ldg_nc_na_f32(p.arena + (size_t)r[x] * p.row_stride + TMA_D);     // in-row first-order weight
-          }
+    int copies = 0;
+    for (int j = lane; j < LK; j += 32) {          // lookup j of the tile -> one bulk copy of its row (OOV id -> zero row)
+      float w = 0.f;
+      bool hit = false;
+      if (j < n) {
+        const int s = j % S;
+        const int64_t id = (int64_t)__ldg(ids + b0 * S + j);
+        if ((uint64_t)id < (uint64_t)s_rows[s]) {
+          const float* row = p.arena + (size_t)(s_off[s] + id) * p.row_stride;
+          w = ldg_nc_na_f32(row + TMA_D);                                         // in-row first-order weight
+          t_bulk_load(tsm_u32(tb + j * 64), row, 64u, bar);
+          hit = true;
+          ++copies;
         }
-        *reinterpret_cast<float*>(tb + tile_bytes + j * 4) = w;
       }
-      t_gather4(tsm_u32(tb + m * 256), &tmap, 0, r[0], r[1], r[2], r[3], bar);
+      if (!hit) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c) *reinterpret_cast<float4*>(tb + j * 64 + c * 16) = f4_zero();
+      }
+      *reinterpret_cast<float*>(tb + tile_bytes + j * 4) = w;
     }
+    // the bytes to expect are known only now; complete_tx of copies that already landed is accounted for when the
+    // expectation is posted, and the phase cannot complete before this one arrival
+    copies = (int)group_sum<32>((float)copies);
+    if (lane == 0) t_mbar_expect_tx(bar, (uint32_t)copies * 64u);
   };
 
   int it = 0;
@@ -123,6 +121,7 @@ __global__ void __launch_bounds__(TMA_WARPS * 32) embed_fm_fwd_tma_kernel(const 
     __syncwarp();
     if (nxt < ntiles) issue(nxt, (it + 1) % TMA_NBUF);
     t_mbar_wait(tsm_u32(&bars[warp * TMA_NBUF + buf]), (uint32_t)((it / TMA_NBUF) & 1));
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // zero rows were ordinary stores; the bulk store reads them
     __syncwarp();                                   // the first-order weights were ordinary shared-memory stores
     unsigned char* tb = mybuf + buf * buf_bytes;
     const int64_t b0 = tile * TMA_EX;
@@ -162,10 +161,6 @@ __global__ void __launch_bounds__(TMA_WARPS * 32) embed_fm_fwd_tma_kernel(const 
   if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-typedef CUresult (*EncodeTiledFnE)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 }  // namespace dr
 
 using namespace dr;
@@ -184,24 +179,6 @@ extern "C" int dr_embed_fm_fwd_tma(const float* arena, int64_t total_rows, const
   DR_REQUIRE(aligned16(arena) && (!out_stack || aligned16(out_stack)) && (!out_sum || aligned16(out_sum)), DR_EALIGN,
              "dr_embed_fm_fwd_tma: arena / out_stack / out_sum not 16-B aligned");
   if (B == 0) return DR_OK;
-  static EncodeTiledFnE enc = nullptr;
-  if (!enc) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
-    DR_REQUIRE(e == cudaSuccess && q == cudaDriverEntryPointSuccess && fn, DR_ENOTSUP,
-               "dr_embed_fm_fwd_tma: cuTensorMapEncodeTiled entry point not available");
-    enc = (EncodeTiledFnE)fn;
-  }
-  CUtensorMap tm;
-  cuuint64_t dims[2] = {(cuuint64_t)row_stride, (cuuint64_t)total_rows};
-  cuuint64_t strides[1] = {(cuuint64_t)row_stride * 4};
-  cuuint32_t box[2] = {(cuuint32_t)TMA_D, 1u};       // gather4: four 1-row boxes of D floats per instruction
-  cuuint32_t es[2] = {1u, 1u};
-  CUresult r = enc(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(arena), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  DR_REQUIRE(r == CUDA_SUCCESS, DR_EINVAL, "dr_embed_fm_fwd_tma: cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
   EmbedTmaParams p{};
   p.arena = arena; p.total_rows = total_rows; p.slot_offsets = slot_offsets; p.rows = rows; p.ids = ids; p.bias = bias;
   p.B = B; p.S = S; p.row_stride = row_stride; p.out_stack = out_stack; p.out_sum = out_sum; p.out_logit = out_logit;
@@ -213,17 +190,17 @@ extern "C" int dr_embed_fm_fwd_tma(const float* arena, int64_t total_rows, const
     DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 1;
     DR_CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, TMA_WARPS * 32, smem));
-    int64_t ctas = (int64_t)kNumSMs * (occ > 0 ? occ : 1);
+    int64_t ctas = (int64_t)num_sms() * (occ > 0 ? occ : 1);
     if (ctas * TMA_WARPS > ntiles) ctas = (ntiles + TMA_WARPS - 1) / TMA_WARPS;
-    k<<<(unsigned)ctas, TMA_WARPS * 32, smem, st>>>(p, tm);
+    k<<<(unsigned)ctas, TMA_WARPS * 32, smem, st>>>(p);
   } else {
     auto k = embed_fm_fwd_tma_kernel<int32_t>;
     DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 1;
     DR_CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, TMA_WARPS * 32, smem));
-    int64_t ctas = (int64_t)kNumSMs * (occ > 0 ? occ : 1);
+    int64_t ctas = (int64_t)num_sms() * (occ > 0 ? occ : 1);
     if (ctas * TMA_WARPS > ntiles) ctas = (ntiles + TMA_WARPS - 1) / TMA_WARPS;
-    k<<<(unsigned)ctas, TMA_WARPS * 32, smem, st>>>(p, tm);
+    k<<<(unsigned)ctas, TMA_WARPS * 32, smem, st>>>(p);
   }
   DR_CUDA_LAUNCH_CHECK("dr_embed_fm_fwd_tma");
   return DR_OK;

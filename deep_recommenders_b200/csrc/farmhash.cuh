@@ -1,5 +1,5 @@
 // FarmHash Fingerprint64 (== farmhashna::Hash64, google/farmhash, MIT licence), restated from the published
-// algorithm for both the host compiler and sm_100a.  TensorFlow's categorical_column_with_hash_bucket is
+// algorithm for both the host compiler and sm_90a.  TensorFlow's categorical_column_with_hash_bucket is
 // string_to_hash_bucket_fast(str(value), N) = Fingerprint64(bytes) mod N; FarmHash is a third-party dependency
 // of TensorFlow, not vendored in the reference (SURVEY.md 8c).  The same source serves
 //   * the device kernels of idpipe.cu (bit-exact ids are required: SURVEY 8a row E), and

@@ -70,7 +70,7 @@ static int launch_groups(K kern, int64_t B, int LPR, cudaStream_t st, const char
   const int G = 32 / LPR;
   const int64_t ntiles = (B + G - 1) / G;
   int64_t ctas = (ntiles + 7) / 8;
-  if (ctas > kNumSMs * 8) ctas = kNumSMs * 8;
+  if (ctas > num_sms() * 8) ctas = num_sms() * 8;
   kern<<<(int)ctas, 256, 0, st>>>(args...);
   DR_CUDA_LAUNCH_CHECK(name);
   return DR_OK;
@@ -139,7 +139,7 @@ extern "C" int dr_sgd_step(float* p, const float* g, int64_t n, float lr, void* 
   DR_REQUIRE(p && g && n >= 0, DR_EINVAL, "dr_sgd_step: bad arguments");
   if (n == 0) return DR_OK;
   int64_t ctas = (n + 255) / 256;
-  if (ctas > kNumSMs * 8) ctas = kNumSMs * 8;
+  if (ctas > num_sms() * 8) ctas = num_sms() * 8;
   sgd_kernel<<<(int)ctas, 256, 0, (cudaStream_t)stream>>>(p, g, n, lr);
   DR_CUDA_LAUNCH_CHECK("dr_sgd_step");
   return DR_OK;
@@ -151,7 +151,7 @@ extern "C" int dr_bce_logits_fwd_bwd(const float* z, const float* z_add, const f
   cudaStream_t st = (cudaStream_t)stream;
   DR_CUDA_CALL(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
   int64_t ctas = (B + 255) / 256;
-  if (ctas > kNumSMs * 4) ctas = kNumSMs * 4;
+  if (ctas > num_sms() * 4) ctas = num_sms() * 4;
   bce_kernel<<<(int)ctas, 256, 0, st>>>(z, z_add, y, B, 1.f / (float)B, prob_out, loss_out, gz);
   DR_CUDA_LAUNCH_CHECK("dr_bce_logits_fwd_bwd");
   return DR_OK;

@@ -4,7 +4,7 @@
 
 namespace dr {
 
-int g_tune_gemm_variant = 2;   // library default = the shipped core (tcgen05 3xTF32, split in kernel; needs no workspace); 0 = FFMA, 1 = pre-split planes
+int g_tune_gemm_variant = 2;   // library default = the shipped core (wgmma 3xTF32, split in kernel; needs no workspace); 0 = FFMA, 1 = pre-split planes
 int g_tune_gemm_splitk = 0;   // 0 = heuristic
 
 __device__ __forceinline__ float4 load4_guard(const float* __restrict__ base, int64_t r, int64_t c,

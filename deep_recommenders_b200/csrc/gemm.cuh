@@ -5,7 +5,7 @@
 // single-pass TF32/BF16 tensor-core product cannot meet (SURVEY.md section 7, hard part 2).
 // Variant 0 (this file) is an FFMA register-tiled kernel: 128x128x16 CTA tile, 8x8 per
 // thread, global->register->shared double buffering.  Variant 1 (gemm_tc.cu, when built) is
-// the tcgen05 3xTF32 path; both share the epilogues below.
+// the wgmma 3xTF32 path; both share the epilogues below.
 #pragma once
 #include "common.cuh"
 
@@ -37,10 +37,8 @@ struct GemmArgs {
   const int64_t* cand_ids;   // EPI_SCORES
   int64_t row0;              // EPI_SCORES: query row m of this call is global query m + row0 (its positive = candidate m + row0)
   int splitk;                // >= 1
-  int stages;                // 0 = default operand-ring depth; 2 = two stages (161 KB of shared memory instead of 225 KB, so
-                             // an HBM / NVLink-bound kernel on another stream can share the SMs with the persistent GEMM)
-  int share;                 // 1 = co-residency build of the tcgen05 kernel (registers capped, 16 KB less shared memory): the
-                             // HBM / NVLink-bound embedding update on another stream runs on the same SMs (gemm_tc.cu SHARE)
+  int stages;                // 0 = default depth of the raw operand ring (3); 2 = two stages (32 KB less shared memory)
+  int share;                 // 1 = the GEMM runs beside a memory-bound kernel on another stream: same as stages = 2
 };
 
 extern int g_tune_gemm_variant;
@@ -49,8 +47,8 @@ extern int g_tune_gemm_splitk;
 // C = A * B with the given storage flags; picks the tile shape from N. Returns DR_* / cudaError.
 int gemm_launch(const GemmArgs& a, bool transA, bool transB, cudaStream_t st);
 
-// tcgen05 3xTF32 variant (gemm_tc.cu): used when g_tune_gemm_variant == 1, the shape is aligned
-// and the registered workspace (dr_set_workspace) can hold the hi/lo operand planes.
+// wgmma 3xTF32 variants (gemm_tc.cu): g_tune_gemm_variant == 2 splits in the kernel; == 1 needs an aligned shape
+// and a registered workspace (dr_set_workspace) that can hold the hi/lo operand planes.
 bool gemm_tc_eligible(const GemmArgs& a, bool transA, bool transB);
 int gemm_tc_launch(const GemmArgs& a, bool transA, bool transB, cudaStream_t st);
 

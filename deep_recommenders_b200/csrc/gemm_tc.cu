@@ -1,28 +1,26 @@
-// Variant 1 of the fp32 GEMM core: tcgen05 (5th-gen tensor cores) with 3xTF32 split products.
+// The tensor-core form of the fp32 GEMM core: Hopper warpgroup MMA (wgmma) with 3xTF32 split products.
 //
 //   C[M,N] = epilogue( A @ B ),   A = Ah + Al, B = Bh + Bl   (Ah = fp32 with the low 13 mantissa
 //   bits cleared = exactly representable in TF32, Al = A - Ah exactly),
 //   A @ B ~= Al@Bh + Ah@Bl + Ah@Bh      (the dropped Al@Bl term is ~2^-22 relative)
 // which restores fp32-level accuracy (the parity bar is 1e-5 relative, out of reach of single-pass
-// TF32/BF16) at 3 tensor-core products per k-step.  The hi/lo planes are produced by
-// split_tf32_kernel into caller-provided workspace (dr_set_workspace) and streamed by TMA.
+// TF32/BF16) at 3 tensor-core products per k-step.
 //
-// Structure (one 128 x BN output tile per CTA, 192 threads, sm_100a only):
-//   warp 0      TMA producer: cp.async.bulk.tensor (SWIZZLE_128B boxes) into a 3-stage smem ring,
-//               completion on "full" mbarriers (expect_tx)
-//   warp 1      TMEM allocator + MMA issuer: one elected lane issues tcgen05.mma.kind::tf32
-//               (M=128, N=BN, K=8) x 4 k-steps x 3 products per stage, accumulator in TMEM;
-//               tcgen05.commit releases the smem stage ("empty" mbarrier) and finally signals
-//               the epilogue ("tmem_full")
-//   warps 2-5   epilogue: tcgen05.ld (32 lanes x 32 columns per warp), fused epilogue (gemm.cuh
-//               Epi modes), vectorised global stores / split-K atomics
-// Variant 2 (INSPLIT, g_tune_gemm_variant == 2): no pre-split planes at all.  TMA stages the RAW fp32 tiles of A and B
-// (half the L2 -> SM operand bytes of variant 1, and no split kernel / plane traffic in HBM), four extra warps split
-// every staged tile in shared memory -- hi overwrites the raw tile in place, lo goes to the slot next to it; the pass
-// is elementwise on 16-B chunks, so it is oblivious to the TMA swizzle -- then fence.proxy.async and arrive on a
-// per-stage "split" mbarrier the MMA issuer waits on instead of the TMA "full" barrier.
-// Operand majors: K-major (row-major [rows, K]) or MN-major ([K, rows] row-major) per operand;
-// both are canonical SWIZZLE_128B UMMA layouts (32 tf32 = 128 B per swizzle row).
+// Structure (one 128 x BN output tile per work item, persistent grid, 416 threads, sm_90a only):
+//   warps 0-7   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async.m64n{BN}k8.tf32 (both operands from
+//               shared memory, accumulator in registers) x 4 k-steps x 3 products per k-block, then the fused epilogue
+//               (gemm.cuh Epi modes) straight from the accumulator registers (float2 stores / split-K reductions)
+//   warps 8-11  splitters: turn every staged raw fp32 tile into its hi and lo planes in the layout wgmma reads
+//   warp 12     TMA producer: cp.async.bulk.tensor into the raw ring, completion on "full" mbarriers (expect_tx)
+// wgmma reads 32-bit operands from shared memory K-major only (canonical SWIZZLE_128B layout, 32 tf32 = 128 B per row).
+// An operand stored K-major (row-major [rows, K]) is staged by TMA in exactly that layout and split chunk by chunk; an
+// operand stored MN-major ([K, rows] row-major: the weight of a forward layer, both operands of a weight gradient) is
+// staged as stored and TRANSPOSED by the same splitter pass, which has to touch every element anyway.
+// Two rings decouple the stages: raw tiles (TMA -> splitters), planes (splitters -> wgmma), each with full / empty
+// mbarriers; fence.proxy.async orders the splitters' generic stores before wgmma's reads.
+// Variant 1 (g_tune_gemm_variant == 1, PRESPLIT): the hi/lo planes are produced K-major in caller-provided workspace
+// (dr_set_workspace) by split_tf32_kernel / split_tf32_transpose_kernel and TMA loads them straight into the plane
+// ring; variant 2 (the default) needs no workspace and no pre-pass.
 #include "gemm.cuh"
 #include <cuda.h>
 #include <float.h>
@@ -31,17 +29,17 @@
 namespace dr {
 
 // ---- workspace registered by the host (dr_set_workspace) ----------------------------------------
-int g_tune_gemm_bn = 0;   // 0 = auto, 128 or 256: tensor-core tile width
-int g_tune_tc_min_n = 32;   // 32 since round 2 (BN = 32 / 64 tiles of the in-kernel-split core: C2 step 0.849 -> 0.822 ms)
+int g_tune_gemm_bn = 0;     // 0 = auto; 32 / 64 / 128 cap the tile width (wider requests run 128: the accumulator of a
+                            // 64 x 256 warpgroup tile would take 128 registers per thread)
+int g_tune_tc_min_n = 32;   // outputs narrower than this stay on the FFMA kernel
 int g_tune_tc_l2_promo = 256;
-int g_tune_tc_mn = 1;     // 1 = feed MN-major operands as stored (SWIZZLE_128B_BASE32B); 0 = transpose them in the split pre-pass
 static void* g_ws_ptr = nullptr;
 static size_t g_ws_bytes = 0;
 
-// Plane cache (dr_gemm_plane_cache): inside a train step every tensor is split into its TF32 hi/lo
-// planes ONCE and the planes are shared by all the GEMMs that read it (x: forward and dW; gz: dX and
+// Plane cache (dr_gemm_plane_cache, variant 1): inside a train step every tensor is split into its TF32 hi/lo
+// planes ONCE per layout and the planes are shared by all the GEMMs that read it (x: forward and dW; gz: dX and
 // dW; W: forward and dX).  Off by default: without it every GEMM call splits its own operands.
-struct PlaneEntry { const float* src; size_t elems; float* hi; float* lo; };
+struct PlaneEntry { const float* src; size_t elems; bool transposed; float* hi; float* lo; int64_t pitch; };
 static PlaneEntry g_planes[64];
 static int g_nplanes = 0;
 static bool g_cache_on = false;
@@ -49,9 +47,11 @@ static size_t g_bump = 0;     // floats used at the front of the workspace
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 32;          // 32 tf32 = 128 bytes = one SWIZZLE_128B row
-constexpr int TC_THREADS = 192;
-constexpr int TC_SPLIT_WARPS = 4;                              // variant 2: warps 6..9 split the staged fp32 tiles
-constexpr int TC_THREADS_INSPLIT = TC_THREADS + 32 * TC_SPLIT_WARPS;
+constexpr int TC_CONSUMERS = 256;  // two warpgroups
+constexpr int TC_SPLITTERS = 128;
+constexpr int TC_THREADS = TC_CONSUMERS + TC_SPLITTERS + 32;
+constexpr int TC_PLANE_STAGES = 2;
+constexpr int TC_MAX_RAW_STAGES = 4;
 
 // ---- small PTX wrappers ----------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -61,6 +61,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
@@ -73,92 +76,76 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       ::"r"(smem_u32(bar)), "r"(parity)
       : "memory");
 }
-// ---- per-role wait-time profile (diagnostic instantiation only: template flag PROF, knob gemm_prof) ------------------
-// slots: 0 producer waits for a free stage, 1 splitter waits for TMA data, 2 splitter splits, 3 MMA waits for operands,
-// 4 MMA waits for a free accumulator, 5 epilogue waits for the accumulator, 6 epilogue body, 7 kernel span (CTA 0..n
-// summed), 8 CTAs, 9 k-blocks issued.  Cycles of one representative thread per role, summed over CTAs.
-__device__ unsigned long long g_tc_prof[16];
-
-template <bool PROF>
-__device__ __forceinline__ void mbar_wait_t(uint64_t* bar, uint32_t parity, unsigned long long& acc) {
-  if (PROF) {
-    const long long t0 = clock64();
-    mbar_wait(bar, parity);
-    acc += (unsigned long long)(clock64() - t0);
-  } else {
-    mbar_wait(bar, parity);
-  }
-}
-
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// Epilogue output path: a [32 rows x 32 floats] slab staged in shared memory (SWIZZLE_128B layout) leaves as ONE TMA
-// store (or, for split-K partial sums, one TMA reduce-add: the fp32 additions happen at the L2, no per-element atomics).
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(tm), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* tm, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(tm), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-constexpr int TC_EPI_STAGING = 4 * 2 * 4096;   // 4 epilogue warps x 2 slabs x (32 rows x 128 B)
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// UMMA shared-memory descriptor (cute::UMMA::SmemDescriptor bit layout), SWIZZLE_128B, version 1.
-// layout_type: 2 = SWIZZLE_128B (K-major operands), 1 = SWIZZLE_128B_BASE32B (the only layout UMMA
-// accepts for MN-major 32-bit operands; TMA counterpart CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type = 2) {
+// wgmma shared-memory matrix descriptor of a K-major SWIZZLE_128B operand: rows of 128 B, 8-row swizzle groups 1024 B
+// apart (stride byte offset); the leading byte offset is not used by swizzled K-major layouts.  The tile base is
+// 1024-B aligned, so the base-offset field stays 0; a k-step of 8 tf32 advances the start address by 32 B.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;   // descriptor version (Blackwell)
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024u >> 4) << 32;
+  d |= (uint64_t)1 << 62;   // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): TF32 x TF32 -> F32, dense.
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4)                       // c_format = F32
-         | (2u << 7) | (2u << 10)        // a_format = b_format = TF32
-         | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16)
-         | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// D[64 x N] += A[64 x 8] * B[8 x N], tf32 operands from shared memory, fp32 accumulator fragment in registers
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t da, uint64_t db);
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(1));
 }
 
 __global__ void __launch_bounds__(256) split_tf32_kernel(const float* __restrict__ x, int64_t n4,
@@ -234,162 +221,35 @@ __device__ __forceinline__ float epi_scalar_tc(const GemmArgs& a, float acc, int
   }
 }
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 
-__device__ int g_store_hi = 0;      // device copy of the tc_store_hi knob (dr_tune_set)
-// Variant 2 splitter: elementwise over 16-B chunks of one staged tile (BYTES multiple of 16 * NT * 4 or smaller tail).
-template <int BYTES, int NT>
-__device__ __forceinline__ void split_tile_inplace(uint8_t* hi, uint8_t* lo, int tid) {
-  constexpr int CHUNKS = BYTES / 16;
-  constexpr int PER = (CHUNKS + NT - 1) / NT;
-#pragma unroll
-  for (int i0 = 0; i0 < PER; i0 += 4) {
-    float4 v[4];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int c = (i0 + u) * NT + tid;
-      if (i0 + u < PER && c < CHUNKS) v[u] = *reinterpret_cast<const float4*>(hi + (size_t)c * 16);
+// Splitter pass over one staged operand tile of ROWS x 32 floats: hi = top 19 bits, lo = v - hi (exact), both written in
+// the K-major SWIZZLE_128B layout (16-B chunk c of row r at r * 128 + ((c ^ (r & 7)) << 4)).
+//   K-major raw tile: TMA staged it in that very layout, so the pass is elementwise on 16-B chunks;
+//   MN-major raw tile: [32 k-rows][ROWS] as stored; a thread gathers 4 consecutive k of one row (the lanes of a warp read
+//   32 consecutive floats of one k-row: conflict free) and writes one chunk (8 lanes cover all 32 banks: conflict free).
+template <int ROWS, bool MN>
+__device__ __forceinline__ void split_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int tid) {
+  constexpr int CHUNKS = ROWS * 8;
+#pragma unroll 4
+  for (int idx = tid; idx < CHUNKS; idx += TC_SPLITTERS) {
+    float4 v;
+    uint32_t off;
+    if (!MN) {
+      off = (uint32_t)idx * 16u;
+      v = *reinterpret_cast<const float4*>(raw + off);
+    } else {
+      const int r = idx % ROWS, c = idx / ROWS;
+      const float* src = reinterpret_cast<const float*>(raw) + (4 * c) * ROWS + r;
+      v = make_float4(src[0], src[ROWS], src[2 * ROWS], src[3 * ROWS]);
+      off = (uint32_t)r * 128u + (uint32_t)((c ^ (r & 7)) << 4);
     }
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int c = (i0 + u) * NT + tid;
-      if (i0 + u < PER && c < CHUNKS) {
-        float4 h, l;
-        h.x = __uint_as_float(__float_as_uint(v[u].x) & 0xFFFFE000u); l.x = v[u].x - h.x;
-        h.y = __uint_as_float(__float_as_uint(v[u].y) & 0xFFFFE000u); l.y = v[u].y - h.y;
-        h.z = __uint_as_float(__float_as_uint(v[u].z) & 0xFFFFE000u); l.z = v[u].z - h.z;
-        h.w = __uint_as_float(__float_as_uint(v[u].w) & 0xFFFFE000u); l.w = v[u].w - h.w;
-        // The hi plane is NOT written back: kind::tf32 reads the top 19 bits of a 32-bit operand and ignores the low 13
-        // mantissa bits, i.e. the raw fp32 tile already IS the hi plane (bits & 0xFFFFE000) as far as the tensor core is
-        // concerned.  Only lo = v - hi is produced: one shared-memory store per chunk instead of two (knob tc_store_hi=1
-        // restores the explicit store; the 1e-5 parity tests would catch a core that rounded instead of truncating).
-        if (g_store_hi) *reinterpret_cast<float4*>(hi + (size_t)c * 16) = h;
-        *reinterpret_cast<float4*>(lo + (size_t)c * 16) = l;
-      }
-    }
-  }
-}
-
-// Epilogue of ONE work item for one epilogue warp (TMEM lane quarter q): tcgen05.ld 32 x 32 slabs of the accumulator at
-// `tmem_acc`, fused epilogue, output through the swizzled staging buffer + TMA store / reduce-add (or register stores).
-// Shared by the single-CTA kernel and the CTA-pair kernel.  mw = first output row of this warp's quarter.
-template <int BN, bool SHARE>
-__device__ __forceinline__ void tc_epilogue_item(const GemmArgs& a, const CUtensorMap* tmC, const int tma_out,
-                                                 const uint32_t tmem_acc, const int q, const int lane, const int64_t mw,
-                                                 const int64_t n0, uint8_t* stg, uint32_t& slab, const bool vec_ok) {
-  const int64_t m = mw + lane;
-#pragma unroll 1
-  for (int c = 0; c < BN / 32; ++c) {
-    uint32_t r[32];
-    tmem_ld_32x32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-    const int64_t nb = n0 + c * 32;
-    if (tma_out) {
-      if (mw < a.M && nb < a.N) {            // warp-uniform
-        uint8_t* sb = SHARE ? stg : stg + (slab & 1u) * 4096;
-        if (lane == 0) {                            // the store issued from this buffer two slabs ago (SHARE: the
-          if (SHARE) bulk_wait_group_read<0>();     // previous one) has read it
-          else bulk_wait_group_read<1>();
-        }
-        __syncwarp();
-        const bool row_ok = m < a.M;
-        float o[32];
-        if (a.epi == EPI_STORE || a.epi == EPI_ATOMIC) {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) o[jj] = __uint_as_float(r[jj]);
-        } else if (a.epi == EPI_BIAS_ACT) {
-          // one coalesced bias load per slab (lane l holds bias[nb + l]), broadcast by shuffles; the activation
-          // switch is hoisted out of the element loop
-          const float bl = (a.bias && nb + lane < a.N) ? __ldg(a.bias + nb + lane) : 0.f;
-          if (a.act == DR_ACT_RELU) {
-#pragma unroll
-            for (int jj = 0; jj < 32; ++jj)
-              o[jj] = fmaxf(__uint_as_float(r[jj]) + __shfl_sync(0xffffffffu, bl, jj), 0.f);
-          } else if (a.act == DR_ACT_NONE) {
-#pragma unroll
-            for (int jj = 0; jj < 32; ++jj) o[jj] = __uint_as_float(r[jj]) + __shfl_sync(0xffffffffu, bl, jj);
-          } else {
-#pragma unroll
-            for (int jj = 0; jj < 32; ++jj)
-              o[jj] = act_apply(__uint_as_float(r[jj]) + __shfl_sync(0xffffffffu, bl, jj), a.act);
-          }
-        } else if (a.epi == EPI_SCORES) {
-          // v = acc - log p[n] + dup(m, n) * MIN_FLOAT (sbcnm.py:78-86, 52-75): lane l holds log p and the id of column
-          // nb + l (one coalesced load each per slab), broadcast by shuffles; the thread's own row id is loaded once
-          const int64_t mg = m + a.row0;
-          const bool col_ok = nb + lane < a.N;
-          const float lpl = (a.bias && col_ok) ? logf(__ldg(a.bias + nb + lane)) : 0.f;
-          const long long idl = (a.cand_ids && col_ok) ? (long long)__ldg(a.cand_ids + nb + lane) : -1ll;
-          const long long idm = (a.cand_ids && row_ok && mg < a.N) ? (long long)__ldg(a.cand_ids + mg) : -2ll;
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) {
-            float v = __uint_as_float(r[jj]) - __shfl_sync(0xffffffffu, lpl, jj);
-            if (a.cand_ids) {
-              const long long idj = __shfl_sync(0xffffffffu, idl, jj);
-              if (mg != nb + jj && idj == idm) v += (-FLT_MAX / 100.0f);
-            }
-            o[jj] = v;
-          }
-        } else if (a.epi == EPI_ACTGRAD && a.act == DR_ACT_RELU && nb + 31 < a.N && mw + 31 < a.M) {
-          // relu'(y) = [y > 0].  The y slab is fetched COALESCED (each load instruction reads 4 whole 128-B rows) into
-          // the staging buffer in the same swizzled layout, then every thread reads its own row from shared memory
-          // (a thread reading its row straight from global memory costs 32 scattered 16-B requests per instruction).
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = i * 4 + (lane >> 3), ch = lane & 7;
-            const float4 yv = __ldg(reinterpret_cast<const float4*>(a.aux0 + (mw + rr) * a.ldc + nb + ch * 4));
-            *reinterpret_cast<float4*>(sb + rr * 128 + ((ch ^ (rr & 7)) << 4)) = yv;
-          }
-          __syncwarp();
-#pragma unroll
-          for (int ch = 0; ch < 8; ++ch) {
-            const float4 yv = *reinterpret_cast<const float4*>(sb + lane * 128 + ((ch ^ (lane & 7)) << 4));
-            o[4 * ch + 0] = yv.x > 0.f ? __uint_as_float(r[4 * ch + 0]) : 0.f;
-            o[4 * ch + 1] = yv.y > 0.f ? __uint_as_float(r[4 * ch + 1]) : 0.f;
-            o[4 * ch + 2] = yv.z > 0.f ? __uint_as_float(r[4 * ch + 2]) : 0.f;
-            o[4 * ch + 3] = yv.w > 0.f ? __uint_as_float(r[4 * ch + 3]) : 0.f;
-          }
-          __syncwarp();     // every lane has read its row before anyone overwrites the buffer with the output
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj)
-            o[jj] = (row_ok && nb + jj < a.N) ? epi_scalar_tc(a, __uint_as_float(r[jj]), m, nb + jj) : 0.f;
-        }
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch)
-          *reinterpret_cast<float4*>(sb + lane * 128 + ((ch ^ (lane & 7)) << 4)) =
-              make_float4(o[4 * ch], o[4 * ch + 1], o[4 * ch + 2], o[4 * ch + 3]);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-          if (a.epi == EPI_ATOMIC) tma_reduce_add_2d(tmC, sb, (int)nb, (int)mw);
-          else tma_store_2d(tmC, sb, (int)nb, (int)mw);
-          bulk_commit_group();
-        }
-        ++slab;
-      }
-    } else if (m < a.M && nb < a.N) {
-      if (a.epi == EPI_ATOMIC) {
-#pragma unroll
-        for (int jj = 0; jj < 32; ++jj)
-          if (nb + jj < a.N) red_add_f32(a.C + m * a.ldc + nb + jj, __uint_as_float(r[jj]));
-      } else if (vec_ok && nb + 31 < a.N) {
-#pragma unroll
-        for (int jj = 0; jj < 32; jj += 4) {
-          float4 o;
-          o.x = epi_scalar_tc(a, __uint_as_float(r[jj + 0]), m, nb + jj + 0);
-          o.y = epi_scalar_tc(a, __uint_as_float(r[jj + 1]), m, nb + jj + 1);
-          o.z = epi_scalar_tc(a, __uint_as_float(r[jj + 2]), m, nb + jj + 2);
-          o.w = epi_scalar_tc(a, __uint_as_float(r[jj + 3]), m, nb + jj + 3);
-          *reinterpret_cast<float4*>(a.C + m * a.ldc + nb + jj) = o;
-        }
-      } else {
-#pragma unroll
-        for (int jj = 0; jj < 32; ++jj)
-          if (nb + jj < a.N) a.C[m * a.ldc + nb + jj] = epi_scalar_tc(a, __uint_as_float(r[jj]), m, nb + jj);
-      }
-    }
+    float4 h, l;
+    h.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); l.x = v.x - h.x;
+    h.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u); l.y = v.y - h.y;
+    h.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); l.z = v.z - h.z;
+    h.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u); l.w = v.w - h.w;
+    *reinterpret_cast<float4*>(hi + off) = h;
+    *reinterpret_cast<float4*>(lo + off) = l;
   }
 }
 
@@ -412,421 +272,159 @@ __device__ __forceinline__ TcItem tc_decode(int64_t item, int64_t n_tiles, int64
   return t;
 }
 
-// Persistent, warp-specialised: the accumulator is double buffered in TMEM (2 x BN columns) so the
-// epilogue of item j overlaps the TMA/MMA main loop of item j+1.
-// SHARE (per-call GemmArgs::share, weight-gradient GEMMs that run beside the HBM-bound embedding update): the same kernel
-// built to leave room on the SM for a second resident kernel -- registers capped at 96 / thread (30.7 K of the 64 K file
-// instead of 53.8 K) and ONE epilogue staging slab per warp (16 KB less shared memory), so that CTAs of the embedding
-// backward (58 registers, 1 KB of shared memory) run on the same SMs while the GEMM's main loop is shared-memory bound.
-template <int BN, int STAGES, bool A_MN, bool B_MN, bool INSPLIT = false, bool PROF = false, bool SHARE = false>
-__global__ void __launch_bounds__(INSPLIT ? TC_THREADS_INSPLIT : TC_THREADS, SHARE ? 2 : 1)
+// Fused epilogue of one warpgroup's 64 x BN accumulator.  Fragment layout of wgmma's D: warp w of the warpgroup owns rows
+// 16 w .. 16 w + 15; d[4 j + {0, 1}] are columns 8 j + 2 (lane % 4) + {0, 1} of row lane / 4, d[4 j + {2, 3}] the same
+// columns of row lane / 4 + 8.  Four lanes write one whole 32-B sector of a row.
+template <int BN>
+__device__ __forceinline__ void tc_epilogue(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw, const int64_t n0,
+                                            const int lane, const bool vec_ok) {
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int64_t m = mw + (lane >> 2) + 8 * half;
+    if (m >= a.M) continue;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int64_t n = n0 + 8 * j + 2 * (lane & 3);
+      if (n >= a.N) continue;
+      const float v0 = d[4 * j + 2 * half], v1 = d[4 * j + 2 * half + 1];
+      float* c = a.C + m * a.ldc + n;
+      if (a.epi == EPI_ATOMIC) {
+        red_add_f32(c, v0);
+        if (n + 1 < a.N) red_add_f32(c + 1, v1);
+      } else if (vec_ok && n + 1 < a.N) {
+        *reinterpret_cast<float2*>(c) = make_float2(epi_scalar_tc(a, v0, m, n), epi_scalar_tc(a, v1, m, n + 1));
+      } else {
+        c[0] = epi_scalar_tc(a, v0, m, n);
+        if (n + 1 < a.N) c[1] = epi_scalar_tc(a, v1, m, n + 1);
+      }
+    }
+  }
+}
+
+// Persistent, warp-specialised.  `raw_stages` (run-time: 2 or 3) is the depth of the raw ring; the plane ring is two deep.
+// Shared memory: planes 2 x [Ah | Al | Bh | Bl], then (variant 2) raw_stages x [A raw | B raw].
+template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
+// Registers are allocated to warps in groups of four, so 13 warps count as 16: 65536 / 512 = 128 registers per thread.
+// The BN = 128 instantiations hold 64 accumulators and spill one 4-byte value (8 bytes of stack) at that cap.
+__global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-               const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-               const __grid_constant__ CUtensorMap tmC, const int tma_out,
-               const GemmArgs a, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
+               const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const GemmArgs a,
+               const int raw_stages, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
                const int64_t total_items) {
   constexpr int A_TILE = TC_BM * TC_BK * 4;   // 16 KB
   constexpr int B_TILE = BN * TC_BK * 4;
-  constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;
+  constexpr int PLANE_STAGE = 2 * A_TILE + 2 * B_TILE;
+  constexpr int RAW_STAGE = A_TILE + B_TILE;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], split_bar[STAGES], tmem_full_bar[2],
-      tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_slot;
+  uint8_t* planes = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* raws = planes + TC_PLANE_STAGES * PLANE_STAGE;
+  __shared__ __align__(8) uint64_t raw_full[TC_MAX_RAW_STAGES], raw_empty[TC_MAX_RAW_STAGES],
+      pl_full[TC_PLANE_STAGES], pl_empty[TC_PLANE_STAGES];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t kblocks = (a.K + TC_BK - 1) / TC_BK;
-  const long long prof_t0 = PROF ? clock64() : 0;
-  unsigned long long pw0 = 0, pw1 = 0, pw2 = 0;   // per-thread wait / work accumulators (PROF only)
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAh) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAl) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBh) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBl) : "memory");
-    if (tma_out) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmC) : "memory");
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-      mbar_init(&split_bar[s], 32 * TC_SPLIT_WARPS);   // every splitter thread arrives
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < TC_MAX_RAW_STAGES; ++s) {
+      mbar_init(&raw_full[s], 1);                    // the producer's expect_tx arrival
+      mbar_init(&raw_empty[s], TC_SPLITTERS);        // every splitter thread arrives
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full_bar[s], 1);
-      mbar_init(&tmem_empty_bar[s], 128);   // every epilogue thread arrives
+    for (int s = 0; s < TC_PLANE_STAGES; ++s) {
+      mbar_init(&pl_full[s], PRESPLIT ? 1 : TC_SPLITTERS);
+      mbar_init(&pl_empty[s], TC_CONSUMERS);         // every consumer thread arrives
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {   // TMEM: 2 accumulator stages x BN fp32 columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)),
-                 "r"((uint32_t)(2 * BN))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
 
-  if (warp == 0) {
+  if (warp == (TC_CONSUMERS + TC_SPLITTERS) / 32) {
     if (lane == 0) {
       // ===== TMA producer =====
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAh) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBh) : "memory");
       uint32_t it = 0;
       for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
         const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
         for (int i = 0; i < t.nkb; ++i, ++it) {
-          const int s = (int)(it % STAGES);
-          const uint32_t ph = (it / STAGES) & 1u;
-          mbar_wait_t<PROF>(&empty_bar[s], ph ^ 1u, pw0);
-          // INSPLIT: only the raw fp32 tiles travel (tmAh / tmBh map the source tensors); they land in the hi slots
-          mbar_expect_tx(&full_bar[s], (uint32_t)(INSPLIT ? (A_TILE + B_TILE) : STAGE));
-          uint8_t* st = smem + (size_t)s * STAGE;
           const int k = (t.kb0 + i) * TC_BK;
-          if (!A_MN) {
-            tma_load_2d(st, &tmAh, &full_bar[s], k, (int)t.m0);
-            if (!INSPLIT) tma_load_2d(st + A_TILE, &tmAl, &full_bar[s], k, (int)t.m0);
-          } else {     // MN-major: one [32 k-rows x 32 floats] box per 32-wide MN atom
-#pragma unroll
-            for (int jj = 0; jj < TC_BM / 32; ++jj) {
-              tma_load_2d(st + jj * 4096, &tmAh, &full_bar[s], (int)t.m0 + jj * 32, k);
-              if (!INSPLIT) tma_load_2d(st + A_TILE + jj * 4096, &tmAl, &full_bar[s], (int)t.m0 + jj * 32, k);
-            }
-          }
-          if (!B_MN) {
-            tma_load_2d(st + 2 * A_TILE, &tmBh, &full_bar[s], k, (int)t.n0);
-            if (!INSPLIT) tma_load_2d(st + 2 * A_TILE + B_TILE, &tmBl, &full_bar[s], k, (int)t.n0);
+          if (PRESPLIT) {      // K-major planes from the workspace straight into the plane ring
+            const int s = (int)(it % TC_PLANE_STAGES);
+            mbar_wait(&pl_empty[s], ((it / TC_PLANE_STAGES) & 1u) ^ 1u);
+            mbar_expect_tx(&pl_full[s], (uint32_t)PLANE_STAGE);
+            uint8_t* st = planes + (size_t)s * PLANE_STAGE;
+            tma_load_2d(st, &tmAh, &pl_full[s], k, (int)t.m0);
+            tma_load_2d(st + A_TILE, &tmAl, &pl_full[s], k, (int)t.m0);
+            tma_load_2d(st + 2 * A_TILE, &tmBh, &pl_full[s], k, (int)t.n0);
+            tma_load_2d(st + 2 * A_TILE + B_TILE, &tmBl, &pl_full[s], k, (int)t.n0);
           } else {
-#pragma unroll
-            for (int jj = 0; jj < BN / 32; ++jj) {
-              tma_load_2d(st + 2 * A_TILE + jj * 4096, &tmBh, &full_bar[s], (int)t.n0 + jj * 32, k);
-              if (!INSPLIT) tma_load_2d(st + 2 * A_TILE + B_TILE + jj * 4096, &tmBl, &full_bar[s], (int)t.n0 + jj * 32, k);
-            }
+            const int s = (int)(it % (uint32_t)raw_stages);
+            mbar_wait(&raw_empty[s], ((it / (uint32_t)raw_stages) & 1u) ^ 1u);
+            mbar_expect_tx(&raw_full[s], (uint32_t)RAW_STAGE);
+            uint8_t* st = raws + (size_t)s * RAW_STAGE;
+            if (!A_MN) tma_load_2d(st, &tmAh, &raw_full[s], k, (int)t.m0);
+            else tma_load_2d(st, &tmAh, &raw_full[s], (int)t.m0, k);
+            if (!B_MN) tma_load_2d(st + A_TILE, &tmBh, &raw_full[s], k, (int)t.n0);
+            else tma_load_2d(st + A_TILE, &tmBh, &raw_full[s], (int)t.n0, k);
           }
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc = make_idesc(TC_BM, BN, A_MN, B_MN);
-      uint32_t it = 0, j = 0;
-      for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x, ++j) {
+  } else if (threadIdx.x >= TC_CONSUMERS) {
+    // ===== splitter warps: raw fp32 tile -> TF32 hi / lo planes, K-major =====
+    if (!PRESPLIT) {
+      const int tid = (int)threadIdx.x - TC_CONSUMERS;
+      uint32_t it = 0;
+      for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
         const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
-        const uint32_t as = j & 1u, aph = (j >> 1) & 1u;
-        mbar_wait_t<PROF>(&tmem_empty_bar[as], aph ^ 1u, pw1);      // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * (uint32_t)BN;
         for (int i = 0; i < t.nkb; ++i, ++it) {
-          const int s = (int)(it % STAGES);
-          const uint32_t ph = (it / STAGES) & 1u;
-          mbar_wait_t<PROF>(INSPLIT ? &split_bar[s] : &full_bar[s], ph, pw0);
-          if (PROF) ++pw2;
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)s * STAGE);
-          const uint32_t sb = sa + 2 * A_TILE;
-#pragma unroll
-          for (int k = 0; k < TC_BK / 8; ++k) {
-            // K-major SWIZZLE_128B: one k-step = 8 tf32 = 32 B inside the 128-B row; 8-row groups 1024 B apart
-            // MN-major SWIZZLE_128B_BASE32B: one k-step = 8 k-rows = 1024 B (two 4-row swizzle groups 512 B
-            // apart), 32-wide MN atoms 4096 B apart.
-            const uint32_t a_off = A_MN ? (uint32_t)k * 1024u : (uint32_t)k * 32u;
-            const uint32_t b_off = B_MN ? (uint32_t)k * 1024u : (uint32_t)k * 32u;
-            const uint32_t a_lbo = A_MN ? 4096u : 16u, a_sbo = A_MN ? 512u : 1024u, a_lt = A_MN ? 1u : 2u;
-            const uint32_t b_lbo = B_MN ? 4096u : 16u, b_sbo = B_MN ? 512u : 1024u, b_lt = B_MN ? 1u : 2u;
-            const uint64_t dAh = make_smem_desc(sa + a_off, a_lbo, a_sbo, a_lt);
-            const uint64_t dAl = make_smem_desc(sa + A_TILE + a_off, a_lbo, a_sbo, a_lt);
-            const uint64_t dBh = make_smem_desc(sb + b_off, b_lbo, b_sbo, b_lt);
-            const uint64_t dBl = make_smem_desc(sb + B_TILE + b_off, b_lbo, b_sbo, b_lt);
-            const uint32_t acc0 = (i > 0 || k > 0) ? 1u : 0u;
-            tc_mma_tf32(d_tmem, dAl, dBh, idesc, acc0);   // small cross terms first
-            tc_mma_tf32(d_tmem, dAh, dBl, idesc, 1u);
-            tc_mma_tf32(d_tmem, dAh, dBh, idesc, 1u);
-          }
-          tc_commit(&empty_bar[s]);          // smem stage reusable once these MMAs retire
+          const int s = (int)(it % (uint32_t)raw_stages), p = (int)(it % TC_PLANE_STAGES);
+          mbar_wait(&raw_full[s], (it / (uint32_t)raw_stages) & 1u);        // TMA bytes of this stage have landed
+          mbar_wait(&pl_empty[p], ((it / TC_PLANE_STAGES) & 1u) ^ 1u);      // wgmma has finished reading the planes
+          const uint8_t* rw = raws + (size_t)s * RAW_STAGE;
+          uint8_t* pl = planes + (size_t)p * PLANE_STAGE;
+          split_tile<TC_BM, A_MN>(rw, pl, pl + A_TILE, tid);
+          split_tile<BN, B_MN>(rw + A_TILE, pl + 2 * A_TILE, pl + 2 * A_TILE + B_TILE, tid);
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to wgmma
+          mbar_arrive(&pl_full[p]);
+          mbar_arrive(&raw_empty[s]);
         }
-        tc_commit(&tmem_full_bar[as]);       // accumulator of this item complete
       }
     }
-    __syncwarp();
-  } else if (INSPLIT && warp >= 6) {
-    // ===== splitter warps 6..9 (variant 2): raw fp32 tile -> TF32 hi (in place) + lo (next slot) =====
-    const int tid = (int)threadIdx.x - TC_THREADS;
-    constexpr int NSPLIT = 32 * TC_SPLIT_WARPS;
+  } else {
+    // ===== consumer warpgroups: rows [64 wg, 64 wg + 64) of the tile =====
+    const int wg = warp >> 2;
+    const bool vec_ok = ((a.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 7u) == 0);
     uint32_t it = 0;
     for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
       const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
+      float d[BN / 2];
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
       for (int i = 0; i < t.nkb; ++i, ++it) {
-        const int s = (int)(it % STAGES);
-        const uint32_t ph = (it / STAGES) & 1u;
-        mbar_wait_t<PROF>(&full_bar[s], ph, pw0);   // TMA bytes of this stage have landed (visible to generic loads)
-        const long long ts0 = PROF ? clock64() : 0;
-        uint8_t* st = smem + (size_t)s * STAGE;
-        split_tile_inplace<A_TILE, NSPLIT>(st, st + A_TILE, tid);
-        split_tile_inplace<B_TILE, NSPLIT>(st + 2 * A_TILE, st + 2 * A_TILE + B_TILE, tid);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to tcgen05.mma
-        mbar_arrive(&split_bar[s]);
-        if (PROF) pw1 += (unsigned long long)(clock64() - ts0);
-      }
-    }
-  } else {
-    // ===== epilogue warps 2..5: TMEM lane quarter = warp % 4 =====
-    // tcgen05.ld hands thread t row t of a 32 x 32 slab.  Stored straight from registers that is 32 rows x 16 B per
-    // instruction (every store touches 32 different lines; round 1 measured the kernel EPILOGUE-bound because of it).
-    // Instead the slab is written to shared memory in the TMA SWIZZLE_128B layout (16-B chunk c of row t at
-    // t*128 + ((c ^ (t & 7)) << 4): conflict-free for a row-per-thread writer) and one elected lane issues a TMA store
-    // -- or a TMA reduce-add for split-K partial sums -- which also clips the M / N edges.
-    const int q = warp & 3;
-    const bool vec_ok = ((a.ldc & 3) == 0) && aligned16(a.C);
-    uint8_t* stg = smem + (size_t)STAGES * STAGE + (size_t)q * (SHARE ? 4096 : 8192);
-    uint32_t j = 0, slab = 0;
-    for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x, ++j) {
-      const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
-      const uint32_t as = j & 1u, aph = (j >> 1) & 1u;
-      mbar_wait_t<PROF>(&tmem_full_bar[as], aph, pw0);
-      const long long te0 = PROF ? clock64() : 0;
-      tc_fence_after();
-      tc_epilogue_item<BN, SHARE>(a, &tmC, tma_out, tmem_base + as * (uint32_t)BN, q, lane, t.m0 + q * 32, t.n0, stg, slab, vec_ok);
-      tc_fence_before();
-      mbar_arrive(&tmem_empty_bar[as]);      // this thread is done reading accumulator stage `as`
-      if (PROF) pw1 += (unsigned long long)(clock64() - te0);
-    }
-    if (tma_out && lane == 0) bulk_wait_group_all();   // every TMA store / reduce of this warp has completed
-  }
-  if (PROF) {   // one representative thread per role adds its counters
-    if (warp == 0 && lane == 0) {
-      atomicAdd(&g_tc_prof[0], pw0);
-      atomicAdd(&g_tc_prof[7], (unsigned long long)(clock64() - prof_t0));
-      atomicAdd(&g_tc_prof[8], 1ull);
-    }
-    if (warp == 1 && lane == 0) { atomicAdd(&g_tc_prof[3], pw0); atomicAdd(&g_tc_prof[4], pw1); atomicAdd(&g_tc_prof[9], pw2); }
-    if (threadIdx.x == 64) { atomicAdd(&g_tc_prof[5], pw0); atomicAdd(&g_tc_prof[6], pw1); }
-    if (INSPLIT && threadIdx.x == TC_THREADS) { atomicAdd(&g_tc_prof[1], pw0); atomicAdd(&g_tc_prof[2], pw1); }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN))
-                 : "memory");
-  }
-}
-
-
-// ======================================================================================================================
-// CTA-pair variant (tcgen05 cta_group::2): two SMs of one TPC work on one 256 x BN output tile.
-//
-// Why: the single-CTA in-kernel-split main loop is SHARED-MEMORY-BANDWIDTH bound -- per 128 x 256 x 32 k-block an SM moves
-// 288 KB through its shared memory (48 KB TMA in, 48 + 48 KB split read / lo write, 144 KB tensor-core operand reads)
-// = 2250 cycles at 128 B / cycle against 1536 cycles of MMA time (profiles/gemm_prof_*).  In a CTA pair each CTA stages
-// its own 128 rows of A and only HALF of the B tile (BN / 2 columns); one `tcgen05.mma.cta_group::2` (M = 256) issued by
-// the leader CTA feeds both SMs' tensor cores, each SM reading its half of B once for both.  Per SM and k-block:
-// 32 KB TMA in, 32 + 32 KB split, 96 KB operand reads = 192 KB = 1500 cycles < the 1536 cycles of its 12 MMAs.
-//
-// Roles per CTA are those of gemm_tc_kernel<INSPLIT> (TMA producer, MMA issuer, 4 epilogue warps, 4 splitter warps);
-// what crosses the pair:
-//   * splitter threads of BOTH CTAs arrive on the LEADER's per-stage `split` mbarrier (remote arrive through mapa) after
-//     their fence.proxy.async -- the leader's MMA thread waits for 256 arrivals, then issues the 12 MMAs of the k-block;
-//   * tcgen05.commit ... multicast::cluster frees the stage in both CTAs (`empty`) and, after the last k-block, publishes
-//     the accumulator (each CTA's TMEM holds its own 128 rows x BN columns) to both epilogues (`tmem_full`);
-//   * epilogue threads of both CTAs arrive on the leader's `tmem_empty` mbarrier (256 arrivals);
-//   * TMEM is allocated / freed with cta_group::2 by warp 1 of each CTA; cluster barriers bracket the kernel so that no
-//     remote arrive or peer shared-memory read can hit a CTA that has not initialised or has already exited.
-// Work item = (256-row m tile, n tile, k split), strided over the persistent grid of pairs.
-constexpr int TC_PAIR_BM = 256;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(rank)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair(uint64_t* bar) {     // arrives on `bar` in both CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma_tf32_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-template <int BN, int STAGES, bool A_MN, bool B_MN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS_INSPLIT, 1)
-gemm_tc_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmC, const int tma_out, const GemmArgs a, const int64_t m_tiles,
-                    const int64_t n_tiles, const int64_t per, const int64_t total_items) {
-  constexpr int BH = BN / 2;                     // columns of the B tile this CTA stages
-  constexpr int A_TILE = TC_BM * TC_BK * 4;      // this CTA's 128 rows: 16 KB
-  constexpr int B_TILE = BH * TC_BK * 4;
-  constexpr int STAGE = 2 * A_TILE + 2 * B_TILE; // [A raw = hi | A lo | B raw = hi | B lo]
-  constexpr bool SHARE = false;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], split_bar[STAGES], tmem_full_bar[2],
-      tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_slot;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();       // 0 = leader (issues the MMAs), 1 = peer
-  const int64_t pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int64_t kblocks = (a.K + TC_BK - 1) / TC_BK;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    if (tma_out) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmC) : "memory");
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);                         // one multicast commit of the leader per phase
-      mbar_init(&split_bar[s], 2 * 32 * TC_SPLIT_WARPS);   // leader only: the splitter threads of both CTAs
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full_bar[s], 1);
-      mbar_init(&tmem_empty_bar[s], 2 * 128);              // leader only: the epilogue threads of both CTAs
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {   // TMEM: 2 accumulator stages x BN fp32 columns, in both CTAs (same address)
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)),
-                 "r"((uint32_t)(2 * BN))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();          // barriers of BOTH CTAs are initialised, TMEM is allocated in both
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (each CTA: its 128 rows of A, its BN/2 columns of B, its own barriers) =====
-      uint32_t it = 0;
-      for (int64_t item = pair; item < total_items; item += npairs) {
-        const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
-        const int m0 = (int)(t.m0 * 2) + (int)rank * TC_BM;          // tc_decode counts 128-row tiles: pair tiles are 256
-        const int n0 = (int)t.n0 + (int)rank * BH;
-        for (int i = 0; i < t.nkb; ++i, ++it) {
-          const int s = (int)(it % STAGES);
-          const uint32_t ph = (it / STAGES) & 1u;
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-          mbar_expect_tx(&full_bar[s], (uint32_t)(A_TILE + B_TILE));
-          uint8_t* st = smem + (size_t)s * STAGE;
-          const int k = (t.kb0 + i) * TC_BK;
-          if (!A_MN) {
-            tma_load_2d(st, &tmA, &full_bar[s], k, m0);
-          } else {
+        const int p = (int)(it % TC_PLANE_STAGES);
+        mbar_wait(&pl_full[p], (it / TC_PLANE_STAGES) & 1u);
+        const uint32_t sa = smem_u32(planes + (size_t)p * PLANE_STAGE) + (uint32_t)wg * (64u * 128u);
+        const uint32_t sb = smem_u32(planes + (size_t)p * PLANE_STAGE) + 2 * A_TILE;
+        wgmma_fence();
 #pragma unroll
-            for (int jj = 0; jj < TC_BM / 32; ++jj) tma_load_2d(st + jj * 4096, &tmA, &full_bar[s], m0 + jj * 32, k);
-          }
-          if (!B_MN) {
-            tma_load_2d(st + 2 * A_TILE, &tmB, &full_bar[s], k, n0);
-          } else {
-#pragma unroll
-            for (int jj = 0; jj < BH / 32; ++jj)
-              tma_load_2d(st + 2 * A_TILE + jj * 4096, &tmB, &full_bar[s], n0 + jj * 32, k);
-          }
+        for (int k = 0; k < TC_BK / 8; ++k) {
+          const uint64_t dAh = make_smem_desc(sa + k * 32), dAl = make_smem_desc(sa + A_TILE + k * 32);
+          const uint64_t dBh = make_smem_desc(sb + k * 32), dBl = make_smem_desc(sb + B_TILE + k * 32);
+          wgmma_tf32<BN>(d, dAl, dBh);   // small cross terms first
+          wgmma_tf32<BN>(d, dAh, dBl);
+          wgmma_tf32<BN>(d, dAh, dBh);
+        }
+        wgmma_commit();
+        if (i > 0) {                     // the previous k-block has retired: its planes may be overwritten
+          wgmma_wait<1>();
+          mbar_arrive(&pl_empty[p ^ 1]);
         }
       }
+      wgmma_wait<0>();
+      mbar_arrive(&pl_empty[(it - 1) % TC_PLANE_STAGES]);
+      tc_epilogue<BN>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane, vec_ok);
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      // ===== MMA issuer (leader CTA only): M = 256 across the pair =====
-      constexpr uint32_t idesc = make_idesc(TC_PAIR_BM, BN, A_MN, B_MN);
-      uint32_t it = 0, j = 0;
-      for (int64_t item = pair; item < total_items; item += npairs, ++j) {
-        const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
-        const uint32_t as = j & 1u, aph = (j >> 1) & 1u;
-        mbar_wait(&tmem_empty_bar[as], aph ^ 1u);      // both epilogues have drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * (uint32_t)BN;
-        for (int i = 0; i < t.nkb; ++i, ++it) {
-          const int s = (int)(it % STAGES);
-          const uint32_t ph = (it / STAGES) & 1u;
-          mbar_wait(&split_bar[s], ph);                // both CTAs have split this stage
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)s * STAGE);
-          const uint32_t sb = sa + 2 * A_TILE;
-#pragma unroll
-          for (int k = 0; k < TC_BK / 8; ++k) {
-            const uint32_t a_off = A_MN ? (uint32_t)k * 1024u : (uint32_t)k * 32u;
-            const uint32_t b_off = B_MN ? (uint32_t)k * 1024u : (uint32_t)k * 32u;
-            const uint32_t a_lbo = A_MN ? 4096u : 16u, a_sbo = A_MN ? 512u : 1024u, a_lt = A_MN ? 1u : 2u;
-            const uint32_t b_lbo = B_MN ? 4096u : 16u, b_sbo = B_MN ? 512u : 1024u, b_lt = B_MN ? 1u : 2u;
-            const uint64_t dAh = make_smem_desc(sa + a_off, a_lbo, a_sbo, a_lt);
-            const uint64_t dAl = make_smem_desc(sa + A_TILE + a_off, a_lbo, a_sbo, a_lt);
-            const uint64_t dBh = make_smem_desc(sb + b_off, b_lbo, b_sbo, b_lt);
-            const uint64_t dBl = make_smem_desc(sb + B_TILE + b_off, b_lbo, b_sbo, b_lt);
-            const uint32_t acc0 = (i > 0 || k > 0) ? 1u : 0u;
-            tc_mma_tf32_pair(d_tmem, dAl, dBh, idesc, acc0);
-            tc_mma_tf32_pair(d_tmem, dAh, dBl, idesc, 1u);
-            tc_mma_tf32_pair(d_tmem, dAh, dBh, idesc, 1u);
-          }
-          tc_commit_pair(&empty_bar[s]);               // stage reusable in both CTAs once these MMAs retire
-        }
-        tc_commit_pair(&tmem_full_bar[as]);            // accumulator complete in both CTAs' TMEM
-      }
-    }
-    __syncwarp();
-  } else if (warp >= 6) {
-    // ===== splitter warps 6..9: lo = raw - trunc_tf32(raw) next to the raw tile (the raw tile is the hi plane) =====
-    const int tid = (int)threadIdx.x - TC_THREADS;
-    constexpr int NSPLIT = 32 * TC_SPLIT_WARPS;
-    uint32_t it = 0;
-    for (int64_t item = pair; item < total_items; item += npairs) {
-      const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
-      for (int i = 0; i < t.nkb; ++i, ++it) {
-        const int s = (int)(it % STAGES);
-        const uint32_t ph = (it / STAGES) & 1u;
-        mbar_wait(&full_bar[s], ph);
-        uint8_t* st = smem + (size_t)s * STAGE;
-        split_tile_inplace<A_TILE, NSPLIT>(st, st + A_TILE, tid);
-        split_tile_inplace<B_TILE, NSPLIT>(st + 2 * A_TILE, st + 2 * A_TILE + B_TILE, tid);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_arrive_cluster(&split_bar[s], 0);         // on the leader's barrier
-      }
-    }
-  } else {
-    // ===== epilogue warps 2..5 (each CTA: its own 128 rows) =====
-    const int q = warp & 3;
-    const bool vec_ok = ((a.ldc & 3) == 0) && aligned16(a.C);
-    uint8_t* stg = smem + (size_t)STAGES * STAGE + (size_t)q * 8192;
-    uint32_t j = 0, slab = 0;
-    for (int64_t item = pair; item < total_items; item += npairs, ++j) {
-      const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
-      const uint32_t as = j & 1u, aph = (j >> 1) & 1u;
-      mbar_wait(&tmem_full_bar[as], aph);
-      tc_fence_after();
-      tc_epilogue_item<BN, SHARE>(a, &tmC, tma_out, tmem_base + as * (uint32_t)BN, q, lane,
-                                  t.m0 * 2 + (int64_t)rank * TC_BM + q * 32, t.n0, stg, slab, vec_ok);
-      tc_fence_before();
-      mbar_arrive_cluster(&tmem_empty_bar[as], 0);     // on the leader's barrier
-    }
-    if (tma_out && lane == 0) bulk_wait_group_all();
-  }
-  tc_fence_before();
-  cluster_sync_all();          // every MMA has retired (the epilogues saw the last commit), every remote arrive has landed
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN))
-                 : "memory");
   }
 }
 
@@ -849,20 +447,21 @@ static int get_encode() {
   return DR_OK;
 }
 
-// 2-D fp32 tensor [outer, inner] (inner contiguous, pitch floats), box {32, box_outer}, SWIZZLE_128B.
-static int make_map(CUtensorMap* tm, const float* base, int64_t inner, int64_t outer, int64_t pitch, int box_outer,
-                    bool mn_major = false) {
+// 2-D fp32 tensor [outer, inner] (inner contiguous, pitch floats), box {box_inner, box_outer}.  K-major operand tiles
+// are boxes {32, rows} in SWIZZLE_128B (the layout wgmma reads); MN-major ones are boxes {rows, 32} staged unswizzled
+// for the transposing splitter pass.
+static int make_map(CUtensorMap* tm, const float* base, int64_t inner, int64_t outer, int64_t pitch, int box_inner,
+                    int box_outer, bool swizzle) {
   cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
   cuuint64_t strides[1] = {(cuuint64_t)pitch * 4};
-  cuuint32_t box[2] = {32u, (cuuint32_t)box_outer};
+  cuuint32_t box[2] = {(cuuint32_t)box_inner, (cuuint32_t)box_outer};
   cuuint32_t estr[2] = {1u, 1u};
   CUresult r = g_encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                         // K-major operand: consecutive k-blocks of a tile walk along each row 128 B at a time -- fetch 256 B
                         // per L2 miss so every second k-block finds its rows in L2 (knob tc_l2_promo: 128 / 256)
-                        (!mn_major && g_tune_tc_l2_promo == 256) ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
-                                                                 : CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        (swizzle && g_tune_tc_l2_promo == 256) ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
+                                                               : CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("gemm_tc: cuTensorMapEncodeTiled failed (CUresult %d; inner=%lld outer=%lld pitch=%lld)", (int)r,
@@ -874,129 +473,57 @@ static int make_map(CUtensorMap* tm, const float* base, int64_t inner, int64_t o
 
 static inline int64_t round4(int64_t v) { return (v + 3) & ~(int64_t)3; }
 
-// Sizes (floats) of the K-major hi/lo planes: A -> [M, pitch], B -> [N, pitch].  An operand that is
+// Sizes (floats) of the K-major hi/lo planes of variant 1: A -> [M, pitch], B -> [N, pitch].  An operand that is
 // already K-major keeps its source pitch (one flat float4 pass); a transposed one gets round4(K).
 static void plane_elems(const GemmArgs& a, bool ta, bool tb, size_t* ae, size_t* be) {
   const int64_t kp = round4(a.K);
-  if (g_tune_tc_mn) {       // operands stay in their stored layout (flat split, source pitch)
-    *ae = (size_t)(ta ? a.K : a.M) * (size_t)a.lda;
-    *be = (size_t)(tb ? a.N : a.K) * (size_t)a.ldb;
-    return;
-  }
   *ae = (size_t)a.M * (size_t)(!ta ? a.lda : kp);
   *be = (size_t)a.N * (size_t)(tb ? a.ldb : kp);
 }
 
-bool gemm_tc_eligible(const GemmArgs& a, bool ta, bool tb) {
-  if (g_tune_gemm_variant == 2) {   // in-kernel split: raw operands by TMA, no workspace
-    if (a.N < g_tune_tc_min_n || (a.N & 3) || a.M < 64 || a.K < 32) return false;
-    if ((a.lda & 3) || !aligned16(a.A) || (a.ldb & 3) || !aligned16(a.B)) return false;
-    if (a.M >= ((int64_t)1 << 31) || a.K >= ((int64_t)1 << 31) || a.N >= ((int64_t)1 << 31)) return false;
-    return true;
-  }
-  if (g_tune_gemm_variant != 1) return false;
-  // measured (profiles/README.md): for N = 32 the extra hi/lo split of the activations costs more than the
-  // 128 x 32 tensor-core tile saves over the FFMA kernel, so skinny layers stay on FFMA unless tc_min_n is lowered
-  if (a.N < (g_tune_tc_min_n > 96 ? g_tune_tc_min_n : 96) || (a.N & 3) || a.M < 64 || a.K < 32) return false;
-  // operands already K-major are split in place with float4 accesses
-  if ((!ta || g_tune_tc_mn) && ((a.lda & 3) || !aligned16(a.A))) return false;
-  if ((tb || g_tune_tc_mn) && ((a.ldb & 3) || !aligned16(a.B))) return false;
-  size_t ae, be;
-  plane_elems(a, ta, tb, &ae, &be);
-  if (!g_ws_ptr) return false;
-  if (g_cache_on && g_tune_tc_mn) {      // operands whose planes are already cached need no new space
-    auto cached = [](const float* src, size_t elems) {
-      for (int i = 0; i < g_nplanes; ++i)
-        if (g_planes[i].src == src && g_planes[i].elems == elems) return true;
-      return false;
-    };
-    size_t need = 0;
-    if (!cached(a.A, ae)) need += 2 * ae;
-    if (!cached(a.B, be)) need += 2 * be;
-    if ((g_bump + need) * sizeof(float) > g_ws_bytes) return false;
-  } else {
-    const size_t need = (ae + be) * 2 * sizeof(float) + 4096;
-    if (g_ws_bytes < need) return false;
-  }
-  if (a.M >= ((int64_t)1 << 31) || a.K >= ((int64_t)1 << 31) || a.N >= ((int64_t)1 << 31)) return false;
-  return true;
+static bool plane_cached(const float* src, size_t elems, bool transposed) {
+  for (int i = 0; i < g_nplanes; ++i)
+    if (g_planes[i].src == src && g_planes[i].elems == elems && g_planes[i].transposed == transposed) return true;
+  return false;
 }
 
-int g_tune_tc_stages = 0;    // 0 = default ring depth per tile width; 2 = two stages for BN = 128 (leaves ~64 KB of shared
-                            // memory per SM so an HBM-bound kernel on another stream can co-reside with the persistent GEMM)
-int g_tune_tc_tma_out = 1;   // 1 (default) = epilogue through shared memory + TMA store / reduce-add; 0 = round-1 register stores
-int g_tune_gemm_prof = 0;   // 1 = launch the instrumented instantiation (BN = 128 INSPLIT only); read with dr_gemm_prof_read
+bool gemm_tc_eligible(const GemmArgs& a, bool ta, bool tb) {
+  if (g_tune_gemm_variant != 1 && g_tune_gemm_variant != 2) return false;
+  if (a.N < g_tune_tc_min_n || (a.N & 3) || a.M < 64 || a.K < 32) return false;
+  if (a.M >= ((int64_t)1 << 31) || a.K >= ((int64_t)1 << 31) || a.N >= ((int64_t)1 << 31)) return false;
+  if (g_tune_gemm_variant == 2)     // in-kernel split: raw operands by TMA, no workspace
+    return !((a.lda & 3) || !aligned16(a.A) || (a.ldb & 3) || !aligned16(a.B));
+  // operands already K-major are split in place with float4 accesses
+  if (!ta && ((a.lda & 3) || !aligned16(a.A))) return false;
+  if (tb && ((a.ldb & 3) || !aligned16(a.B))) return false;
+  if (!g_ws_ptr) return false;
+  size_t ae, be;
+  plane_elems(a, ta, tb, &ae, &be);
+  size_t need = 0;
+  if (!(g_cache_on && plane_cached(a.A, ae, ta))) need += 2 * ae;
+  if (!(g_cache_on && plane_cached(a.B, be, !tb))) need += 2 * be;
+  return ((g_cache_on ? g_bump : 0) + need) * sizeof(float) <= g_ws_bytes;
+}
 
-template <int BN, int STAGES, bool A_MN, bool B_MN, bool INSPLIT = false, bool SHARE = false>
-static int launch_tc(const CUtensorMap* tms, const GemmArgs& a, cudaStream_t st) {
-  constexpr int STAGE = 2 * TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4;
-  constexpr size_t smem = (size_t)STAGES * STAGE + (SHARE ? TC_EPI_STAGING / 2 : TC_EPI_STAGING) + 1024;
-  static_assert(smem <= 232448, "operand ring + epilogue staging exceed the 227 KB of shared memory per CTA");
-  constexpr bool kProfInst = INSPLIT && BN == 128;
-  auto k = SHARE ? gemm_tc_kernel<BN, STAGES, A_MN, B_MN, INSPLIT, false, SHARE>
-           : (kProfInst && g_tune_gemm_prof) ? gemm_tc_kernel<BN, STAGES, A_MN, B_MN, INSPLIT, kProfInst>
-                                             : gemm_tc_kernel<BN, STAGES, A_MN, B_MN, INSPLIT, false>;
+int g_tune_tc_stages = 0;    // 0 = three raw stages; 2 = two (32 KB less shared memory at the widest tile)
+int g_tune_tc_pair = 1;      // accepted and read back for callers that set it; H100 has no two-CTA MMA, so it selects nothing
+
+template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
+static int launch_tc(const CUtensorMap* tms, const GemmArgs& a, int raw_stages, cudaStream_t st) {
+  constexpr int PLANE_STAGE = 2 * TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4;
+  const size_t smem = (size_t)TC_PLANE_STAGES * PLANE_STAGE + (PRESPLIT ? 0 : (size_t)raw_stages * (PLANE_STAGE / 2)) + 1024;
+  static_assert((size_t)TC_PLANE_STAGES * PLANE_STAGE + 3 * (PLANE_STAGE / 2) + 1024 + 256 <= 232448,
+                "plane ring + raw ring exceed the 227 KB of shared memory per CTA");
+  auto k = gemm_tc_kernel<BN, A_MN, B_MN, PRESPLIT>;
   DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  // output through TMA (store / reduce-add) whenever C is 16-B aligned with a 16-B multiple pitch
-  CUtensorMap tmC;
-  memset(&tmC, 0, sizeof(tmC));
-  int tma_out = (g_tune_tc_tma_out && (a.ldc & 3) == 0 && aligned16(a.C)) ? 1 : 0;
-  if (tma_out)
-    if (int rc = make_map(&tmC, a.C, a.N, a.M, a.ldc, 32)) return rc;
   const int64_t m_tiles = (a.M + TC_BM - 1) / TC_BM, n_tiles = (a.N + BN - 1) / BN;
   const int64_t kblocks = (a.K + TC_BK - 1) / TC_BK;
   const int64_t per = (kblocks + a.splitk - 1) / a.splitk;
   const int64_t splits = (kblocks + per - 1) / per;          // every split owns >= 1 k-block
   const int64_t total = m_tiles * n_tiles * splits;
-  const int64_t ctas = total < (int64_t)kNumSMs ? total : (int64_t)kNumSMs;
-  k<<<(unsigned)ctas, INSPLIT ? TC_THREADS_INSPLIT : TC_THREADS, smem, st>>>(tms[0], tms[1], tms[2], tms[3], tmC, tma_out, a,
-                                                                               m_tiles, n_tiles, per, total);
+  const int64_t ctas = total < (int64_t)num_sms() ? total : (int64_t)num_sms();
+  k<<<(unsigned)ctas, TC_THREADS, smem, st>>>(tms[0], tms[1], tms[2], tms[3], a, raw_stages, m_tiles, n_tiles, per, total);
   DR_CUDA_LAUNCH_CHECK("gemm_tc");
-  return DR_OK;
-}
-
-
-int g_tune_tc_pair = 1;      // 1 (default) = CTA-pair kernel (cta_group::2) for N >= 128 outputs where its 74 workers beat the 148
-                             // single CTAs (rule in gemm_tc_launch); 2 = always for N >= 128; 0 = never
-
-template <int BN, int STAGES, bool A_MN, bool B_MN>
-static int launch_tc_pair(const CUtensorMap* tms, const GemmArgs& a, cudaStream_t st) {
-  constexpr int STAGE = 2 * TC_BM * TC_BK * 4 + 2 * (BN / 2) * TC_BK * 4;
-  constexpr size_t smem = (size_t)STAGES * STAGE + TC_EPI_STAGING + 1024;
-  static_assert(smem <= 232448, "operand ring + epilogue staging exceed the 227 KB of shared memory per CTA");
-  auto k = gemm_tc_pair_kernel<BN, STAGES, A_MN, B_MN>;
-  DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  CUtensorMap tmC;
-  memset(&tmC, 0, sizeof(tmC));
-  int tma_out = (g_tune_tc_tma_out && (a.ldc & 3) == 0 && aligned16(a.C)) ? 1 : 0;
-  if (tma_out)
-    if (int rc = make_map(&tmC, a.C, a.N, a.M, a.ldc, 32)) return rc;
-  const int64_t m_tiles = (a.M + TC_PAIR_BM - 1) / TC_PAIR_BM, n_tiles = (a.N + BN - 1) / BN;
-  const int64_t kblocks = (a.K + TC_BK - 1) / TC_BK;
-  const int64_t pairs_max = kNumSMs / 2;
-  int64_t splitk = a.splitk;
-  if (a.epi == EPI_ATOMIC && a.splitk > 1) {
-    // split-K callers sized `splitk` for 128 x 128 tiles on 148 CTAs; here the workers are 74 pairs on 256 x BN tiles:
-    // the split count whose item total fills whole rounds of the pairs best (>= 8 k-blocks per split)
-    const int64_t base = m_tiles * n_tiles;
-    int64_t best = 1;
-    double best_eff = 0.0;
-    const int64_t smax = kblocks / 8 > 1 ? (kblocks / 8 < 256 ? kblocks / 8 : 256) : 1;
-    for (int64_t sk = 1; sk <= smax; ++sk) {
-      const int64_t items = base * sk;
-      const int64_t rounds = (items + pairs_max - 1) / pairs_max;
-      const double eff = (double)items / (double)(rounds * pairs_max);
-      if (eff > best_eff + 1e-9 && (rounds <= 4 || eff > 0.97)) { best_eff = eff; best = sk; }
-      if (rounds > 4) break;
-    }
-    splitk = best;
-  }
-  const int64_t per = (kblocks + splitk - 1) / splitk;
-  const int64_t splits = (kblocks + per - 1) / per;
-  const int64_t total = m_tiles * n_tiles * splits;
-  const int64_t pairs = total < pairs_max ? total : pairs_max;
-  k<<<(unsigned)(2 * pairs), TC_THREADS_INSPLIT, smem, st>>>(tms[0], tms[2], tmC, tma_out, a, m_tiles, n_tiles, per, total);
-  DR_CUDA_LAUNCH_CHECK("gemm_tc_pair");
   return DR_OK;
 }
 
@@ -1007,7 +534,7 @@ static int make_planes(const float* src, bool stored_k_major, int64_t rows, int6
   if (stored_k_major) {
     const int64_t n4 = rows * ld / 4;
     int64_t ctas = (n4 + 255) / 256;
-    if (ctas > kNumSMs * 8) ctas = kNumSMs * 8;
+    if (ctas > num_sms() * 8) ctas = num_sms() * 8;
     if (ctas < 1) ctas = 1;
     split_tf32_kernel<<<(unsigned)ctas, 256, 0, st>>>(src, n4, hi, lo);
     DR_CUDA_LAUNCH_CHECK("split_tf32");
@@ -1015,7 +542,7 @@ static int make_planes(const float* src, bool stored_k_major, int64_t rows, int6
   } else {
     const int64_t kp = round4(K);
     const int64_t tiles = ((K + 31) / 32) * ((rows + 31) / 32);
-    int64_t ctas = tiles < (int64_t)kNumSMs * 16 ? tiles : (int64_t)kNumSMs * 16;
+    int64_t ctas = tiles < (int64_t)num_sms() * 16 ? tiles : (int64_t)num_sms() * 16;
     if (ctas < 1) ctas = 1;
     split_tf32_transpose_kernel<<<(unsigned)ctas, dim3(32, 8), 0, st>>>(src, K, rows, ld, kp, hi, lo);
     DR_CUDA_LAUNCH_CHECK("split_tf32_transpose");
@@ -1030,172 +557,73 @@ int gemm_tc_launch(const GemmArgs& a0, bool ta, bool tb, cudaStream_t st) {
   if (a.splitk < 1) a.splitk = 1;
   const int64_t kblocks = (a.K + TC_BK - 1) / TC_BK;
   if (a.splitk > kblocks) a.splitk = (int)kblocks;
+  // skinny outputs (the 256->32 tower layer and its weight gradient) get a 128 x 32 / 128 x 64 tile
+  int bn = a.N <= 32 ? 32 : (a.N <= 64 ? 64 : 128);
+  if (g_tune_gemm_bn == 32 || g_tune_gemm_bn == 64) bn = g_tune_gemm_bn;
+  CUtensorMap tms[4];
   if (g_tune_gemm_variant == 2) {
-    // Variant 2: tensor maps straight on the source operands (consumed as stored), split in shared memory.
+    // Variant 2: tensor maps straight on the source operands (staged as stored), split in shared memory.
     const bool A_MN = ta, B_MN = !tb;
-    CUtensorMap tm2[4];
+    const int raw_stages = (g_tune_tc_stages == 2 || a.stages == 2 || a.share) ? 2 : 3;
     if (!A_MN) {
-      if (int rc = make_map(&tm2[0], a.A, a.K, a.M, a.lda, TC_BM)) return rc;
+      if (int rc = make_map(&tms[0], a.A, a.K, a.M, a.lda, TC_BK, TC_BM, true)) return rc;
     } else {
-      if (int rc = make_map(&tm2[0], a.A, a.M, a.K, a.lda, TC_BK, true)) return rc;
-    }
-    // 128 x 256 tiles (2-stage ring) when they waste no more columns than 128-wide ones (N = 256, 416: C2 step
-    // 0.686 -> 0.657 ms); N = 832 (C3) keeps 128.  Knob gemm_bn: 0 = this rule, 128 / 256 = force.
-    const int64_t pad256 = (a.N + 255) / 256 * 256, pad128 = (a.N + 127) / 128 * 128;
-    const int64_t tiles256 = ((a.M + TC_BM - 1) / TC_BM) * (pad256 / 256) * (a.splitk > 0 ? a.splitk : 1);
-    const bool two_stage = g_tune_tc_stages == 2 || a.stages == 2;      // forces the 128-wide tile
-    const bool wide = !two_stage && !a.share && a.N >= 256 && (g_tune_gemm_bn == 256 ||
-                                     (g_tune_gemm_bn == 0 && pad256 <= pad128 && tiles256 >= 2 * kNumSMs));   // enough tiles to fill the SMs
-    const int bn = a.N <= 32 ? 32 : (a.N <= 64 ? 64 : (wide ? 256 : 128));
-    const int pbn = (a.N >= 256 && pad256 <= pad128) ? 256 : 128;
-    bool use_pair = g_tune_tc_pair != 0 && a.N >= 128 && !a.share && !two_stage && a.M >= 128;
-    if (use_pair && g_tune_tc_pair == 1 && !(a.epi == EPI_ATOMIC && a.splitk > 1)) {
-      // rounds x cycles per k-block of one worker (measured, profiles/gemm_prof_*: the single-CTA loop is bound by shared
-      // memory at 2250 / 1500 cycles per 128 x 256 / 128 x 128 x 32 k-block, a pair by its MMAs at 1536 per 256 x 256 and by
-      // shared memory at 1125 per 256 x 128): small problems that fill the 148 single CTAs better than the 74 pairs stay
-      // on the single-CTA kernel (knob tc_pair = 2 forces the pair kernel)
-      const int64_t items_p = ((a.M + TC_PAIR_BM - 1) / TC_PAIR_BM) * ((a.N + pbn - 1) / pbn);
-      const int64_t items_s = ((a.M + TC_BM - 1) / TC_BM) * ((a.N + bn - 1) / bn);
-      const int64_t pairs_max = kNumSMs / 2;
-      const double t_p = (double)((items_p + pairs_max - 1) / pairs_max) * (pbn == 256 ? 1536.0 : 1125.0);
-      const double t_s = (double)((items_s + kNumSMs - 1) / kNumSMs) * (bn == 256 ? 2250.0 : 1500.0);
-      if (t_p > 0.9 * t_s) use_pair = false;
-    }
-    if (use_pair) {
-      // CTA-pair kernel: 256 x BN tiles, each CTA stages its 128 rows of A and BN / 2 columns of B
-      if (!B_MN) {
-        if (int rc = make_map(&tm2[2], a.B, a.K, a.N, a.ldb, pbn / 2)) return rc;
-      } else {
-        if (int rc = make_map(&tm2[2], a.B, a.N, a.K, a.ldb, TC_BK, true)) return rc;
-      }
-#define DR_TCP_LAUNCH(BN_, ST_)                                                             \
-      do {                                                                                  \
-        if (!A_MN && !B_MN) return launch_tc_pair<BN_, ST_, false, false>(tm2, a, st);      \
-        if (!A_MN && B_MN) return launch_tc_pair<BN_, ST_, false, true>(tm2, a, st);        \
-        if (A_MN && !B_MN) return launch_tc_pair<BN_, ST_, true, false>(tm2, a, st);        \
-        return launch_tc_pair<BN_, ST_, true, true>(tm2, a, st);                            \
-      } while (0)
-      if (pbn == 256) DR_TCP_LAUNCH(256, 3);
-      DR_TCP_LAUNCH(128, 4);
-#undef DR_TCP_LAUNCH
+      if (int rc = make_map(&tms[0], a.A, a.M, a.K, a.lda, TC_BM, TC_BK, false)) return rc;
     }
     if (!B_MN) {
-      if (int rc = make_map(&tm2[2], a.B, a.K, a.N, a.ldb, bn)) return rc;
+      if (int rc = make_map(&tms[2], a.B, a.K, a.N, a.ldb, TC_BK, bn, true)) return rc;
     } else {
-      if (int rc = make_map(&tm2[2], a.B, a.N, a.K, a.ldb, TC_BK, true)) return rc;
+      if (int rc = make_map(&tms[2], a.B, a.N, a.K, a.ldb, bn, TC_BK, false)) return rc;
     }
-    tm2[1] = tm2[0];
-    tm2[3] = tm2[2];
-#define DR_TC2_LAUNCH(BN_, ST_)                                                             \
+    tms[1] = tms[0];
+    tms[3] = tms[2];
+#define DR_TC2_LAUNCH(BN_)                                                                  \
     do {                                                                                    \
-      if (!A_MN && !B_MN) return launch_tc<BN_, ST_, false, false, true>(tm2, a, st);       \
-      if (!A_MN && B_MN) return launch_tc<BN_, ST_, false, true, true>(tm2, a, st);         \
-      if (A_MN && !B_MN) return launch_tc<BN_, ST_, true, false, true>(tm2, a, st);         \
-      return launch_tc<BN_, ST_, true, true, true>(tm2, a, st);                             \
+      if (!A_MN && !B_MN) return launch_tc<BN_, false, false, false>(tms, a, raw_stages, st);  \
+      if (!A_MN && B_MN) return launch_tc<BN_, false, true, false>(tms, a, raw_stages, st);    \
+      if (A_MN && !B_MN) return launch_tc<BN_, true, false, false>(tms, a, raw_stages, st);    \
+      return launch_tc<BN_, true, true, false>(tms, a, raw_stages, st);                        \
     } while (0)
-    if (bn == 32) DR_TC2_LAUNCH(32, 4);
-    if (bn == 64) DR_TC2_LAUNCH(64, 4);
-    if (two_stage) DR_TC2_LAUNCH(128, 2);
-    // co-residency build (GemmArgs::share): only the operand layout of the weight-gradient GEMM (X^T and gZ as stored)
-    if (a.share && bn == 128 && A_MN && B_MN) return launch_tc<128, 3, true, true, true, true>(tm2, a, st);
-    if (bn == 256) DR_TC2_LAUNCH(256, 2);
-    DR_TC2_LAUNCH(128, 3);
+    if (bn == 32) DR_TC2_LAUNCH(32);
+    if (bn == 64) DR_TC2_LAUNCH(64);
+    DR_TC2_LAUNCH(128);
 #undef DR_TC2_LAUNCH
   }
+  // Variant 1: K-major hi/lo planes in the workspace.  A(m,k): !ta -> stored [M,K] (flat split), ta -> stored [K,M]
+  // (transposing split); B(k,n): tb -> stored [N,K] (flat), !tb -> stored [K,N] (transposing).
   size_t ae, be;
   plane_elems(a, ta, tb, &ae, &be);
-  const size_t need = (ae + be) * 2 * sizeof(float);
-  DR_REQUIRE(g_ws_ptr && (g_tune_tc_mn || g_ws_bytes >= need), DR_EINVAL, "gemm_tc: workspace too small (%zu needed)", need);
-  float* Ah = reinterpret_cast<float*>(g_ws_ptr);
-  float* Al = Ah + ae;
-  float* Bh = Al + ae;
-  float* Bl = Bh + be;
+  if (!g_cache_on) g_bump = 0;
+  auto planes = [&](const float* src, size_t elems, bool transposed, int64_t rows, int64_t ld, float** hi, float** lo,
+                    int64_t* pitch) -> int {
+    if (g_cache_on)
+      for (int i = 0; i < g_nplanes; ++i)
+        if (g_planes[i].src == src && g_planes[i].elems == elems && g_planes[i].transposed == transposed) {
+          *hi = g_planes[i].hi; *lo = g_planes[i].lo; *pitch = g_planes[i].pitch;
+          return DR_OK;
+        }
+    DR_REQUIRE(g_ws_ptr && (g_bump + 2 * elems) * sizeof(float) <= g_ws_bytes, DR_EINVAL,
+               "gemm_tc: workspace exhausted (%zu B registered)", g_ws_bytes);
+    *hi = reinterpret_cast<float*>(g_ws_ptr) + g_bump;
+    *lo = *hi + elems;
+    g_bump += 2 * elems;
+    if (int rc = make_planes(src, !transposed, rows, a.K, ld, *hi, *lo, pitch, st)) return rc;
+    if (g_cache_on && g_nplanes < 64) g_planes[g_nplanes++] = PlaneEntry{src, elems, transposed, *hi, *lo, *pitch};
+    return DR_OK;
+  };
+  float *Ah, *Al, *Bh, *Bl;
   int64_t pa = 0, pb = 0;
-  CUtensorMap tms[4];
-  if (g_tune_tc_mn) {
-    // MN-major operands are consumed as stored (SWIZZLE_128B_BASE32B): no transposing pre-pass.
-    const bool A_MN = ta, B_MN = !tb;
-    if (!g_cache_on) g_bump = 0;
-    auto planes = [&](const float* src, size_t elems, int64_t rows, int64_t ld, float** hi, float** lo,
-                      int64_t* pitch) -> int {
-      if (g_cache_on)
-        for (int i = 0; i < g_nplanes; ++i)
-          if (g_planes[i].src == src && g_planes[i].elems == elems) {
-            *hi = g_planes[i].hi; *lo = g_planes[i].lo; *pitch = ld;
-            return DR_OK;
-          }
-      DR_REQUIRE((g_bump + 2 * elems) * sizeof(float) <= g_ws_bytes, DR_EINVAL,
-                 "gemm_tc: workspace exhausted (%zu B registered)", g_ws_bytes);
-      *hi = reinterpret_cast<float*>(g_ws_ptr) + g_bump;
-      *lo = *hi + elems;
-      g_bump += 2 * elems;
-      if (g_cache_on && g_nplanes < 64) g_planes[g_nplanes++] = PlaneEntry{src, elems, *hi, *lo};
-      return make_planes(src, true, rows, 0, ld, *hi, *lo, pitch, st);
-    };
-    if (int rc = planes(a.A, ae, ta ? a.K : a.M, a.lda, &Ah, &Al, &pa)) return rc;
-    if (int rc = planes(a.B, be, tb ? a.N : a.K, a.ldb, &Bh, &Bl, &pb)) return rc;
-    if (!A_MN) {
-      if (int rc = make_map(&tms[0], Ah, a.K, a.M, pa, TC_BM)) return rc;
-      if (int rc = make_map(&tms[1], Al, a.K, a.M, pa, TC_BM)) return rc;
-    } else {
-      if (int rc = make_map(&tms[0], Ah, a.M, a.K, pa, TC_BK, true)) return rc;
-      if (int rc = make_map(&tms[1], Al, a.M, a.K, pa, TC_BK, true)) return rc;
-    }
-    // skinny outputs (the 256->32 tower layer and its weight gradient) get a 128 x 32 tile and a deeper ring
-    const int bn = a.N <= 32 ? 32 : (a.N <= 64 ? 64 : 128);
-    if (!B_MN) {
-      if (int rc = make_map(&tms[2], Bh, a.K, a.N, pb, bn)) return rc;
-      if (int rc = make_map(&tms[3], Bl, a.K, a.N, pb, bn)) return rc;
-    } else {
-      if (int rc = make_map(&tms[2], Bh, a.N, a.K, pb, TC_BK, true)) return rc;
-      if (int rc = make_map(&tms[3], Bl, a.N, a.K, pb, TC_BK, true)) return rc;
-    }
-#define DR_TC_LAUNCH(BN_, ST_)                                                              \
-    do {                                                                                    \
-      if (!A_MN && !B_MN) return launch_tc<BN_, ST_, false, false>(tms, a, st);             \
-      if (!A_MN && B_MN) return launch_tc<BN_, ST_, false, true>(tms, a, st);               \
-      if (A_MN && !B_MN) return launch_tc<BN_, ST_, true, false>(tms, a, st);               \
-      return launch_tc<BN_, ST_, true, true>(tms, a, st);                                   \
-    } while (0)
-    if (bn == 32) DR_TC_LAUNCH(32, 4);
-    if (bn == 64) DR_TC_LAUNCH(64, 4);
-    DR_TC_LAUNCH(128, 3);
-#undef DR_TC_LAUNCH
-  }
-  // A(m,k): !ta -> stored [M,K] (already K-major);  ta -> stored [K,M] -> transpose
-  if (int rc = make_planes(a.A, !ta, a.M, a.K, a.lda, Ah, Al, &pa, st)) return rc;
-  // B(k,n):  tb -> stored [N,K] (already K-major); !tb -> stored [K,N] -> transpose
-  if (int rc = make_planes(a.B, tb, a.N, a.K, a.ldb, Bh, Bl, &pb, st)) return rc;
-  // measured on B200 (profiles/): 128 x 128 tiles with a 3-stage ring beat 128 x 256 with 2 stages
-  const bool wide = (g_tune_gemm_bn == 256);
-  const int BN = wide ? 256 : 128;
-  if (int rc = make_map(&tms[0], Ah, a.K, a.M, pa, TC_BM)) return rc;
-  if (int rc = make_map(&tms[1], Al, a.K, a.M, pa, TC_BM)) return rc;
-  if (int rc = make_map(&tms[2], Bh, a.K, a.N, pb, BN)) return rc;
-  if (int rc = make_map(&tms[3], Bl, a.K, a.N, pb, BN)) return rc;
-  if (wide) return launch_tc<256, 2, false, false>(tms, a, st);
-  return launch_tc<128, 3, false, false>(tms, a, st);
+  if (int rc = planes(a.A, ae, ta, a.M, a.lda, &Ah, &Al, &pa)) return rc;
+  if (int rc = planes(a.B, be, !tb, a.N, a.ldb, &Bh, &Bl, &pb)) return rc;
+  if (int rc = make_map(&tms[0], Ah, a.K, a.M, pa, TC_BK, TC_BM, true)) return rc;
+  if (int rc = make_map(&tms[1], Al, a.K, a.M, pa, TC_BK, TC_BM, true)) return rc;
+  if (int rc = make_map(&tms[2], Bh, a.K, a.N, pb, TC_BK, bn, true)) return rc;
+  if (int rc = make_map(&tms[3], Bl, a.K, a.N, pb, TC_BK, bn, true)) return rc;
+  if (bn == 32) return launch_tc<32, false, false, true>(tms, a, 0, st);
+  if (bn == 64) return launch_tc<64, false, false, true>(tms, a, 0, st);
+  return launch_tc<128, false, false, true>(tms, a, 0, st);
 }
 
-}  // namespace dr
-
-extern "C" int dr_gemm_prof_read(uint64_t* out16, int reset) {
-  DR_REQUIRE(out16, DR_EINVAL, "dr_gemm_prof_read: null output");
-  unsigned long long h[16];
-  DR_CUDA_CALL(cudaMemcpyFromSymbol(h, dr::g_tc_prof, sizeof(h)));
-  for (int i = 0; i < 16; ++i) out16[i] = (uint64_t)h[i];
-  if (reset) {
-    memset(h, 0, sizeof(h));
-    DR_CUDA_CALL(cudaMemcpyToSymbol(dr::g_tc_prof, h, sizeof(h)));
-  }
-  return DR_OK;
-}
-
-namespace dr {
-int gemm_set_store_hi(int v) {       // developer knob tc_store_hi (api.cu)
-  DR_CUDA_CALL(cudaMemcpyToSymbol(g_store_hi, &v, sizeof(int)));
-  return DR_OK;
-}
 }  // namespace dr
 
 extern "C" int dr_gemm_plane_cache(int enable) {

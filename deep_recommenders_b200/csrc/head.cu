@@ -106,7 +106,7 @@ extern "C" int dr_dense_head_bce_fwd_bwd(const float* a, const float* w, const f
   if (gb) DR_CUDA_CALL(cudaMemsetAsync(gb, 0, sizeof(float), st));
   if (gb_prev) DR_CUDA_CALL(cudaMemsetAsync(gb_prev, 0, sizeof(float) * K, st));
   int64_t ctas = (B + 7) / 8;                  // 8 warps per CTA, one row per warp iteration
-  if (ctas > (int64_t)kNumSMs * 8) ctas = (int64_t)kNumSMs * 8;
+  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
   const float invB = 1.f / (float)B;
 #define DR_HEAD(KPL)                                                                                               \
   head_bce_kernel<KPL><<<(unsigned)ctas, 256, 0, st>>>(a, w, bias, z_add, y, B, K, prev_act, invB, logit_out, prob_out, \

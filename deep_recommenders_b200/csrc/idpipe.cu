@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(256) vocab_lookup_i64_kernel(const int64_t* __
 
 static inline unsigned grid_for(int64_t n) {
   int64_t ctas = (n + 255) / 256;
-  if (ctas > kNumSMs * 8) ctas = kNumSMs * 8;
+  if (ctas > num_sms() * 8) ctas = num_sms() * 8;
   return (unsigned)(ctas < 1 ? 1 : ctas);
 }
 

@@ -61,7 +61,7 @@ extern "C" int dr_adam_step(float* p, float* g, float* m, float* v, int64_t n, f
              "dr_adam_step: beta1=%g beta2=%g eps=%g out of range", (double)beta1, (double)beta2, (double)eps);
   const int vec_ok = aligned16(p) && aligned16(g) && aligned16(m) && aligned16(v);
   int64_t ctas = (n / 4 + 255) / 256;
-  if (ctas > kNumSMs * 8) ctas = kNumSMs * 8;
+  if (ctas > num_sms() * 8) ctas = num_sms() * 8;
   if (ctas < 1) ctas = 1;
   adam_kernel<<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, lr_t, 1.f - beta1, 1.f - beta2, eps,
                                                                  zero_grad, vec_ok, lr_t_dev);
@@ -174,7 +174,7 @@ extern "C" int dr_lazy_adam_rows(const void* ids, int id_bytes, int64_t B, int S
   const int64_t n = B * S;
   const int64_t groups_per_cta = 256 / lpr;
   int64_t ctas = (n + groups_per_cta - 1) / groups_per_cta;
-  if (ctas > (int64_t)kNumSMs * 8) ctas = (int64_t)kNumSMs * 8;
+  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
   cudaStream_t st = (cudaStream_t)stream;
 #define DR_LAZY(L, IdT)                                                                                              \
   lazy_adam_rows_kernel<L, IdT><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, n, S, rows, slot_offsets, p, g, m, v, \

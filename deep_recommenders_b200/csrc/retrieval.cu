@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(256) column_rank_kernel(const float* __restric
 
 static inline unsigned flat_grid(int64_t n) {
   int64_t ctas = (n + 255) / 256;
-  if (ctas > kNumSMs * 8) ctas = kNumSMs * 8;
+  if (ctas > num_sms() * 8) ctas = num_sms() * 8;
   return (unsigned)(ctas < 1 ? 1 : ctas);
 }
 

@@ -325,7 +325,7 @@ using namespace dr;
 
 namespace dr {
 // ---- tensor-core form (round 2): the contraction Q C^T (sbcnm.py:129) and the two gradient contractions run on the
-// tcgen05 3xTF32 GEMM core; the score block [rb, nc] of rb query rows lives in a caller-provided workspace between the
+// wgmma 3xTF32 GEMM core; the score block [rb, nc] of rb query rows lives in a caller-provided workspace between the
 // GEMM and two one-pass kernels (the FFMA kernels above never materialise scores but reach ~18 TFLOP/s; this form trades
 // rb * nc * 4 B of scratch traffic -- ~1 ms / GiB at HBM speed -- for tensor-core contractions).
 int softmax_scores_block(const float* q_blk, const float* c, const float* p, const int64_t* ids, int64_t row0, int64_t rb,
@@ -487,7 +487,7 @@ extern "C" int dr_inbatch_softmax_bwd_ws(const float* q, const float* c, const f
       if (int rc = softmax_scores_block(q + r0 * D, c, p, cand_ids, r0, rb, nc, D, scores_ws, st)) return rc;
     const int64_t work = rb * ((nc & 3) ? nc : nc / 4);
     int64_t ctas = (work + 255) / 256;
-    if (ctas > (int64_t)kNumSMs * 16) ctas = (int64_t)kNumSMs * 16;
+    if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
     softmax_rows_bwd_kernel<<<(unsigned)ctas, 256, 0, st>>>(scores_ws, rb, nc, r0, inv_tau, w, lse, gloss);
     DR_CUDA_LAUNCH_CHECK("softmax_rows_bwd");
     if (int rc = softmax_grad_block(scores_ws, q + r0 * D, c, rb, nc, D, gq + r0 * D, gc, st)) return rc;

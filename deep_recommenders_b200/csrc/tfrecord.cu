@@ -282,9 +282,9 @@ extern "C" int dr_example_parse_feature(const uint8_t* buf, const int64_t* rec_o
 // Large batches CAN be parsed by several host threads (dr_set_host_threads; tf.data's num_parallel_calls): record
 // ranges are counted in parallel, a serial prefix over the ranges gives every range its output offsets, then the
 // ranges are filled in parallel -- the output is identical for any thread count.  The threaded path walks every
-// record three times instead of two; on the 8-vCPU build container it is 3-5x faster than serial when the output
-// buffers are already faulted in, and erratic (first-touch page faults of fresh buffers) otherwise
-// (profiles/README.md, tfrecord_parse_r01.json), so serial is the default and threading is opt-in.
+// record three times instead of two; it pays only when the output buffers are already faulted in (first-touch page
+// faults of fresh buffers dominate otherwise; tools/bench_tfrecord.py times both), so serial is the default and
+// threading is opt-in.
 namespace dr {
 namespace tfr {
 

@@ -9,10 +9,9 @@ Layout in HBM (layout="fused", the default when the first-order term exists and 
   weight : [sum_s rows_s, 32] fp32   row = [ D embedding floats | w | pad ] in ONE 128-byte,
            128-byte-aligned line: the first-order weight w of an id (the
            Dense(1, kernel_initializer="zeros") kernel entry of the reference's multi-hot linear
-           term) travels in the same HBM line as its embedding vector.  Measured on B200
-           (profiles/): L2 fills from HBM in 128-B lines, so a 64-B row costs 128 B of DRAM traffic
-           anyway and a separate 4-B first-order gather costs another 128 B; fusing them halves the
-           random DRAM lines per lookup.
+           term) travels in the same HBM line as its embedding vector: a separate 4-B first-order
+           gather would touch a second random DRAM line per lookup; fusing them halves the random
+           lines per lookup.
   bias   : [1]                       that Dense's bias.
 layout="split": weight [sum rows, D] and linear [sum rows] as two arrays (two random lines per
 lookup; used for D >= 32 where the row already fills whole lines).  Table s occupies rows

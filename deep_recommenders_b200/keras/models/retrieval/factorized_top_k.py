@@ -8,7 +8,7 @@ Mirrors reference keras/models/retrieval/factorized_top_k.py:
   :139-262  Streaming(k, query_model, handle_incomplete_batches, num_parallel_calls, sorted_order)
   :265-334  BruteForce(k, query_model)
   :464-522  FactorizedTopK(candidates, metrics, k, name)
-The arithmetic runs in the CUDA library: scores = Q @ C^T through dr_scores_fwd (tcgen05 3xTF32 / FFMA GEMM),
+The arithmetic runs in the CUDA library: scores = Q @ C^T through dr_scores_fwd (wgmma 3xTF32 / FFMA GEMM),
 selection through dr_topk_rows (tf.math.top_k order: descending, ties -> lower index), the index shuffles through
 dr_take_long_axis / dr_exclude_adjust, the metric through dr_rowwise_dot / dr_column_rank.
 
@@ -209,7 +209,7 @@ class Faiss(TopK):
     """The reference wraps the third-party faiss ANN library here (:337-461); outside this build's path."""
 
     def __init__(self, *args, **kwargs):
-        raise NotImplementedError("Faiss index: third-party ANN library, outside the B200 hot path (SURVEY.md 8f); "
+        raise NotImplementedError("Faiss index: third-party ANN library, outside the CUDA hot path (SURVEY.md 8f); "
                                   "use BruteForce or Streaming")
 
     def index(self, candidates, identifiers=None):   # pragma: no cover

@@ -311,7 +311,7 @@ class InBatchSoftmax(torch.autograd.Function):
         loss = torch.empty((1,), device=q.device, dtype=torch.float32)
         ws = None
         if nq * nc >= SOFTMAX_TC_MIN_SCORES and D >= 32:
-            # tensor-core form: score blocks through the tcgen05 GEMM, kept in a scratch buffer for the backward
+            # tensor-core form: score blocks through the wgmma GEMM, kept in a scratch buffer for the backward
             rows = min(nq, max(128, SOFTMAX_TC_WS_BYTES // (4 * nc) // 128 * 128))
             ws = torch.empty((rows, nc), device=q.device, dtype=torch.float32)
             check(lib.dr_inbatch_softmax_fwd_ws(q.data_ptr(), c.data_ptr(), _ptr(w), _ptr(p), _ptr(ids), float(inv_tau),

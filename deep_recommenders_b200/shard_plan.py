@@ -1,6 +1,6 @@
 """Pure-Python partition arithmetic of the row-sharded embedding tables (SURVEY.md section 8e).
 
-The reference is single-process; this is the B200 design: all S tables of a model share one
+The reference is single-process; this is the multi-GPU design: all S tables of a model share one
 global row space (row = slot_offset[s] + id), row r is owned by rank r mod G and stored at local
 index r div G.  Shared by the CUDA path (sharded.py) and the gloo CPU protocol tests.
 """

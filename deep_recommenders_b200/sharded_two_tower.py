@@ -84,7 +84,7 @@ class ShardedTwoTowerTrainStep:
         self.gc_rot = torch.empty((G * b, D), **f)
         self.gc_all = torch.empty((G, b, D), **f)
         self.gc_local = torch.empty((b, D), **f)
-        # scores of this rank's b queries against all G b candidates: tcgen05 form when the block is big enough to pay
+        # scores of this rank's b queries against all G b candidates: tensor-core form when the block is big enough to pay
         from . import ops as _ops
         big = b * G * b >= _ops.SOFTMAX_TC_MIN_SCORES and D >= 32 and b * G * b * 4 <= _ops.SOFTMAX_TC_WS_BYTES
         self.scores_ws = torch.empty((b, G * b), **f) if big else None

@@ -1,5 +1,5 @@
 /*
- * deeprec_b200.h -- C-ABI of the B200-native hot path of deep_recommenders.
+ * deeprec_b200.h -- C-ABI of the CUDA-native (H100, sm_90a) hot path of deep_recommenders.
  *
  * One shared library (libdeeprec_b200.so), extern "C", plain pointers and sizes,
  * no torch / C++ types.  The reference (LongmaoTeamTf/deep_recommenders) has no FFI at
@@ -98,12 +98,11 @@ int dr_embed_fm_bwd(const void* ids, int id_bytes, const int64_t* rows,
                     float scale, void* stream);
 
 /* Opt-in variant of dr_embed_fm_fwd that stages the rows THROUGH TMA INTO SHARED MEMORY
- * (cp.async.bulk.tensor ... tile::gather4, four rows per instruction, mbarrier completion; the stacked rows leave as one
+ * (one cp.async.bulk copy per looked-up row, mbarrier completion; the stacked rows leave as one
  * cp.async.bulk store per tile).  Same outputs as dr_embed_fm_fwd (stack bit-exact; logit / sum_e up to summation order).
  * Serves the fused row layout only: all tables in ONE arena `arena` [total_rows, row_stride] with the first-order weight
  * at float D of the row (DR_EMBED_LIN_IN_ROW), D = 16, S <= 32; slot_offsets[s] = first arena row of table s.
- * Returns DR_ENOTSUP otherwise.  Measured slower than the register-load kernel for uniform and for Zipf ids on B200
- * (DESIGN.md section 4): shipped as the measured alternative, not as the default. */
+ * Returns DR_ENOTSUP otherwise.  Shipped as the alternative to measure against, not as the default. */
 int dr_embed_fm_fwd_tma(const float* arena, int64_t total_rows, const int64_t* slot_offsets,
                         const int64_t* rows, const void* ids, int id_bytes, const float* bias, int64_t B, int S,
                         int D, int64_t row_stride, float* out_stack, float* out_sum, float* out_logit,
@@ -193,7 +192,7 @@ int dr_inbatch_softmax_bwd(const float* q, const float* c, const float* w, const
                            const float* lse, const float* gloss,
                            float* gq, float* gc, void* stream);
 
-/* Tensor-core form of the same loss (the contraction of sbcnm.py:129 and both gradient contractions on the tcgen05
+/* Tensor-core form of the same loss (the contraction of sbcnm.py:129 and both gradient contractions on the wgmma
  * 3xTF32 GEMM core).  scores_ws: caller-provided scratch [ws_rows, nc] floats; query rows are processed in blocks of
  * ws_rows (ws_rows >= nq: one block).  Same arguments, results and reduction as dr_inbatch_softmax_fwd / _bwd.
  * bwd: scores_valid != 0 and ws_rows >= nq means scores_ws still holds what the forward of the SAME inputs left there
@@ -242,7 +241,7 @@ int dr_shard_bucket_ids(const void* ids, int id_bytes, int64_t n, int S,
                         const int64_t* slot_offsets, const int64_t* rows, int G, int64_t cap,
                         int64_t* send_counts, int64_t* send_ids, int32_t* inv, int32_t* overflow,
                         void* stream);
-/* Row-sharded gather / update fused with the exchange over NVLink peer memory (the B200 path for
+/* Row-sharded gather / update fused with the exchange over NVLink peer memory (the multi-GPU path for
  * N > 1).  peer_bases[world] (device array): base of every rank's arena, mapped into this process
  * (CUDA IPC / symmetric memory); all ranks use the same row_stride.  Lookup (s, id) reads global
  * row slot_offsets[s] + id from rank (row mod world) at local row (row div world) -- the LDG.128
@@ -491,12 +490,6 @@ int dr_gemm_plane_cache(int enable);
 int dr_tune_set(const char* key, int value);
 /* Developer hook: read a knob back (tc_pair, tc_dw_share, gemm_variant, gemm_bn, tc_min_n); DR_EINVAL for other keys. */
 int dr_tune_get(const char* key, int* value);
-/* Developer hook: per-role wait cycles of the tcgen05 GEMM core, accumulated over the launches made while the knob
- * `gemm_prof` is 1 (instrumented instantiation: BN = 128, split in kernel).  out16 (HOST pointer, 16 counters):
- * 0 producer waits for a free stage, 1 splitter waits for TMA data, 2 splitter work, 3 MMA issuer waits for operands,
- * 4 MMA issuer waits for a free accumulator, 5 epilogue waits for the accumulator, 6 epilogue work, 7 kernel span,
- * 8 CTAs, 9 k-blocks issued (cycles of one thread per role, summed over CTAs).  reset != 0 clears the counters.  */
-int dr_gemm_prof_read(uint64_t* out16, int reset);
 
 /* Developer hook: C[M,N] = op(A) @ op(B); transA: A stored [K,M]; transB: B stored [N,K].  */
 int dr_debug_gemm(const float* A, const float* B, float* C, int64_t M, int64_t N, int64_t K,

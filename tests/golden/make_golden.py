@@ -1,9 +1,9 @@
 """Generates tests/golden/hotpath_golden_{f32,f64}.npz by EXECUTING THE REFERENCE'S OWN SOURCE FILES
-(read from /root/reference, never copied) under the numpy-backed `tensorflow` stand-in in
-oracle/tf_shim.  Run here (the CPU container); the .npz files are committed and travel to the GPU
-box, /root/reference does not.
+(read from a checkout of the reference, never copied) under the numpy-backed `tensorflow` stand-in in
+oracle/tf_shim.  Nothing calls this script: the .npz files are committed, and the tests read only them.
+Run it by hand, on any machine (no GPU needed), when the oracle's pins have to be regenerated:
 
-    python tests/golden/make_golden.py
+    DR_REFERENCE=<checkout of LongmaoTeamTf/deep_recommenders> python tests/golden/make_golden.py
 
 What executes from the reference:
   keras/models/ranking/fm.py        FM.call (:23-37), FactorizationMachine.call (:54-63)
@@ -26,7 +26,9 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REFERENCE = os.environ.get("DR_REFERENCE", "/root/reference")
+REFERENCE = os.environ.get("DR_REFERENCE")
+if not REFERENCE or not os.path.isdir(os.path.join(REFERENCE, "deep_recommenders")):
+    raise SystemExit("make_golden.py: set DR_REFERENCE to a checkout of the reference repository")
 sys.path.insert(0, os.path.join(ROOT, "oracle", "tf_shim"))
 sys.path.insert(0, REFERENCE)
 sys.dont_write_bytecode = True

@@ -15,10 +15,9 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(autouse=True, params=["ffma", "tc", "tc2", "tc2pair"])
 def gemm_variant(request):
-    """Every test in this file runs under all GEMM cores: FFMA, tcgen05 3xTF32 on pre-split planes (tc) and
-    tcgen05 3xTF32 with the hi/lo split inside the kernel (tc2 = library defaults: at these small sizes the selection rule
-    mostly picks the single-CTA kernel; tc2pair forces the CTA-pair kernel `tcgen05.mma.cta_group::2` for every output at
-    least 128 wide; the full-size file also forces the single-CTA kernel where the default is the pair)."""
+    """Every test in this file runs under all GEMM cores: FFMA, wgmma 3xTF32 on pre-split planes (tc) and
+    wgmma 3xTF32 with the hi/lo split inside the kernel (tc2 = library defaults; tc2pair sets the `tc_pair` knob, which
+    selects nothing on H100 -- there is one wgmma kernel -- and must leave every result unchanged)."""
     from deep_recommenders_b200 import _lib
     pair_default = _lib.tune_get("tc_pair")
     if request.param == "tc":

@@ -1,6 +1,6 @@
 """Rows D and X at BASELINE.json's FULL sizes (C2: M = 65536, C3: M = 131072) through the C-ABI against the float64
 oracle.  These are the shapes the small cases of test_gpu_dense_cross.py never reach: the persistent multi-tile
-schedule of the tcgen05 core, the TMEM double-buffer phase wrap (hundreds of tiles per CTA) and split-K weight
+schedule of the wgmma core, the mbarrier phase wrap of its two rings (hundreds of tiles per CTA) and split-K weight
 gradients with K = M = 65536 / 131072.
 
 The check is mask-consistent: the ReLU mask the backward uses is the one of the GPU's own forward output `y`
@@ -32,9 +32,9 @@ def _sample_rows(M, n, rng):
 
 @pytest.fixture(params=["tc2", "tc", "ffma", "tc2share", "tc2single", "tc2pair"])
 def gemm_core(request):
-    """tc2 = the shipped core under the library defaults; tc2single / tc2pair force the single-CTA kernel / the CTA-pair
-    kernel (tcgen05.mma.cta_group::2, 256 x BN tiles over two SMs); tc2share = the co-residency build of the
-    weight-gradient GEMM (knob tc_dw_share: registers capped at 96, one epilogue staging slab)."""
+    """tc2 = the shipped core under the library defaults; tc2single / tc2pair set the `tc_pair` knob (it selects nothing
+    on H100, results must not change); tc2share = the weight-gradient GEMM with the shorter raw operand ring (knob
+    tc_dw_share)."""
     from deep_recommenders_b200 import _lib
     pair_default = _lib.tune_get("tc_pair")
     if request.param == "tc":

@@ -308,3 +308,32 @@ def test_train_step_dw_first_with_shared_sm_gemm_equals_default(use_graph):
     assert torch.allclose(m1.embeddings.weight, m2.embeddings.weight, rtol=1e-5, atol=1e-7)
     for a, b in zip(t1.w + t1.b, t2.w + t2.b):          # (the flat buffer has uninitialised 16-B padding between them)
         assert torch.allclose(a, b, rtol=1e-5, atol=1e-7)
+
+
+def test_bench_dump_outputs_is_reproducible(tmp_path):
+    """`bench.py --dump-outputs DIR` writes the last timed step's outputs as float32 arrays, and two runs with the same
+    arguments see the same inputs: their dumps agree up to the summation order of the atomics."""
+    import os
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    dumps = []
+    for run in ("a", "b"):
+        d = tmp_path / run
+        r = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--gpus", "1", "--steps", "3", "--warmup", "3",
+                            "--no-cpu-baseline", "--dump-outputs", str(d)], capture_output=True, text=True, timeout=900,
+                           cwd=str(tmp_path))
+        assert r.returncode == 0, r.stderr[-2000:]
+        import json
+        assert json.loads(r.stdout.strip().splitlines()[-1])["steps"] == 3
+        dumps.append({f[:-4]: np.load(d / f) for f in sorted(os.listdir(d))})
+    a, b = dumps
+    assert set(a) == set(b) == {"loss", "prob", "tower", "embedding_rows_sample"}
+    assert a["loss"].shape == (1,) and a["prob"].shape == (65536,)
+    total = 0
+    for name in a:
+        assert a[name].dtype == np.float32 and np.isfinite(a[name]).all(), name
+        assert np.abs(a[name] - b[name]).max() <= 1e-5 * np.abs(a[name]).max() + 1e-7, name
+        total += a[name].nbytes
+    assert total <= 64 << 20
+    assert np.abs(a["embedding_rows_sample"]).max() > 0 and 0.0 <= a["prob"].min() and a["prob"].max() <= 1.0

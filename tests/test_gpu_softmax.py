@@ -152,7 +152,7 @@ def test_full_size_c4_properties():
     (64, 130, 32, None, False, True, False, 2 << 30),
 ])
 def test_inbatch_softmax_tensor_core_form(nq, nc, D, tau, use_w, use_p, use_ids, ws_bytes):
-    """The tcgen05 form (dr_inbatch_softmax_fwd_ws / _bwd_ws: score blocks through the 3xTF32 GEMM core) against the
+    """The tensor-core form (dr_inbatch_softmax_fwd_ws / _bwd_ws: score blocks through the 3xTF32 GEMM core) against the
     float64 oracle and against the fused FFMA kernels -- forced on at sizes the default heuristic gives to the latter."""
     from deep_recommenders.keras.models.retrieval import sbcnm
     from deep_recommenders_b200 import ops

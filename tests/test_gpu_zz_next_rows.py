@@ -762,7 +762,6 @@ def test_retrieval_classes_reproduce_the_reference_source_golden():
         assert np.allclose(m.result(), g[f"metric_{tag}"], rtol=1e-6)
 
 
-# ---- written at the end of round 1; first run on a B200 in round 2 (profiles/r02_unverified_tests.log: 175 passed) --------
 import os as _os
 
 @pytest.mark.parametrize("temperature,accidental", [(None, False), (0.5, True)])

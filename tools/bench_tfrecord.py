@@ -1,6 +1,6 @@
 """Host-side throughput of the native TFRecord / tf.train.Example reader (csrc/tfrecord.cu) on MovieLens-shaped
 records (datasets/movielens.py:54-62 schema), against parsing the same records with the protobuf library's Python
-API.  CPU only.  Writes profiles/tfrecord_parse_r01.json when run with --save."""
+API.  CPU only.  Prints one JSON line."""
 import json
 import os
 import sys
@@ -71,9 +71,6 @@ def main():
     except Exception as e:      # pragma: no cover
         out["protobuf_python_records_per_s"] = f"unavailable: {e}"
     print(json.dumps(out))
-    if "--save" in sys.argv:
-        json.dump(out, open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles",
-                                         "tfrecord_parse_r01.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":

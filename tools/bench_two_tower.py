@@ -5,7 +5,6 @@ on 1..8 GPUs with the row-sharded step (deep_recommenders_b200/sharded_two_tower
 
 (N = 1: `python tools/bench_two_tower.py`.)  Timing: CUDA events around K steps after W warm-ups, barrier + synchronize
 on both sides, MAX over ranks; rank 0 prints one JSON line.  Strong scaling in the batch (b = 16384 / N per GPU).
-First run: round 2 (profiles/bench_n*_r02*_c4.json).
 """
 import json
 import os
@@ -75,7 +74,7 @@ def main():
                           "scaling": "strong", "dtype": "f32", "data": "synthetic",
                           "config": {"workload": f"C4 two-tower: {U} users, {I} items, D={D}, global batch {Bg} ({b} per GPU), "
                                                  "embedding towers, SGD, row-sharded tables",
-                                     "softmax_core": "tcgen05 3xTF32 (score block in scratch)" if st.scores_ws is not None
+                                     "softmax_core": "wgmma 3xTF32 (score block in scratch)" if st.scores_ws is not None
                                      else "fused FFMA (scores never materialised)"},
                           "kernel_ms": phases, "global_loss": float(loss)}), flush=True)
     dist.destroy_process_group()

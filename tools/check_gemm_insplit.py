@@ -1,4 +1,4 @@
-"""Variant 2 of the tcgen05 GEMM (hi/lo split inside the kernel) against variant 1 (pre-split planes) and fp64,
+"""Variant 2 of the wgmma GEMM (hi/lo split inside the kernel) against variant 1 (pre-split planes) and fp64,
 through the public Dense forward / backward (NN, NT, TN operand layouts, ragged tiles, split-K weight gradient),
 plus timing at the C2 layer shapes.  Exit code 1 on any mismatch.  Writes gpurun_out/check_gemm_insplit.json."""
 import json
@@ -15,7 +15,6 @@ from check_gemm_tc import run  # noqa: E402
 
 def main():
     _lib.enable_tensor_core_gemm(3 << 30)
-    _lib.tune("tc_mn", 1)
     ok, out = True, []
     shapes = [(256, 64, 128), (300, 96, 200), (1000, 416, 256), (4096, 256, 416), (65536, 416, 256), (65536, 256, 256)]
     for M, K, N in shapes:

@@ -1,4 +1,4 @@
-"""Correctness + timing of the tcgen05 3xTF32 GEMM variant against the FFMA variant and an fp64
+"""Correctness + timing of the wgmma 3xTF32 GEMM variant against the FFMA variant and an fp64
 reference, through the public Dense forward/backward (NN, NT and TN operand layouts)."""
 import json
 import os
@@ -51,7 +51,6 @@ def run(M, K, N, variant, act=1, iters=0):
 
 def main():
     _lib.enable_tensor_core_gemm(3 << 30)
-    _lib.tune("tc_mn", int(os.environ.get("DR_TC_MN", "1")))
     out = []
     shapes = [(256, 64, 128), (300, 96, 200), (1000, 416, 256), (4096, 256, 416), (65536, 416, 256), (65536, 256, 256),
               (131072, 832, 832)]

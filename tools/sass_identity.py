@@ -1,6 +1,6 @@
 """Are the kernels at HEAD the same machine code as at <commit>?  (developer tool, no GPU needed)
 
-Compiles csrc/<file>.cu of both trees for sm_100a and compares the SASS of every kernel the old tree defines,
+Compiles csrc/<file>.cu of both trees for sm_90a and compares the SASS of every kernel the old tree defines,
 instruction by instruction (addresses and encodings stripped).  Template parameters appended since then are matched
 by trying the old mangled name with `Lb0E` (= false) inserted for each added bool.  Used at the end of round 1, after
 the GPU budget was spent, to show that the host-side / opt-in changes made after the last GPU-verified commit left
@@ -16,7 +16,7 @@ import sys
 import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr"]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr"]
 
 
 def compile_tree(src_dir, inc_dir, name, out):
