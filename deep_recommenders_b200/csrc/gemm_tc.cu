@@ -38,8 +38,10 @@ static size_t g_ws_bytes = 0;
 
 // Plane cache (dr_gemm_plane_cache, variant 1): inside a train step every tensor is split into its TF32 hi/lo
 // planes ONCE per layout and the planes are shared by all the GEMMs that read it (x: forward and dW; gz: dX and
-// dW; W: forward and dX).  Off by default: without it every GEMM call splits its own operands.
-struct PlaneEntry { const float* src; size_t elems; bool transposed; float* hi; float* lo; int64_t pitch; };
+// dW; W: forward and dX).  Off by default: without it every GEMM call splits its own operands.  An entry is keyed by
+// the whole view it was split from (pointer, layout, rows, K, pitch): one pointer read as [128, 64] and as [64, 128],
+// or with K = 33 and K = 36 (same plane pitch), has other planes.
+struct PlaneEntry { const float* src; bool transposed; int64_t rows, K, ld; float* hi; float* lo; int64_t pitch; };
 static PlaneEntry g_planes[64];
 static int g_nplanes = 0;
 static bool g_cache_on = false;
@@ -481,10 +483,12 @@ static void plane_elems(const GemmArgs& a, bool ta, bool tb, size_t* ae, size_t*
   *be = (size_t)a.N * (size_t)(tb ? a.ldb : kp);
 }
 
-static bool plane_cached(const float* src, size_t elems, bool transposed) {
-  for (int i = 0; i < g_nplanes; ++i)
-    if (g_planes[i].src == src && g_planes[i].elems == elems && g_planes[i].transposed == transposed) return true;
-  return false;
+static const PlaneEntry* plane_cached(const float* src, bool transposed, int64_t rows, int64_t K, int64_t ld) {
+  for (int i = 0; i < g_nplanes; ++i) {
+    const PlaneEntry& e = g_planes[i];
+    if (e.src == src && e.transposed == transposed && e.rows == rows && e.K == K && e.ld == ld) return &e;
+  }
+  return nullptr;
 }
 
 bool gemm_tc_eligible(const GemmArgs& a, bool ta, bool tb) {
@@ -500,8 +504,8 @@ bool gemm_tc_eligible(const GemmArgs& a, bool ta, bool tb) {
   size_t ae, be;
   plane_elems(a, ta, tb, &ae, &be);
   size_t need = 0;
-  if (!(g_cache_on && plane_cached(a.A, ae, ta))) need += 2 * ae;
-  if (!(g_cache_on && plane_cached(a.B, be, !tb))) need += 2 * be;
+  if (!(g_cache_on && plane_cached(a.A, ta, a.M, a.K, a.lda))) need += 2 * ae;
+  if (!(g_cache_on && plane_cached(a.B, !tb, a.N, a.K, a.ldb))) need += 2 * be;
   return ((g_cache_on ? g_bump : 0) + need) * sizeof(float) <= g_ws_bytes;
 }
 
@@ -597,18 +601,18 @@ int gemm_tc_launch(const GemmArgs& a0, bool ta, bool tb, cudaStream_t st) {
   auto planes = [&](const float* src, size_t elems, bool transposed, int64_t rows, int64_t ld, float** hi, float** lo,
                     int64_t* pitch) -> int {
     if (g_cache_on)
-      for (int i = 0; i < g_nplanes; ++i)
-        if (g_planes[i].src == src && g_planes[i].elems == elems && g_planes[i].transposed == transposed) {
-          *hi = g_planes[i].hi; *lo = g_planes[i].lo; *pitch = g_planes[i].pitch;
-          return DR_OK;
-        }
+      if (const PlaneEntry* e = plane_cached(src, transposed, rows, a.K, ld)) {
+        *hi = e->hi; *lo = e->lo; *pitch = e->pitch;
+        return DR_OK;
+      }
     DR_REQUIRE(g_ws_ptr && (g_bump + 2 * elems) * sizeof(float) <= g_ws_bytes, DR_EINVAL,
                "gemm_tc: workspace exhausted (%zu B registered)", g_ws_bytes);
     *hi = reinterpret_cast<float*>(g_ws_ptr) + g_bump;
     *lo = *hi + elems;
     g_bump += 2 * elems;
     if (int rc = make_planes(src, !transposed, rows, a.K, ld, *hi, *lo, pitch, st)) return rc;
-    if (g_cache_on && g_nplanes < 64) g_planes[g_nplanes++] = PlaneEntry{src, elems, transposed, *hi, *lo, *pitch};
+    if (g_cache_on && g_nplanes < 64)
+      g_planes[g_nplanes++] = PlaneEntry{src, transposed, rows, a.K, ld, *hi, *lo, *pitch};
     return DR_OK;
   };
   float *Ah, *Al, *Bh, *Bl;
