@@ -11,3 +11,11 @@ The top-level `deep_recommenders` package in this repo is an import alias of thi
 reference's import lines work unchanged.
 """
 __version__ = "0.1.0"
+
+
+def __getattr__(name):
+    # the whole-step trainers, resolved on first use (importing the package stays free of torch)
+    if name == "DCNTrainStep":
+        from .dcn_training import DCNTrainStep
+        return DCNTrainStep
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

@@ -47,6 +47,7 @@ _SIGS = {
     "dr_dense_bwd_chain": [_p, _p, _p, _p, _i64, _i, _i, _i, _p, _p, _p, _p, _p, _i, _p],
     "dr_cross_fwd": [_p, _p, _p, _p, _p, _p, _f, _i64, _i, _i, _p, _p, _p, _p],
     "dr_cross_bwd": [_p, _p, _p, _p, _p, _f, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p],
+    "dr_cross_bwd_acc": [_p, _p, _p, _p, _p, _f, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p],
     "dr_inbatch_softmax_fwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p],
     "dr_inbatch_softmax_bwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p, _p, _p],
     "dr_inbatch_softmax_fwd_ws": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _i64, _p, _p, _p],
@@ -59,6 +60,7 @@ _SIGS = {
     "dr_sgd_step": [_p, _p, _i64, _f, _p],
     "dr_bce_logits_fwd_bwd": [_p, _p, _p, _i64, _p, _p, _p, _p],
     "dr_dense_head_bce_fwd_bwd": [_p, _p, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p],
+    "dr_dcn_head_bce_fwd_bwd": [_p, _p, _p, _p, _p, _i64, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p],
     # SURVEY 8(f) "next" rows
     "dr_adam_step": [_p, _p, _p, _p, _i64, _f, _f, _f, _f, _i, _p, _p],
     "dr_adam_advance": [_p, _f, _f, _f, _p, _p],

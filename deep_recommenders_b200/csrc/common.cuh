@@ -136,6 +136,13 @@ __device__ __forceinline__ float4 f4_shfl_down(float4 v, int delta) {
                      __shfl_down_sync(0xffffffffu, v.z, delta), __shfl_down_sync(0xffffffffu, v.w, delta));
 }
 
+// V consecutive floats moved as one access: V = 4 is a 128-bit load / store (16-B aligned address), V = 1 the scalar
+// form of the same kernel for shapes that are not a multiple of 4 wide.
+template <int V>
+struct alignas(4 * V) Vec {
+  float v[V];
+};
+
 __device__ __forceinline__ float act_apply(float v, int act) {
   switch (act) {
     case DR_ACT_RELU: return fmaxf(v, 0.f);

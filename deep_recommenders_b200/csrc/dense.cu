@@ -158,7 +158,68 @@ __global__ void __launch_bounds__(256) cross_bwd_prologue_kernel(const float* __
   }
 }
 
-int g_tune_tc_dw_stages = 0;   // 2: weight-gradient GEMMs use the two-stage ring (co-residency with the embedding update)
+// The same prologue for a caller that builds the x0 gradient in place (dr_cross_bwd_acc): h = g*x0 ; gx0 += g*u ;
+// gb[n] += sum_m h[m,n].  V = 4 when every row is 16-B aligned and d % 4 == 0 (N = d / 4 columns of Vec<4>), else V = 1.
+// blockDim = (32, 8): a warp reads 32 consecutive columns of a row (512 B at V = 4), four rows in flight per thread.
+template <int V>
+__global__ void __launch_bounds__(256) cross_bwd_prologue_acc_kernel(const Vec<V>* __restrict__ g,
+                                                                      const Vec<V>* __restrict__ x0,
+                                                                      const Vec<V>* __restrict__ u, int64_t M, int64_t N,
+                                                                      int64_t rows_per_cta, Vec<V>* __restrict__ h,
+                                                                      Vec<V>* __restrict__ gx0, float* __restrict__ gb) {
+  __shared__ Vec<V> part[8][33];
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  const int64_t r0 = (int64_t)blockIdx.x * rows_per_cta;
+  const int64_t r1 = min(M, r0 + rows_per_cta);
+  constexpr int R = 4;
+  for (int64_t nb = 0; nb < N; nb += 32) {
+    const int64_t n = nb + tx;
+    Vec<V> acc = {};
+    if (n < N) {
+      for (int64_t r = r0 + ty; r < r1; r += 8 * R) {
+        Vec<V> gv[R], xv[R], uv[R], ov[R];
+#pragma unroll
+        for (int i = 0; i < R; ++i) {
+          const int64_t o = (r + 8 * i) * N + n;
+          if (r + 8 * i < r1) {
+            gv[i] = g[o];
+            xv[i] = x0[o];
+            if (gx0) { uv[i] = u[o]; ov[i] = gx0[o]; }
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < R; ++i) {
+          const int64_t o = (r + 8 * i) * N + n;
+          if (r + 8 * i < r1) {
+            Vec<V> hv;
+#pragma unroll
+            for (int e = 0; e < V; ++e) {
+              hv.v[e] = gv[i].v[e] * xv[i].v[e];
+              acc.v[e] += hv.v[e];
+              if (gx0) ov[i].v[e] += gv[i].v[e] * uv[i].v[e];
+            }
+            h[o] = hv;
+            if (gx0) gx0[o] = ov[i];
+          }
+        }
+      }
+    }
+    part[ty][tx] = acc;
+    __syncthreads();
+    if (ty == 0 && n < N && gb) {
+#pragma unroll
+      for (int e = 0; e < V; ++e) {
+        float t = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) t += part[i][tx].v[e];
+        red_add_f32(gb + n * V + e, t);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+int g_tune_tc_dw_stages = 0;  // 2: weight-gradient GEMMs use the two-stage ring (co-residency with the embedding update)
 int g_tune_tc_dw_share = 0;    // 1: weight-gradient GEMMs use the co-residency build (capped registers, smaller staging)
 
 static int64_t rows_per_cta_for(int64_t M) {
@@ -338,6 +399,59 @@ extern "C" int dr_cross_bwd(const float* x0, const float* x, const float* w, con
   if (int rc = gemm_launch(a1, false, true, st)) return rc;
   if (int rc = gemm_xt_g(x, t_ws, guk, B, d, r, st)) return rc;                    // gU = x^T t
   GemmArgs a2 = mk(t_ws, uk, gx, B, d, r, r, r, d, EPI_CROSS_DX);                  // gx = t @ U^T + ...
+  a2.alpha = alpha; a2.aux0 = h_ws; a2.aux1 = g;
+  return gemm_launch(a2, false, true, st);
+}
+
+extern "C" int dr_cross_bwd_acc(const float* x0, const float* x, const float* w, const float* uk, const float* vk,
+                                float alpha, const float* u_saved, const float* xu_saved, const float* g, int64_t B,
+                                int d, int r, float* h_ws, float* t_ws, float* gx0, float* gx, float* gw, float* guk,
+                                float* gvk, float* gb, int x_is_x0, void* stream) {
+  DR_REQUIRE(x0 && x && g && h_ws, DR_EINVAL, "dr_cross_bwd_acc: null pointer");
+  DR_REQUIRE(B >= 0 && d >= 1 && r >= 0, DR_EINVAL, "dr_cross_bwd_acc: bad shape");
+  DR_REQUIRE(!gx0 || u_saved, DR_EINVAL, "dr_cross_bwd_acc: gx0 requested but u_saved is NULL");
+  if (x_is_x0)
+    DR_REQUIRE(gx0 && x == x0, DR_EINVAL, "dr_cross_bwd_acc: x_is_x0 needs gx0 and x == x0");
+  else
+    DR_REQUIRE(gx, DR_EINVAL, "dr_cross_bwd_acc: gx is NULL (only the x_is_x0 form accumulates it into gx0)");
+  if (r == 0)
+    DR_REQUIRE(w && gw, DR_EINVAL, "dr_cross_bwd_acc: full-rank needs W and gW");
+  else
+    DR_REQUIRE(uk && vk && guk && gvk && xu_saved && t_ws, DR_EINVAL, "dr_cross_bwd_acc: low-rank operands missing");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (gb) DR_CUDA_CALL(cudaMemsetAsync(gb, 0, sizeof(float) * d, st));
+  if (B == 0) return DR_OK;
+  {
+    const int64_t rpc = rows_per_cta_for(B);
+    const int64_t ctas = (B + rpc - 1) / rpc;
+    const bool vec = (d & 3) == 0 && aligned16(g) && aligned16(x0) && aligned16(h_ws) &&
+                     (!gx0 || (aligned16(u_saved) && aligned16(gx0)));
+    if (vec) {
+      using V4 = Vec<4>;
+      cross_bwd_prologue_acc_kernel<4><<<(unsigned)ctas, dim3(32, 8), 0, st>>>(
+          reinterpret_cast<const V4*>(g), reinterpret_cast<const V4*>(x0), reinterpret_cast<const V4*>(u_saved), B, d / 4,
+          rpc, reinterpret_cast<V4*>(h_ws), reinterpret_cast<V4*>(gx0), gb);
+    } else {
+      using V1 = Vec<1>;
+      cross_bwd_prologue_acc_kernel<1><<<(unsigned)ctas, dim3(32, 8), 0, st>>>(
+          reinterpret_cast<const V1*>(g), reinterpret_cast<const V1*>(x0), reinterpret_cast<const V1*>(u_saved), B, d, rpc,
+          reinterpret_cast<V1*>(h_ws), reinterpret_cast<V1*>(gx0), gb);
+    }
+    DR_CUDA_LAUNCH_CHECK("cross_bwd_prologue_acc");
+  }
+  float* dx = x_is_x0 ? gx0 : gx;                        // bottom layer of a stack: x IS x0, one gradient buffer
+  const int epi = x_is_x0 ? EPI_CROSS_DX_ACC : EPI_CROSS_DX;
+  if (r == 0) {
+    GemmArgs a = mk(h_ws, w, dx, B, d, d, d, d, d, epi);                           // gx (+)= h @ W^T + alpha*h + g
+    a.alpha = alpha; a.aux0 = h_ws; a.aux1 = g;
+    if (int rc = gemm_launch(a, false, true, st)) return rc;
+    return gemm_xt_g(x, h_ws, gw, B, d, d, st);
+  }
+  if (int rc = gemm_xt_g(xu_saved, h_ws, gvk, B, r, d, st)) return rc;             // gV = (xU)^T h
+  GemmArgs a1 = mk(h_ws, vk, t_ws, B, r, d, d, d, r, EPI_STORE);                   // t = h @ V^T
+  if (int rc = gemm_launch(a1, false, true, st)) return rc;
+  if (int rc = gemm_xt_g(x, t_ws, guk, B, d, r, st)) return rc;                    // gU = x^T t
+  GemmArgs a2 = mk(t_ws, uk, dx, B, d, r, r, r, d, epi);                           // gx (+)= t @ U^T + ...
   a2.alpha = alpha; a2.aux0 = h_ws; a2.aux1 = g;
   return gemm_launch(a2, false, true, st);
 }

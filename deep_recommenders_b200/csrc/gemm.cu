@@ -48,8 +48,10 @@ __device__ __forceinline__ float epi_scalar(const GemmArgs& a, float acc, int64_
   }
 }
 
-template <int BM, int BN, int BK, int TM, int TN, bool TA, bool TB>
-__global__ void __launch_bounds__(256) sgemm_kernel(const GemmArgs a) {
+// ACC (EPI_CROSS_DX_ACC) is a compile-time form with kernels of its own (sgemm_acc_kernel), so that the kernels of every
+// other epilogue compile exactly as they do without it.
+template <int BM, int BN, int BK, int TM, int TN, bool TA, bool TB, bool ACC>
+__device__ __forceinline__ void sgemm_body(const GemmArgs& a) {
   constexpr int NT = 256;
   constexpr int TX = BN / TN, TY = BM / TM;
   static_assert(TX * TY == NT, "thread tile mismatch");
@@ -205,7 +207,14 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const GemmArgs a) {
     for (int v = 0; v < NVN; ++v) {
       const int64_t n = n0 + v * (BN / NVN) + tx * VN;
       if (n >= a.N) continue;
-      if (a.epi == EPI_ATOMIC) {
+      if constexpr (ACC) {
+#pragma unroll
+        for (int e = 0; e < VN; ++e)
+          if (n + e < a.N) {
+            const int64_t off = m * a.ldc + n + e;
+            a.C[off] += acc[i][v * VN + e] + a.alpha * __ldg(a.aux0 + off) + __ldg(a.aux1 + off);
+          }
+      } else if (a.epi == EPI_ATOMIC) {
 #pragma unroll
         for (int e = 0; e < VN; ++e)
           if (n + e < a.N) red_add_f32(a.C + m * a.ldc + n + e, acc[i][v * VN + e]);
@@ -225,10 +234,24 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const GemmArgs a) {
   }
 }
 
+template <int BM, int BN, int BK, int TM, int TN, bool TA, bool TB>
+__global__ void __launch_bounds__(256) sgemm_kernel(const GemmArgs a) {
+  sgemm_body<BM, BN, BK, TM, TN, TA, TB, false>(a);
+}
+
+// EPI_CROSS_DX_ACC: the only GEMM that accumulates into C is the Cross input gradient h @ W^T (A as stored, B transposed).
+template <int BM, int BN, int BK, int TM, int TN>
+__global__ void __launch_bounds__(256) sgemm_acc_kernel(const GemmArgs a) {
+  sgemm_body<BM, BN, BK, TM, TN, false, true, true>(a);
+}
+
 template <int BM, int BN, int BK, int TM, int TN>
 static int launch_cfg(const GemmArgs& a, bool ta, bool tb, cudaStream_t st) {
   dim3 grid((unsigned)((a.M + BM - 1) / BM), (unsigned)((a.N + BN - 1) / BN), (unsigned)a.splitk);
-  if (!ta && !tb) sgemm_kernel<BM, BN, BK, TM, TN, false, false><<<grid, 256, 0, st>>>(a);
+  if (a.epi == EPI_CROSS_DX_ACC) {
+    DR_REQUIRE(!ta && tb, DR_ENOTSUP, "gemm: the accumulating Cross epilogue serves A as stored, B transposed only");
+    sgemm_acc_kernel<BM, BN, BK, TM, TN><<<grid, 256, 0, st>>>(a);
+  } else if (!ta && !tb) sgemm_kernel<BM, BN, BK, TM, TN, false, false><<<grid, 256, 0, st>>>(a);
   else if (!ta && tb) sgemm_kernel<BM, BN, BK, TM, TN, false, true><<<grid, 256, 0, st>>>(a);
   else if (ta && !tb) sgemm_kernel<BM, BN, BK, TM, TN, true, false><<<grid, 256, 0, st>>>(a);
   else sgemm_kernel<BM, BN, BK, TM, TN, true, true><<<grid, 256, 0, st>>>(a);

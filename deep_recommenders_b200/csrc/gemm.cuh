@@ -19,6 +19,8 @@ enum Epi : int {
   EPI_CROSS = 4,      // u = acc + bias[n] + alpha*aux1[m,n]; out2 = u; C = aux0*u + aux1  (aux0=x0, aux1=x)
   EPI_CROSS_DX = 5,   // C = acc + alpha*aux0[m,n] + aux1[m,n]    (aux0 = h, aux1 = g)
   EPI_SCORES = 6,     // C = acc - log(p[n]) + dup(m,n)*MIN_FLOAT  (bias = p or null, ids in aux ptr)
+  EPI_CROSS_DX_ACC = 7,   // C += acc + alpha*aux0[m,n] + aux1[m,n]   (EPI_CROSS_DX accumulated into C; splitk == 1, so each
+                          // element has one owner: a plain load-add-store, no reduction traffic, deterministic)
 };
 
 struct GemmArgs {

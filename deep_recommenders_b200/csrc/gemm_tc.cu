@@ -277,7 +277,9 @@ __device__ __forceinline__ TcItem tc_decode(int64_t item, int64_t n_tiles, int64
 // Fused epilogue of one warpgroup's 64 x BN accumulator.  Fragment layout of wgmma's D: warp w of the warpgroup owns rows
 // 16 w .. 16 w + 15; d[4 j + {0, 1}] are columns 8 j + 2 (lane % 4) + {0, 1} of row lane / 4, d[4 j + {2, 3}] the same
 // columns of row lane / 4 + 8.  Four lanes write one whole 32-B sector of a row.
-template <int BN>
+// ACC (EPI_CROSS_DX_ACC, C += acc + alpha*aux0 + aux1) is a compile-time form with kernels of its own (gemm_tc_acc_kernel),
+// so that the kernels of every other epilogue compile exactly as they do without it.
+template <int BN, bool ACC>
 __device__ __forceinline__ void tc_epilogue(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw, const int64_t n0,
                                             const int lane, const bool vec_ok) {
 #pragma unroll
@@ -290,7 +292,11 @@ __device__ __forceinline__ void tc_epilogue(const GemmArgs& a, const float (&d)[
       if (n >= a.N) continue;
       const float v0 = d[4 * j + 2 * half], v1 = d[4 * j + 2 * half + 1];
       float* c = a.C + m * a.ldc + n;
-      if (a.epi == EPI_ATOMIC) {
+      if constexpr (ACC) {
+        const int64_t off = m * a.ldc + n;
+        c[0] += v0 + a.alpha * __ldg(a.aux0 + off) + __ldg(a.aux1 + off);
+        if (n + 1 < a.N) c[1] += v1 + a.alpha * __ldg(a.aux0 + off + 1) + __ldg(a.aux1 + off + 1);
+      } else if (a.epi == EPI_ATOMIC) {
         red_add_f32(c, v0);
         if (n + 1 < a.N) red_add_f32(c + 1, v1);
       } else if (vec_ok && n + 1 < a.N) {
@@ -305,14 +311,11 @@ __device__ __forceinline__ void tc_epilogue(const GemmArgs& a, const float (&d)[
 
 // Persistent, warp-specialised.  `raw_stages` (run-time: 2 or 3) is the depth of the raw ring; the plane ring is two deep.
 // Shared memory: planes 2 x [Ah | Al | Bh | Bl], then (variant 2) raw_stages x [A raw | B raw].
-template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
-// Registers are allocated to warps in groups of four, so 13 warps count as 16: 65536 / 512 = 128 registers per thread.
-// The BN = 128 instantiations hold 64 accumulators and spill one 4-byte value (8 bytes of stack) at that cap.
-__global__ void __launch_bounds__(TC_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-               const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const GemmArgs a,
-               const int raw_stages, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
-               const int64_t total_items) {
+template <int BN, bool A_MN, bool B_MN, bool PRESPLIT, bool ACC>
+__device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUtensorMap& tmAl, const CUtensorMap& tmBh,
+                                             const CUtensorMap& tmBl, const GemmArgs& a, const int raw_stages,
+                                             const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
+                                             const int64_t total_items) {
   constexpr int A_TILE = TC_BM * TC_BK * 4;   // 16 KB
   constexpr int B_TILE = BN * TC_BK * 4;
   constexpr int PLANE_STAGE = 2 * A_TILE + 2 * B_TILE;
@@ -425,9 +428,30 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
       }
       wgmma_wait<0>();
       mbar_arrive(&pl_empty[(it - 1) % TC_PLANE_STAGES]);
-      tc_epilogue<BN>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane, vec_ok);
+      tc_epilogue<BN, ACC>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane, vec_ok);
     }
   }
+}
+
+// Registers are allocated to warps in groups of four, so 13 warps count as 16: 65536 / 512 = 128 registers per thread.
+// The BN = 128 instantiations hold 64 accumulators and spill one 4-byte value (8 bytes of stack) at that cap.
+template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+               const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const GemmArgs a,
+               const int raw_stages, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
+               const int64_t total_items) {
+  gemm_tc_body<BN, A_MN, B_MN, PRESPLIT, false>(tmAh, tmAl, tmBh, tmBl, a, raw_stages, m_tiles, n_tiles, per, total_items);
+}
+
+// EPI_CROSS_DX_ACC: the only GEMM that accumulates into C is the Cross input gradient h @ W^T, both operands K-major.
+template <int BN, bool PRESPLIT>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_acc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+                   const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const GemmArgs a,
+                   const int raw_stages, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
+                   const int64_t total_items) {
+  gemm_tc_body<BN, false, false, PRESPLIT, true>(tmAh, tmAl, tmBh, tmBl, a, raw_stages, m_tiles, n_tiles, per, total_items);
 }
 
 // ---- host side ---------------------------------------------------------------------------------------
@@ -495,6 +519,7 @@ bool gemm_tc_eligible(const GemmArgs& a, bool ta, bool tb) {
   if (g_tune_gemm_variant != 1 && g_tune_gemm_variant != 2) return false;
   if (a.N < g_tune_tc_min_n || (a.N & 3) || a.M < 64 || a.K < 32) return false;
   if (a.M >= ((int64_t)1 << 31) || a.K >= ((int64_t)1 << 31) || a.N >= ((int64_t)1 << 31)) return false;
+  if (a.epi == EPI_CROSS_DX_ACC && (ta || !tb)) return false;     // accumulate form: K-major operands only (gemm_tc_acc_kernel)
   if (g_tune_gemm_variant == 2)     // in-kernel split: raw operands by TMA, no workspace
     return !((a.lda & 3) || !aligned16(a.A) || (a.ldb & 3) || !aligned16(a.B));
   // operands already K-major are split in place with float4 accesses
@@ -519,6 +544,9 @@ static int launch_tc(const CUtensorMap* tms, const GemmArgs& a, int raw_stages, 
   static_assert((size_t)TC_PLANE_STAGES * PLANE_STAGE + 3 * (PLANE_STAGE / 2) + 1024 + 256 <= 232448,
                 "plane ring + raw ring exceed the 227 KB of shared memory per CTA");
   auto k = gemm_tc_kernel<BN, A_MN, B_MN, PRESPLIT>;
+  if constexpr (!A_MN && !B_MN && BN <= 64) {
+    if (a.epi == EPI_CROSS_DX_ACC) k = gemm_tc_acc_kernel<BN, PRESPLIT>;
+  }
   DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t m_tiles = (a.M + TC_BM - 1) / TC_BM, n_tiles = (a.N + BN - 1) / BN;
   const int64_t kblocks = (a.K + TC_BK - 1) / TC_BK;
@@ -564,6 +592,9 @@ int gemm_tc_launch(const GemmArgs& a0, bool ta, bool tb, cudaStream_t st) {
   // skinny outputs (the 256->32 tower layer and its weight gradient) get a 128 x 32 / 128 x 64 tile
   int bn = a.N <= 32 ? 32 : (a.N <= 64 ? 64 : 128);
   if (g_tune_gemm_bn == 32 || g_tune_gemm_bn == 64) bn = g_tune_gemm_bn;
+  // the accumulating epilogue holds three addresses per element: beside the 64 accumulators of a 128-wide tile it does not
+  // fit the 128-register cap without spilling, so it runs 128 x 64 tiles at most
+  if (a.epi == EPI_CROSS_DX_ACC && bn == 128) bn = 64;
   CUtensorMap tms[4];
   if (g_tune_gemm_variant == 2) {
     // Variant 2: tensor maps straight on the source operands (staged as stored), split in shared memory.

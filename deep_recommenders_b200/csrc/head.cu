@@ -87,6 +87,119 @@ __global__ void __launch_bounds__(256) head_bce_kernel(const float* __restrict__
   }
 }
 
+// The DCN tail: Dense(1) on concat[x_cross, deep] (the stacking of the reference's tests/keras/test_dcn.py:27-32 on top of
+// keras/models/ranking/dcn.py:70-88, plus the deep tower), sigmoid cross-entropy and their backward, WITHOUT the concat:
+// the two feature blocks are read where they lie and their gradients are written where the two backward chains read them.
+//   z_b = x_cross[b,:].w[0:d] + deep[b,:].w[d:d+n] + bias ;  g_b = (sigmoid(z_b) - y_b) / B
+//   g_xc[b,k] = g_b w[k] ;  g_deep[b,j] = g_b w[d+j] act'(deep[b,j]) ;  gw[k] = sum_b feat[b,k] g_b
+// A row (d + n floats, 960 at d = 832, n = 128) does not fit in a warp's registers next to its two column-sum arrays the
+// way head_bce_kernel keeps it, so a CTA walks the batch in tiles of 8 rows (one per warp): phase 1 stages the tile in
+// shared memory while each warp reduces its row's dot product against w (shared); phase 2 turns the threads into column
+// owners (thread t owns columns t, t + 256, ...), which write the gradients of the 8 rows and keep the column sums of
+// gw / gb_deep in shared memory without atomics.  V as in Vec<V>.
+constexpr int DCN_HEAD_ROWS = 8;
+constexpr int DCN_HEAD_MAX_K = 4096;
+
+template <int V>
+__global__ void __launch_bounds__(256) dcn_head_bce_kernel(const float* __restrict__ xc, const float* __restrict__ deep,
+                                                            const float* __restrict__ w, const float* __restrict__ bias,
+                                                            const float* __restrict__ y, int64_t B, int d, int n, int act,
+                                                            float invB, float* __restrict__ logit_out,
+                                                            float* __restrict__ prob, float* __restrict__ loss,
+                                                            float* __restrict__ g_logit, float* __restrict__ g_xc,
+                                                            float* __restrict__ g_deep, float* __restrict__ gw,
+                                                            float* __restrict__ gb, float* __restrict__ gb_deep) {
+  using T = Vec<V>;
+  constexpr int R = DCN_HEAD_ROWS;
+  extern __shared__ __align__(16) float smem[];
+  const int K = d + n, dv = d / V, Kv = K / V;
+  float* s_w = smem;               // [K]
+  float* s_gw = s_w + K;           // [K]     this CTA's partial sum of gw
+  float* s_gbd = s_gw + K;         // [n]     ... of gb_deep
+  float* s_tile = s_gbd + n;       // [R][K]  the rows of the current tile
+  float* s_g = s_tile + R * K;     // [R]     their g_b
+  float* s_misc = s_g + R;         // loss, gb
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int k = threadIdx.x; k < K; k += blockDim.x) { s_w[k] = __ldg(w + k); s_gw[k] = 0.f; }
+  for (int j = threadIdx.x; j < n; j += blockDim.x) s_gbd[j] = 0.f;
+  if (threadIdx.x < 2) s_misc[threadIdx.x] = 0.f;
+  __syncthreads();
+  const float b0 = bias ? __ldg(bias) : 0.f;
+  float loss_acc = 0.f, gb_acc = 0.f;
+  for (int64_t t0 = (int64_t)blockIdx.x * R; t0 < B; t0 += (int64_t)gridDim.x * R) {
+    const int64_t r = t0 + warp;
+    if (r < B) {
+      const T* xr = reinterpret_cast<const T*>(xc + r * d);
+      const T* dr = reinterpret_cast<const T*>(deep + r * n);
+      const T* wv = reinterpret_cast<const T*>(s_w);
+      T* trow = reinterpret_cast<T*>(s_tile + warp * K);
+      float dot = 0.f;
+#pragma unroll 4
+      for (int c = lane; c < Kv; c += 32) {
+        const T f = c < dv ? xr[c] : dr[c - dv];
+        const T ww = wv[c];
+        trow[c] = f;
+#pragma unroll
+        for (int e = 0; e < V; ++e) dot = fmaf(f.v[e], ww.v[e], dot);
+      }
+      dot = group_sum<32>(dot);
+      if (lane == 0) {
+        const float z = dot + b0, yi = __ldg(y + r);
+        const float pr = 1.f / (1.f + expf(-z));
+        const float g = (pr - yi) * invB;
+        loss_acc += fmaxf(z, 0.f) - z * yi + log1pf(expf(-fabsf(z)));
+        gb_acc += g;
+        s_g[warp] = g;
+        if (logit_out) logit_out[r] = z;
+        if (prob) prob[r] = pr;
+        if (g_logit) g_logit[r] = g;
+      }
+    }
+    __syncthreads();
+    const int rows = (int)min((int64_t)R, B - t0);
+    for (int c = threadIdx.x; c < Kv; c += blockDim.x) {
+      const bool is_x = c < dv;
+      const T ww = reinterpret_cast<const T*>(s_w)[c];
+      T gw_acc = {}, gbd_acc = {};
+#pragma unroll
+      for (int i = 0; i < R; ++i) {
+        if (i < rows) {
+          const T f = reinterpret_cast<const T*>(s_tile + i * K)[c];
+          const float g = s_g[i];
+          T o;
+#pragma unroll
+          for (int e = 0; e < V; ++e) {
+            o.v[e] = g * ww.v[e] * (is_x ? 1.f : act_grad_from_y(f.v[e], act));
+            gw_acc.v[e] = fmaf(f.v[e], g, gw_acc.v[e]);
+            gbd_acc.v[e] += o.v[e];
+          }
+          if (is_x) {
+            if (g_xc) reinterpret_cast<T*>(g_xc + (t0 + i) * d)[c] = o;
+          } else if (g_deep) {
+            reinterpret_cast<T*>(g_deep + (t0 + i) * n)[c - dv] = o;
+          }
+        }
+      }
+#pragma unroll
+      for (int e = 0; e < V; ++e) {
+        s_gw[c * V + e] += gw_acc.v[e];
+        if (!is_x) s_gbd[(c - dv) * V + e] += gbd_acc.v[e];
+      }
+    }
+    __syncthreads();
+  }
+  if (lane == 0) { atomicAdd(&s_misc[0], loss_acc); atomicAdd(&s_misc[1], gb_acc); }
+  __syncthreads();
+  for (int k = threadIdx.x; k < K; k += blockDim.x)
+    if (gw) red_add_f32(gw + k, s_gw[k]);
+  for (int j = threadIdx.x; j < n; j += blockDim.x)
+    if (gb_deep) red_add_f32(gb_deep + j, s_gbd[j]);
+  if (threadIdx.x == 0) {
+    red_add_f32(loss, s_misc[0] * invB);
+    if (gb) red_add_f32(gb, s_misc[1]);
+  }
+}
+
 }  // namespace dr
 
 using namespace dr;
@@ -117,5 +230,42 @@ extern "C" int dr_dense_head_bce_fwd_bwd(const float* a, const float* w, const f
   else DR_HEAD(8);
 #undef DR_HEAD
   DR_CUDA_LAUNCH_CHECK("dr_dense_head_bce_fwd_bwd");
+  return DR_OK;
+}
+
+extern "C" int dr_dcn_head_bce_fwd_bwd(const float* x_cross, const float* deep, const float* w, const float* bias,
+                                       const float* y, int64_t B, int d, int n, int deep_act, float* logit_out,
+                                       float* prob_out, float* loss_out, float* g_logit, float* g_xc, float* g_deep,
+                                       float* gw, float* gb, float* gb_deep, void* stream) {
+  DR_REQUIRE(x_cross && deep && w && y && loss_out, DR_EINVAL, "dr_dcn_head_bce_fwd_bwd: null pointer");
+  DR_REQUIRE(B >= 1 && d >= 1 && n >= 1, DR_EINVAL, "dr_dcn_head_bce_fwd_bwd: B=%lld d=%d n=%d (need all >= 1)",
+             (long long)B, d, n);
+  DR_REQUIRE(deep_act >= DR_ACT_NONE && deep_act <= DR_ACT_TANH, DR_EINVAL,
+             "dr_dcn_head_bce_fwd_bwd: unknown activation %d", deep_act);
+  DR_REQUIRE((int64_t)d + n <= DCN_HEAD_MAX_K, DR_ENOTSUP,
+             "dr_dcn_head_bce_fwd_bwd: d + n = %lld, this kernel serves heads up to %d wide", (long long)d + n,
+             DCN_HEAD_MAX_K);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int K = d + n;
+  DR_CUDA_CALL(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
+  if (gw) DR_CUDA_CALL(cudaMemsetAsync(gw, 0, sizeof(float) * K, st));
+  if (gb) DR_CUDA_CALL(cudaMemsetAsync(gb, 0, sizeof(float), st));
+  if (gb_deep) DR_CUDA_CALL(cudaMemsetAsync(gb_deep, 0, sizeof(float) * n, st));
+  int64_t ctas = (B + DCN_HEAD_ROWS - 1) / DCN_HEAD_ROWS;
+  if (ctas > (int64_t)num_sms() * 4) ctas = (int64_t)num_sms() * 4;
+  const float invB = 1.f / (float)B;
+  const size_t smem = sizeof(float) * ((size_t)(2 + DCN_HEAD_ROWS) * K + n + DCN_HEAD_ROWS + 2);
+  const bool vec = (d & 3) == 0 && (n & 3) == 0 && aligned16(x_cross) && aligned16(deep) && aligned16(g_xc) &&
+                   aligned16(g_deep);
+#define DR_DCN_HEAD(V)                                                                                              \
+  do {                                                                                                              \
+    DR_CUDA_CALL(cudaFuncSetAttribute(dcn_head_bce_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    dcn_head_bce_kernel<V><<<(unsigned)ctas, 256, smem, st>>>(x_cross, deep, w, bias, y, B, d, n, deep_act, invB, logit_out, \
+                                                             prob_out, loss_out, g_logit, g_xc, g_deep, gw, gb, gb_deep); \
+  } while (0)
+  if (vec) DR_DCN_HEAD(4);
+  else DR_DCN_HEAD(1);
+#undef DR_DCN_HEAD
+  DR_CUDA_LAUNCH_CHECK("dr_dcn_head_bce_fwd_bwd");
   return DR_OK;
 }

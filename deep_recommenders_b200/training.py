@@ -79,7 +79,116 @@ def fit_host(trainer, batches, depth: int = 2) -> List[float]:
     return losses
 
 
-class DeepFMTrainStep:
+class _WholeStepDriver:
+    """What every whole-step trainer shares once it has `_enqueue(mark)` (the step as raw C-ABI calls on the current
+    stream), `_persistent_state()`, the static `ids` / `labels` buffers, `loss`, `dev`, `use_graph`, `_copy_stream` and
+    `_staged`: CUDA-graph capture and replay, the host-batch pipeline and the per-kernel-group profile."""
+
+    def profile_kernels(self, ids_pool, labels_pool, iters: int = 10):
+        """Eager (non-graph) passes with a CUDA event on the launching stream between kernel groups.
+        Returns ({"embed_fm_fwd_ms": ...}, {label: mean ms}) -- the live per-kernel timing bench.py
+        reports in `roofline` and `kernel_ms`."""
+        runs = []
+        for it in range(iters + 2):      # back-to-back, no host sync in between (steady-state clocks / caches)
+            self.ids.copy_(ids_pool[it % len(ids_pool)], non_blocking=True)
+            self.labels.copy_(labels_pool[it % len(labels_pool)].reshape(-1), non_blocking=True)
+            evs = []
+
+            def mark(label, evs=evs):
+                e = torch.cuda.Event(enable_timing=True)
+                e.record()
+                evs.append((label, e))
+
+            self._enqueue(mark)
+            runs.append(evs)
+        torch.cuda.synchronize()
+        sums, count = {}, 0
+        for evs in runs[2:]:
+            count += 1
+            for (l0, e0), (l1, e1) in zip(evs[:-1], evs[1:]):
+                sums[l1] = sums.get(l1, 0.0) + e0.elapsed_time(e1)
+        shares = {k: v / count for k, v in sums.items()}
+        return {"embed_fm_fwd_ms": shares["embed_fm_fwd"]}, shares
+
+    def capture(self):
+        """Warm up (sets kernel attributes) then record the step into a CUDA graph.
+
+        Side-effect free: the warm-up launch is a real step on whatever the static id / label buffers hold, so every
+        parameter and every piece of optimizer state (Adam clock, m, v, stamps) is snapshotted before it and restored
+        after it -- `capture()` leaves the trainer bit-identical to how it found it."""
+        n0 = _lib.launch_count()
+        with torch.no_grad():
+            state = self._persistent_state()
+            saved = [t.clone() for t in state]
+            s = torch.cuda.Stream(device=self.dev)
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                self._enqueue()
+            torch.cuda.current_stream().wait_stream(s)
+            torch.cuda.synchronize()
+            for t, keep in zip(state, saved):
+                t.copy_(keep)
+            del saved
+        torch.cuda.synchronize()
+        self.launches_per_step = _lib.launch_count() - n0
+        if self.use_graph:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._enqueue()
+            self.graph = g
+        return self
+
+    def run(self):
+        """One step on whatever is in self.ids / self.labels (device resident)."""
+        if self.graph is not None:
+            self.graph.replay()
+        else:
+            self._enqueue()
+
+    def step(self, ids: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
+        """Device-resident inputs: copy into the static buffers (D2D) and run. Returns loss[1]."""
+        self.ids.copy_(ids, non_blocking=True)
+        self.labels.copy_(labels.reshape(-1), non_blocking=True)
+        self.run()
+        return self.loss
+
+    # ---- end-to-end: host buffers in, loss out ---------------------------------------------------
+    def stage_host(self, ids_host: torch.Tensor, labels_host: torch.Tensor):
+        """Start the H2D copy of the NEXT batch on the copy stream into the spare device buffers."""
+        if not hasattr(self, "_spare"):
+            self._spare = (torch.empty_like(self.ids), torch.empty_like(self.labels))
+        with torch.cuda.stream(self._copy_stream):
+            self._spare[0].copy_(ids_host, non_blocking=True)
+            self._spare[1].copy_(labels_host.reshape(-1), non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record()
+        self._staged = ev
+
+    def train_step_host(self, ids_host, labels_host, next_ids_host=None, next_labels_host=None) -> float:
+        """Public end-to-end step.  ids/labels are HOST tensors (pinned for async copies).  If the
+        caller passes the next batch too, its H2D copy overlaps this step's kernels."""
+        cur = torch.cuda.current_stream()
+        if self._staged is None:
+            self.stage_host(ids_host, labels_host)
+        cur.wait_event(self._staged)
+        # swap staged buffers into the static ones the graph reads (D2D, 13.6 MB at C2)
+        self.ids.copy_(self._spare[0], non_blocking=True)
+        self.labels.copy_(self._spare[1], non_blocking=True)
+        done = torch.cuda.Event()
+        done.record(cur)
+        self._staged = None
+        if next_ids_host is not None:
+            self._copy_stream.wait_event(done)
+            self.stage_host(next_ids_host, next_labels_host)
+        self.run()
+        return float(self.loss.item())          # D2H read of the step's result (synchronises)
+
+    def fit_host(self, batches, depth: int = 2) -> List[float]:
+        """Pipelined epoch loop over HOST batches (see module-level fit_host): the public end-to-end call."""
+        return fit_host(self, batches, depth)
+
+
+class DeepFMTrainStep(_WholeStepDriver):
     def __init__(self, model, batch_size: int, lr: float = 0.01, id_dtype=torch.int64, use_graph: bool = True,
                  optimizer: str = "sgd", beta1: float = 0.9, beta2: float = 0.999, eps: float = 1e-7,
                  embed_fwd: str = "ldg", fwd_chunks: int = 1, dw_first: bool = False):
@@ -416,32 +525,6 @@ class DeepFMTrainStep:
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / iters
 
-    def profile_kernels(self, ids_pool, labels_pool, iters: int = 10):
-        """Eager (non-graph) passes with a CUDA event on the launching stream between kernel groups.
-        Returns ({"embed_fm_fwd_ms": ...}, {label: mean ms}) -- the live per-kernel timing bench.py
-        reports in `roofline` and `kernel_ms`."""
-        runs = []
-        for it in range(iters + 2):      # back-to-back, no host sync in between (steady-state clocks / caches)
-            self.ids.copy_(ids_pool[it % len(ids_pool)], non_blocking=True)
-            self.labels.copy_(labels_pool[it % len(labels_pool)].reshape(-1), non_blocking=True)
-            evs = []
-
-            def mark(label, evs=evs):
-                e = torch.cuda.Event(enable_timing=True)
-                e.record()
-                evs.append((label, e))
-
-            self._enqueue(mark)
-            runs.append(evs)
-        torch.cuda.synchronize()
-        sums, count = {}, 0
-        for evs in runs[2:]:
-            count += 1
-            for (l0, e0), (l1, e1) in zip(evs[:-1], evs[1:]):
-                sums[l1] = sums.get(l1, 0.0) + e0.elapsed_time(e1)
-        shares = {k: v / count for k, v in sums.items()}
-        return {"embed_fm_fwd_ms": shares["embed_fm_fwd"]}, shares
-
     def _persistent_state(self) -> List[torch.Tensor]:
         """Every tensor a step mutates AND a later step reads: parameters and optimizer state."""
         c = self.coll
@@ -465,80 +548,3 @@ class DeepFMTrainStep:
                                            self.state.data_ptr(), ck.step.data_ptr(), ck.lr_hist.data_ptr(),
                                            ck.lr_hist.numel(), ck.lr, ck.beta1, ck.beta2, ck.eps,
                                            torch.cuda.current_stream().cuda_stream), "dr_embed_adam_flush")
-
-    def capture(self):
-        """Warm up (sets kernel attributes) then record the step into a CUDA graph.
-
-        Side-effect free: the warm-up launch is a real step on whatever the static id / label buffers hold, so every
-        parameter and every piece of optimizer state (Adam clock, m, v, stamps) is snapshotted before it and restored
-        after it -- `capture()` leaves the trainer bit-identical to how it found it."""
-        n0 = _lib.launch_count()
-        with torch.no_grad():
-            state = self._persistent_state()
-            saved = [t.clone() for t in state]
-            s = torch.cuda.Stream(device=self.dev)
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                self._enqueue()
-            torch.cuda.current_stream().wait_stream(s)
-            torch.cuda.synchronize()
-            for t, keep in zip(state, saved):
-                t.copy_(keep)
-            del saved
-        torch.cuda.synchronize()
-        self.launches_per_step = _lib.launch_count() - n0
-        if self.use_graph:
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._enqueue()
-            self.graph = g
-        return self
-
-    def run(self):
-        """One step on whatever is in self.ids / self.labels (device resident)."""
-        if self.graph is not None:
-            self.graph.replay()
-        else:
-            self._enqueue()
-
-    def step(self, ids: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
-        """Device-resident inputs: copy into the static buffers (D2D) and run. Returns loss[1]."""
-        self.ids.copy_(ids, non_blocking=True)
-        self.labels.copy_(labels.reshape(-1), non_blocking=True)
-        self.run()
-        return self.loss
-
-    # ---- end-to-end: host buffers in, loss out ---------------------------------------------------
-    def stage_host(self, ids_host: torch.Tensor, labels_host: torch.Tensor):
-        """Start the H2D copy of the NEXT batch on the copy stream into the spare device buffers."""
-        if not hasattr(self, "_spare"):
-            self._spare = (torch.empty_like(self.ids), torch.empty_like(self.labels))
-        with torch.cuda.stream(self._copy_stream):
-            self._spare[0].copy_(ids_host, non_blocking=True)
-            self._spare[1].copy_(labels_host.reshape(-1), non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record()
-        self._staged = ev
-
-    def train_step_host(self, ids_host, labels_host, next_ids_host=None, next_labels_host=None) -> float:
-        """Public end-to-end step.  ids/labels are HOST tensors (pinned for async copies).  If the
-        caller passes the next batch too, its H2D copy overlaps this step's kernels."""
-        cur = torch.cuda.current_stream()
-        if self._staged is None:
-            self.stage_host(ids_host, labels_host)
-        cur.wait_event(self._staged)
-        # swap staged buffers into the static ones the graph reads (D2D, 13.6 MB at C2)
-        self.ids.copy_(self._spare[0], non_blocking=True)
-        self.labels.copy_(self._spare[1], non_blocking=True)
-        done = torch.cuda.Event()
-        done.record(cur)
-        self._staged = None
-        if next_ids_host is not None:
-            self._copy_stream.wait_event(done)
-            self.stage_host(next_ids_host, next_labels_host)
-        self.run()
-        return float(self.loss.item())          # D2H read of the step's result (synchronises)
-
-    def fit_host(self, batches, depth: int = 2) -> List[float]:
-        """Pipelined epoch loop over HOST batches (see module-level fit_host): the public end-to-end call."""
-        return fit_host(self, batches, depth)

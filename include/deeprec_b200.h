@@ -170,6 +170,19 @@ int dr_cross_bwd(const float* x0, const float* x, const float* w, const float* u
                  const float* g, int64_t B, int d, int r,
                  float* h_ws, float* t_ws, float* gx0, float* gx,
                  float* gw, float* guk, float* gvk, float* gb, void* stream);
+/* dr_cross_bwd for a caller that builds the gradient of x0 IN PLACE across a stack of Cross layers
+ *   replaces: the backward of keras/models/ranking/dcn.py:70-88 under the stacking idiom of tests/keras/test_dcn.py:27-32
+ *             (x1 = Cross()(x0, x0); x2 = Cross()(x0, x1); ...), where x0 receives a gradient from EVERY layer.
+ * Same operands and mathematics as dr_cross_bwd, except
+ *   gx0 is ACCUMULATED: gx0 += g*u (the caller initialises it, e.g. with the deep tower's input gradient);
+ *   x_is_x0 != 0 (the bottom layer: x and x0 are the same tensor, x == x0): the input gradient goes into the same
+ *     buffer, gx0 += h @ W^T + alpha*h + g (low rank: t @ U^T + alpha*h + g), and gx may be NULL;
+ *   x_is_x0 == 0: gx is written as by dr_cross_bwd.  gW/gU/gV/gb are OVERWRITTEN. */
+int dr_cross_bwd_acc(const float* x0, const float* x, const float* w, const float* uk,
+                     const float* vk, float alpha, const float* u_saved, const float* xu_saved,
+                     const float* g, int64_t B, int d, int r,
+                     float* h_ws, float* t_ws, float* gx0, float* gx,
+                     float* gw, float* guk, float* gvk, float* gb, int x_is_x0, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Row R (+R1, R2): in-batch softmax loss of the two-tower Retrieval task, fused
@@ -288,6 +301,22 @@ int dr_dense_head_bce_fwd_bwd(const float* a, const float* w, const float* bias,
                               const float* y, int64_t B, int K, int prev_act, float* logit_out,
                               float* prob_out, float* loss_out, float* g_logit, float* g_prev, float* gw,
                               float* gb, float* gb_prev, void* stream);
+
+/* The tail of a DCN in ONE kernel and without the concat: Dense(1)(concat[x_cross, deep]) -> sigmoid cross-entropy (mean
+ * over B, as dr_bce_logits_fwd_bwd) -> their backward.
+ *   replaces: keras/models/ranking/dcn.py:70-88 stacked as in tests/keras/test_dcn.py:27-32 (Cross ... -> Dense(1)), with
+ *             the deep tower's output as the second block of the Dense(1) input.
+ *   x_cross [B,d]: output of the top Cross layer; deep [B,n] = act(z): output of the last DNN layer; w [d+n] (= kernel
+ *   [d+n,1]: rows 0..d-1 multiply x_cross, the rest deep); bias [1] (nullable).  d + n <= 4096, else DR_ENOTSUP.
+ *   logit = x_cross.w[0:d] + deep.w[d:] + bias;  g_logit[b] = (sigmoid - y)/B
+ *   g_xc [B,d] = g_logit * w[0:d]                   gradient into the top Cross layer
+ *   g_deep [B,n] = g_logit * w[d:] * act'(deep)     PRE-activation gradient of the last DNN layer (cf. dr_dense_bwd_chain)
+ *   gw [d+n], gb [1], gb_deep [n] = colsum(g_deep) are OVERWRITTEN;  loss_out [1] OVERWRITTEN.
+ *   logit_out, prob_out, g_logit, g_xc, g_deep, gw, gb, gb_deep may each be NULL. */
+int dr_dcn_head_bce_fwd_bwd(const float* x_cross, const float* deep, const float* w, const float* bias,
+                            const float* y, int64_t B, int d, int n, int deep_act, float* logit_out,
+                            float* prob_out, float* loss_out, float* g_logit, float* g_xc, float* g_deep,
+                            float* gw, float* gb, float* gb_deep, void* stream);
 
 /* =======================================================================================
  * SURVEY.md 8(f) "next" rows: the callers either side of the hot path.
