@@ -101,7 +101,8 @@ __host__ __device__ inline size_t embed_smem_bytes(int S, int warps, int G, int 
 // LINX (experiment, knob embed_fwd_linx): with the in-row first-order weight, size the lane group for the D/4
 // embedding chunks only (D = 16: 4 lanes, 8 examples per warp, no idle lanes) and let lane 0 of the group fetch
 // the weight with a second, scalar load issued right behind its 16-B chunk load (same 128-B line, in flight).
-template <int LPR, typename IdT, int U, bool SHARD, int MINB = 0, bool LINX = false>
+// NOFM (DR_EMBED_NO_FM): the logit is bias + first order only (xDeepFM's linear unit); the FM sums are dead code then.
+template <int LPR, typename IdT, int U, bool SHARD, int MINB = 0, bool LINX = false, bool NOFM = false>
 __global__ void __launch_bounds__(MINB ? 256 : 512, MINB ? MINB : 1) embed_fm_fwd_kernel(const EmbedFwdParams p) {
   constexpr int G = 32 / LPR;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -237,7 +238,7 @@ __global__ void __launch_bounds__(MINB ? 256 : 512, MINB ? MINB : 1) embed_fm_fw
                 (sum.w * sum.w - sq.w);
       t = group_sum<LPR>(t);
       lin = group_sum<LPR>(lin);
-      if (c == 0 && ex_ok) p.out_logit[b] = (bias + lin) + 0.5f * t;
+      if (c == 0 && ex_ok) p.out_logit[b] = NOFM ? (bias + lin) : (bias + lin) + 0.5f * t;
     }
     __syncwarp();   // the id slice is overwritten by the next tile
   }
@@ -385,7 +386,8 @@ __global__ void __launch_bounds__(512) embed_fm_bwd_kernel(const EmbedBwdParams 
 // U slot-steps are loaded before any atomic is issued (the red.global asm is a compiler barrier).
 // LINX (knob embed_bwd_linx, off by default: unmeasured): lane group sized for the D/4 embedding chunks only, the
 // first-order gradient of an in-row weight issued by lane 0 as a scalar red.global.add behind its vector atomic.
-template <int LPR, typename IdT, int U, bool SHARD, bool LINX = false>
+// NOFM (DR_EMBED_NO_FM): dE = g_stack only; g_logit still reaches the first-order weights and the bias.
+template <int LPR, typename IdT, int U, bool SHARD, bool LINX = false, bool NOFM = false>
 __global__ void __launch_bounds__(256) embed_fm_bwd_sp_kernel(const EmbedBwdParams p) {
   constexpr int SPW = 32 / LPR;      // slots per warp-instruction
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -427,8 +429,9 @@ __global__ void __launch_bounds__(256) embed_fm_bwd_sp_kernel(const EmbedBwdPara
   for (int64_t b = warp0; b < p.B; b += nwarps) {
     const float gl = has_fm ? __ldg(p.g_logit + b) : 0.f;
     if (lane == 0) bias_acc += gl;
+    const float gfm = NOFM ? 0.f : gl;   // weight of the FM term in dE
     float4 sum = f4_zero();
-    if (has_fm && chunk_ok) {
+    if (!NOFM && has_fm && chunk_ok) {
       if (p.sum_e) {
         sum = ldg4(p.sum_e + (size_t)b * D + c * 4);
       } else {
@@ -450,10 +453,10 @@ __global__ void __launch_bounds__(256) embed_fm_bwd_sp_kernel(const EmbedBwdPara
           id[u] = (int64_t)__ldg(my_ids + s);
           if (chunk_ok) {
             if (h_ld) {
-              if (has_fm) e[u] = ldg_nc_na_hint(p.stack + ex0 + (size_t)s * D, pol_first);
+              if (!NOFM && has_fm) e[u] = ldg_nc_na_hint(p.stack + ex0 + (size_t)s * D, pol_first);
               if (has_gs) gs[u] = ldg_nc_na_hint(p.g_stack + ex0 + (size_t)s * D, pol_first);
             } else {
-              if (has_fm) e[u] = ldg_nc_na(p.stack + ex0 + (size_t)s * D);
+              if (!NOFM && has_fm) e[u] = ldg_nc_na(p.stack + ex0 + (size_t)s * D);
               if (has_gs) gs[u] = ldg_nc_na(p.g_stack + ex0 + (size_t)s * D);
             }
           }
@@ -474,10 +477,10 @@ __global__ void __launch_bounds__(256) embed_fm_bwd_sp_kernel(const EmbedBwdPara
           }
           if (chunk_ok) {
             float4 d;
-            d.x = scale * fmaf(gl, sum.x - e[u].x, gs[u].x);
-            d.y = scale * fmaf(gl, sum.y - e[u].y, gs[u].y);
-            d.z = scale * fmaf(gl, sum.z - e[u].z, gs[u].z);
-            d.w = scale * fmaf(gl, sum.w - e[u].w, gs[u].w);
+            d.x = scale * fmaf(gfm, sum.x - e[u].x, gs[u].x);
+            d.y = scale * fmaf(gfm, sum.y - e[u].y, gs[u].y);
+            d.z = scale * fmaf(gfm, sum.z - e[u].z, gs[u].z);
+            d.w = scale * fmaf(gfm, sum.w - e[u].w, gs[u].w);
             if (h_red) {
               red_add_v4_hint(row + c * 4, d, pol_first);
               if (LINX && linx_lane) red_add_f32_hint(row + D, scale * gl, pol_first);
@@ -645,6 +648,18 @@ static int dispatch_fwd_linx(const EmbedFwdParams& p, int id_bytes, cudaStream_t
 #undef DR_LINX
 }
 
+// DR_EMBED_NO_FM forward: the default (non-LINX, uncapped) mapping at the default unroll
+template <int LPR, typename IdT>
+static int launch_fwd_nofm(const EmbedFwdParams& p, cudaStream_t st) {
+  constexpr int U = (LPR <= 8) ? 8 : 4;
+  LaunchGeom lg = geom(p.B, p.S, LPR, sizeof(IdT));
+  auto k = embed_fm_fwd_kernel<LPR, IdT, U, false, 0, false, true>;
+  if (lg.smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lg.smem));
+  k<<<lg.ctas, lg.threads, lg.smem, st>>>(p);
+  DR_CUDA_LAUNCH_CHECK("embed_fm_fwd(no_fm)");
+  return DR_OK;
+}
+
 template <int LPR, typename IdT>
 static int launch_fwd(const EmbedFwdParams& p, cudaStream_t st) {
   int U = g_tune_embed_fwd_unroll;
@@ -693,6 +708,23 @@ static int launch_bwd_sp_u(const EmbedBwdParams& p, cudaStream_t st) {
     DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, g_tune_embed_bwd_carveout));
   k<<<(unsigned)ctas, threads, smem, st>>>(p);
   DR_CUDA_LAUNCH_CHECK("embed_fm_bwd_sp");
+  return DR_OK;
+}
+
+// DR_EMBED_NO_FM backward: the slot-parallel kernel (the default mode) whatever the developer mode knob says
+template <int LPR, typename IdT>
+static int launch_bwd_nofm(const EmbedBwdParams& p, cudaStream_t st) {
+  const int threads = 256, warps = threads / 32;
+  const size_t smem = (size_t)p.S * (sizeof(void*) * 2 + sizeof(int64_t) * 2) + kMaxShardWorld * sizeof(void*);
+  int64_t ctas = (p.B + warps - 1) / warps;
+  int per_sm = g_tune_embed_ctas_per_sm > 0 ? g_tune_embed_ctas_per_sm : 8;
+  if (ctas > (int64_t)num_sms() * per_sm) ctas = (int64_t)num_sms() * per_sm;
+  if (ctas < 1) ctas = 1;
+  auto k = embed_fm_bwd_sp_kernel<LPR, IdT, 2, false, false, true>;
+  if (g_tune_embed_bwd_carveout)
+    DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, g_tune_embed_bwd_carveout));
+  k<<<(unsigned)ctas, threads, smem, st>>>(p);
+  DR_CUDA_LAUNCH_CHECK("embed_fm_bwd_sp(no_fm)");
   return DR_OK;
 }
 
@@ -777,6 +809,7 @@ extern "C" int dr_embed_fm_fwd(const float* const* table_ptrs, const float* cons
   p.row_stride = row_stride; p.lin_stride = lin_stride; p.lin_in_row = lin_in_row;
   p.l2_hints = g_tune_embed_l2_hints;
   cudaStream_t st = (cudaStream_t)stream;
+  if (flags & DR_EMBED_NO_FM) DR_DISPATCH_LPR(launch_fwd_nofm, p, st);
   if (g_tune_embed_fwd_linx && lin_in_row && out_logit && lpr_for(D, 0) <= 8) return dispatch_fwd_linx(p, id_bytes, st);
   DR_DISPATCH_LPR(launch_fwd, p, st);
 }
@@ -810,6 +843,7 @@ extern "C" int dr_embed_fm_bwd(const void* ids, int id_bytes, const int64_t* row
   p.l2_hints = g_tune_embed_l2_hints;
   p.mode = g_tune_embed_bwd_mode;
   cudaStream_t st = (cudaStream_t)stream;
+  if (flags & DR_EMBED_NO_FM) DR_DISPATCH_LPR(launch_bwd_nofm, p, st);
   if (g_tune_embed_bwd_linx && p.mode == 0 && lin_in_row && g_logit && lpr_for(D, 0) <= 8) {
     const int lpr = lpr_for(D, 0);
 #define DR_BLINX(L) (id_bytes == 8 ? launch_bwd_sp_u<L, int64_t, 2, true>(p, st) : launch_bwd_sp_u<L, int32_t, 2, true>(p, st))
@@ -868,6 +902,7 @@ extern "C" int dr_embed_fm_fwd_sharded(const float* const* peer_bases, int world
                                        int64_t B, int S, int D, int64_t row_stride, int flags, int64_t lin_offset,
                                        float* out_stack, float* out_sum, float* out_logit, void* stream) {
   if (int rc = check_dims("dr_embed_fm_fwd_sharded", B, S, D, id_bytes)) return rc;
+  DR_REQUIRE(!(flags & DR_EMBED_NO_FM), DR_ENOTSUP, "dr_embed_fm_fwd_sharded: DR_EMBED_NO_FM is not served");
   DR_REQUIRE(lin_offset >= 0 && !((flags & DR_EMBED_LIN_IN_ROW) && lin_offset > 0), DR_EINVAL,
              "dr_embed_fm_fwd_sharded: lin_offset=%lld (must be >= 0 and exclusive with DR_EMBED_LIN_IN_ROW)",
              (long long)lin_offset);
@@ -896,6 +931,7 @@ extern "C" int dr_embed_fm_bwd_sharded(float* const* peer_bases, int world, cons
                                        int S, int D, int64_t row_stride, int flags, int64_t lin_offset, float* g_bias,
                                        float scale, void* stream) {
   if (int rc = check_dims("dr_embed_fm_bwd_sharded", B, S, D, id_bytes)) return rc;
+  DR_REQUIRE(!(flags & DR_EMBED_NO_FM), DR_ENOTSUP, "dr_embed_fm_bwd_sharded: DR_EMBED_NO_FM is not served");
   DR_REQUIRE(lin_offset >= 0 && !((flags & DR_EMBED_LIN_IN_ROW) && lin_offset > 0), DR_EINVAL,
              "dr_embed_fm_bwd_sharded: lin_offset=%lld (must be >= 0 and exclusive with DR_EMBED_LIN_IN_ROW)",
              (long long)lin_offset);

@@ -118,8 +118,11 @@ class EmbeddingCollection(nn.Module):
         o = int(self._offsets[s])
         return self.lin_view()[o:o + self.rows_list[s]]
 
-    def forward(self, ids: torch.Tensor, want_logit: bool = True, bags: Optional[dict] = None):
+    def forward(self, ids: torch.Tensor, want_logit: bool = True, bags: Optional[dict] = None,
+                second_order: bool = True):
         """ids [B, S] int64/int32 -> (stack [B,S,D], logit [B] = bias + linear + FM 2nd order).
+
+        second_order=False: logit = bias + linear only (xDeepFM's linear unit), from the same fused kernel.
 
         bags: {slot: (flat_ids [nnz], row_splits [B+1])} for multi-valued slots (mean-combined embedding,
         summed first-order weights); the matching columns of `ids` are ignored.
@@ -127,6 +130,8 @@ class EmbeddingCollection(nn.Module):
         if ids.dim() != 2 or ids.shape[1] != self.num_slots:
             raise ValueError(f"ids must be [B, {self.num_slots}], got {tuple(ids.shape)}")
         if bags:
+            if not second_order:
+                raise ValueError("second_order=False is not served with multi-valued slots (bags)")
             bad = [s for s in bags if not (0 <= s < self.num_slots)]
             if bad:
                 raise ValueError(f"bags: slot indices {bad} outside [0, {self.num_slots})")
@@ -134,5 +139,5 @@ class EmbeddingCollection(nn.Module):
             return stack, (logit if want_logit else None)
         want = want_logit
         stack, logit = ops.EmbedFM.apply(ids, self.weight, self.linear if want else None,
-                                         self.bias if want else None, self, want)
+                                         self.bias if want else None, self, want, bool(second_order))
         return stack, (logit if want else None)

@@ -12,6 +12,9 @@ def __getattr__(name):
     if name in ("Cross", "DCN"):
         from ..models.ranking import dcn
         return getattr(dcn, name)
+    if name in ("CIN", "XDeepFM"):
+        from ..models.ranking import xdeepfm
+        return getattr(xdeepfm, name)
     if name == "DNN":
         from ..models.ranking.deepfm import DNN
         return DNN

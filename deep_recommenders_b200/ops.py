@@ -12,6 +12,7 @@ from . import _lib
 from ._lib import check
 
 ACT_CODES = {None: 0, "linear": 0, "relu": 1, "sigmoid": 2, "tanh": 3}
+_DR_EMBED_NO_FM = 2
 
 
 def act_code(act) -> int:
@@ -52,15 +53,16 @@ def _ids(t: torch.Tensor, name: str = "ids") -> torch.Tensor:
 # Rows E + L + F: fused multi-slot gather + linear + FM
 # ------------------------------------------------------------------------------------------
 class EmbedFM(torch.autograd.Function):
-    """stack, logit = EmbedFM(ids, weight_arena, linear_arena, bias, meta).
+    """stack, logit = EmbedFM(ids, weight_arena, linear_arena, bias, meta, want_logit, second_order).
 
     `meta` carries the device pointer arrays (table_ptrs, lin_ptrs, rows) of the collection.
     Backward either scatter-adds into dense .grad buffers (meta.sparse_lr is None) or applies
     the fused sparse SGD update in place (meta.sparse_lr = lr) and returns no table gradient.
+    second_order=False (DR_EMBED_NO_FM): the logit is bias + first order only (xDeepFM's linear unit).
     """
 
     @staticmethod
-    def forward(ctx, ids, weight, linear, bias, meta, want_logit: bool):
+    def forward(ctx, ids, weight, linear, bias, meta, want_logit: bool, second_order: bool = True):
         lib = _lib.load()
         ids = _ids(ids)
         B, S = ids.shape
@@ -70,11 +72,14 @@ class EmbedFM(torch.autograd.Function):
         logit = torch.empty((B,), device=weight.device, dtype=torch.float32) if want_logit else None
         tp, lp, rows = meta.pointers(weight, linear)
         has_lin = want_logit and meta.with_linear
+        no_fm = 0 if (second_order or not want_logit) else _DR_EMBED_NO_FM
         check(lib.dr_embed_fm_fwd(tp.data_ptr(), lp.data_ptr() if has_lin else None,
                                   rows.data_ptr(), ids.data_ptr(), ids.element_size(),
                                   _ptr(bias) if want_logit else None, B, S, D, meta.row_stride, meta.lin_stride,
-                                  meta.flags if has_lin else 0, stack.data_ptr(), _ptr(sum_e), _ptr(logit), _stream()), "dr_embed_fm_fwd")
+                                  (meta.flags if has_lin else 0) | no_fm, stack.data_ptr(), _ptr(sum_e), _ptr(logit),
+                                  _stream()), "dr_embed_fm_fwd")
         ctx.meta = meta
+        ctx.no_fm = no_fm
         ctx.want_logit = want_logit
         ctx.has_lin = has_lin
         ctx.has_bias = bias is not None
@@ -96,7 +101,7 @@ class EmbedFM(torch.autograd.Function):
         g_stack = None if g_stack is None else _f32(g_stack, "g_stack")
         g_logit = _f32(g_logit, "g_logit") if (want_logit and g_logit is not None) else None
         if g_stack is None and g_logit is None:
-            return None, None, None, None, None, None
+            return None, None, None, None, None, None, None
         fused = meta.sparse_lr is not None
         if fused:
             gw, gl, gb = weight, linear, bias
@@ -113,13 +118,14 @@ class EmbedFM(torch.autograd.Function):
             check(lib.dr_embed_fm_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(),
                                       stack.data_ptr(), _ptr(sum_e), _ptr(g_logit), _ptr(g_stack),
                                       B, S, D, meta.row_stride, meta.lin_stride,
-                                      meta.flags if lin_grad else 0, tp.data_ptr(),
+                                      (meta.flags if lin_grad else 0) | (ctx.no_fm if g_logit is not None else 0),
+                                      tp.data_ptr(),
                                       lp.data_ptr() if lin_grad else None,
                                       _ptr(gb) if g_logit is not None else None, scale, _stream()),
                   "dr_embed_fm_bwd")
         if fused:
-            return None, None, None, None, None, None
-        return None, gw, gl, gb, None, None
+            return None, None, None, None, None, None, None
+        return None, gw, gl, gb, None, None, None
 
 
 class Gather(torch.autograd.Function):
@@ -281,6 +287,61 @@ class CrossFn(torch.autograd.Function):
         else:
             gx = gx.view(*ctx.lead, d)
         return gx0.view(*ctx.lead, d), gx, gw, guk, gvk, gb, None, None
+
+
+# ------------------------------------------------------------------------------------------
+# Row C: CIN (xDeepFM)
+# ------------------------------------------------------------------------------------------
+class CINFn(torch.autograd.Function):
+    """y [B, H, D], pooled [B, H] = CINFn(x0 [B, m, D], x [B, h, D], kernel [1, m*h, H], bias, act, same, pool).
+
+    `same` is the first layer's call on (x0, x0): one input gradient.  With `pool` False the second output is an empty
+    tensor without gradient."""
+
+    @staticmethod
+    def forward(ctx, x0, x, w, b, act: int, same: bool, pool: bool):
+        lib = _lib.load()
+        x0 = _f32(x0, "x0")
+        x = x0 if same else _f32(x, "x")
+        w = _f32(w, "kernel")
+        b = None if b is None else _f32(b, "bias")
+        B, m, D = x0.shape
+        h = x.shape[1]
+        H = w.shape[-1]
+        if x.shape[0] != B or x.shape[2] != D or w.numel() != m * h * H:
+            raise ValueError(f"CIN: x0 {tuple(x0.shape)}, x {tuple(x.shape)} and kernel {tuple(w.shape)} do not match")
+        y = torch.empty((B, H, D), device=x0.device, dtype=torch.float32)
+        pooled = torch.empty((B, H) if pool else (0,), device=x0.device, dtype=torch.float32)
+        check(lib.dr_cin_fwd(x0.data_ptr(), x.data_ptr(), w.data_ptr(), _ptr(b), B, m, h, D, H, act, y.data_ptr(),
+                             pooled.data_ptr() if pool else None, _stream()), "dr_cin_fwd")
+        ctx.act = act
+        ctx.same = same
+        ctx.set_materialize_grads(False)      # an unused output reaches backward as None, not as zeros to read
+        ctx.save_for_backward(x0, x, w, b, y)
+        if not pool:
+            ctx.mark_non_differentiable(pooled)
+        return y, pooled
+
+    @staticmethod
+    def backward(ctx, gy, gpool):
+        lib = _lib.load()
+        x0, x, w, b, y = ctx.saved_tensors
+        B, m, D = x0.shape
+        h = x.shape[1]
+        H = y.shape[1]
+        gy = None if gy is None else _f32(gy, "gy")
+        gpool = None if (gpool is None or gpool.numel() == 0) else _f32(gpool, "gpool")
+        if gy is None and gpool is None:
+            return None, None, None, None, None, None, None
+        g_ws = torch.empty_like(y)
+        gx0 = torch.empty_like(x0)
+        gx = None if ctx.same else torch.empty_like(x)
+        gw = torch.empty_like(w)
+        gb = None if b is None else torch.empty_like(b)
+        check(lib.dr_cin_bwd(x0.data_ptr(), x.data_ptr(), w.data_ptr(), y.data_ptr(), _ptr(gy), _ptr(gpool),
+                             B, m, h, D, H, ctx.act, int(ctx.same), g_ws.data_ptr(), gx0.data_ptr(), _ptr(gx),
+                             gw.data_ptr(), _ptr(gb), _stream()), "dr_cin_bwd")
+        return gx0, gx, gw, gb, None, None, None
 
 
 # ------------------------------------------------------------------------------------------

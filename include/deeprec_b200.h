@@ -37,6 +37,10 @@ extern "C" {
 #define DR_EMBED_LIN_IN_ROW 1   /* first-order weight of an id is stored IN its row, at float index D
                                    (row_stride >= D+4): it is fetched by the same 128-bit request as the
                                    embedding chunks; lin_ptrs / lin_stride are ignored                  */
+#define DR_EMBED_NO_FM 2        /* dr_embed_fm_fwd / _bwd only: no FM second-order term.  Forward: out_logit =
+                                   bias + sum_s lin_s[id_s] (xDeepFM's linear unit).  Backward: dE = g_stack;
+                                   g_logit still reaches grad_lin and g_bias.  The sharded entries return
+                                   DR_ENOTSUP for it; dr_embed_fm_fwd_tma takes no flags.                  */
 
 /* activation codes (tf.keras.layers.Dense(activation=...)) */
 /* combiner of a multi-valued slot (tf.feature_column.embedding_column(combiner=...)) */
@@ -183,6 +187,34 @@ int dr_cross_bwd_acc(const float* x0, const float* x, const float* w, const floa
                      const float* g, int64_t B, int d, int r,
                      float* h_ws, float* t_ws, float* gx0, float* gx,
                      float* gw, float* guk, float* gvk, float* gb, int x_is_x0, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Row C: xDeepFM's Compressed Interaction Network layer (CIN), the outer product + width-1
+ * conv1d fused into one GEMM whose operand is generated on chip (the [B, D, m*h] outer
+ * product never reaches global memory).
+ *   replaces: keras/models/ranking/xdeepfm.py:71-96 (CIN.call).
+ *   x0 [B, m, D], x [B, h, D], w = the layer's kernel [1, m*h, H] (row i*h + j pairs field i of x0
+ *   with field j of x), bias [H] (nullable), y [B, H, D]:
+ *     y[b,k,d] = act(sum_{i,j} w[i*h+j, k] * x0[b,i,d] * x[b,j,d] + bias[k])
+ *   pooled [B, H] (nullable) receives sum_d y[b,k,d] (xDeepFM's sum pooling), written by the same
+ *   kernel in a fixed order.  act: DR_ACT_*.  Served: 1 <= m, h, H <= 1024, 1 <= D <= 128,
+ *   B * D < 2^31; larger shapes return DR_ENOTSUP.  B = 0 is a no-op (the batch tensors may then
+ *   be NULL; dr_cin_bwd still zeroes gw and gb).  Exact fp32 FFMA.
+ *
+ * dr_cin_bwd: no reference lines (TensorFlow autodiff of the above).
+ *   G = (gy + gpool broadcast over d) * act'(y) is formed once into g_ws [B, H, D]; gy or gpool
+ *   (not both) may be NULL.  Then, overwriting (not accumulating) every output:
+ *     gx0[b,i,d] = sum_{j,k} w[i*h+j,k] x[b,j,d] G[b,k,d]      gx [b,j,d] = sum_{i,k} w[i*h+j,k] x0[b,i,d] G[b,k,d]
+ *     gw[i*h+j,k] = sum_{b,d} x0[b,i,d] x[b,j,d] G[b,k,d]      gb[k] = sum_{b,d} G[b,k,d]  (gb nullable)
+ *   x_is_x0 = 1 (the first layer, called on (x0, x0)): x == x0, h == m, gx must be NULL and both
+ *   contributions land in gx0.  gw is split over the B*D columns and gb over the rows and both are
+ *   summed with floating-point atomics, so their last bits can differ from run to run; y, pooled,
+ *   gx0 and gx are deterministic.                                                          */
+int dr_cin_fwd(const float* x0, const float* x, const float* w, const float* bias, int64_t B,
+               int m, int h, int D, int H, int act, float* y, float* pooled, void* stream);
+int dr_cin_bwd(const float* x0, const float* x, const float* w, const float* y, const float* gy,
+               const float* gpool, int64_t B, int m, int h, int D, int H, int act, int x_is_x0,
+               float* g_ws, float* gx0, float* gx, float* gw, float* gb, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Row R (+R1, R2): in-batch softmax loss of the two-tower Retrieval task, fused
