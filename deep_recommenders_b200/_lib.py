@@ -50,6 +50,10 @@ _SIGS = {
     "dr_cross_bwd_acc": [_p, _p, _p, _p, _p, _f, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p],
     "dr_cin_fwd": [_p, _p, _p, _p, _i64, _i, _i, _i, _i, _i, _p, _p, _p],
     "dr_cin_bwd": [_p, _p, _p, _p, _p, _p, _i64, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p],
+    "dr_din_attn_fwd": [_p, _p, _p, _p, _p, _p, _i64, _i, _i, _i, _i, _i, _p, _p, _p],
+    "dr_din_attn_bwd": [_p, _p, _p, _p, _p, _p, _p, _p, _i64, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p],
+    "dr_dice_fwd": [_p, _p, _i64, _i, _f, _p, _p],
+    "dr_dice_bwd": [_p, _p, _p, _i64, _i, _f, _p, _p, _p],
     "dr_inbatch_softmax_fwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p],
     "dr_inbatch_softmax_bwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p, _p, _p],
     "dr_inbatch_softmax_fwd_ws": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _i64, _p, _p, _p],

@@ -23,7 +23,13 @@ def binary_crossentropy(y_true: torch.Tensor, y_pred: torch.Tensor) -> torch.Ten
     return -(y_true * torch.log(p) + (1.0 - y_true) * torch.log(1.0 - p)).mean(dim=-1)
 
 
-_LOSSES = {"binary_crossentropy": binary_crossentropy}
+def mean_squared_error(y_true: torch.Tensor, y_pred: torch.Tensor) -> torch.Tensor:
+    """tf.keras.losses.mean_squared_error: mean over the last axis of (y_pred - y_true)^2."""
+    return ((y_pred - y_true) ** 2).mean(dim=-1)
+
+
+_LOSSES = {"binary_crossentropy": binary_crossentropy, "mse": mean_squared_error,
+           "mean_squared_error": mean_squared_error}
 
 
 # ---- tf.keras.optimizers ------------------------------------------------------------------------------------------

@@ -2,6 +2,7 @@
 reference does not have it (SURVEY.md section 0, fact 2).  It is provided here as a re-export
 of the hot-path layers so either import path works."""
 from .base import Layer, Model, Dense, Sequential, register_keras_serializable  # noqa: F401
+from .merge import Multiply, Subtract  # noqa: F401
 
 
 def __getattr__(name):
@@ -15,6 +16,9 @@ def __getattr__(name):
     if name in ("CIN", "XDeepFM"):
         from ..models.ranking import xdeepfm
         return getattr(xdeepfm, name)
+    if name in ("ActivationUnit", "Dice", "DIN"):
+        from ..models.ranking import din
+        return getattr(din, name)
     if name == "DNN":
         from ..models.ranking.deepfm import DNN
         return DNN

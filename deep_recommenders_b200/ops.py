@@ -345,6 +345,103 @@ class CINFn(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------
+# Row A: DIN's activation unit (target attention + pooling) and Dice
+# ------------------------------------------------------------------------------------------
+INTERACT_CODES = {None: 0, "none": 0, "subtract": 1, "multiply": 2}
+
+
+class DINAttentionFn(torch.autograd.Function):
+    """pooled [B, D], score [B, T] = DINAttentionFn(keys [B, T, D], query [B, D], W1 [(2|3)D, U], b1, w2 [U, 1] or
+    [U], b2, interact, act, pool): score = act([k | q | f(k, q)] W1 + b1) w2 + b2, pooled = sum_t score * k.
+
+    With `pool` False the first output is an empty tensor without gradient.  An unused output reaches the backward as
+    None, not as zeros to read."""
+
+    @staticmethod
+    def forward(ctx, keys, query, w1, b1, w2, b2, interact: int, act: int, pool: bool):
+        lib = _lib.load()
+        keys = _f32(keys, "keys")
+        query = _f32(query, "query")
+        w1 = _f32(w1, "W1")
+        w2 = _f32(w2, "w2")
+        b1 = None if b1 is None else _f32(b1, "b1")
+        b2 = None if b2 is None else _f32(b2, "b2")
+        if keys.dim() != 3 or query.dim() != 2:
+            raise ValueError(f"DIN attention: keys must be [B, T, D] and query [B, D], got {tuple(keys.shape)} "
+                             f"and {tuple(query.shape)}")
+        B, T, D = keys.shape
+        U = w1.shape[-1]
+        blocks = 3 if interact else 2
+        if query.shape != (B, D) or w1.shape != (blocks * D, U) or w2.numel() != U:
+            raise ValueError(f"DIN attention: keys {tuple(keys.shape)}, query {tuple(query.shape)}, W1 "
+                             f"{tuple(w1.shape)} and w2 {tuple(w2.shape)} do not match")
+        score = torch.empty((B, T), device=keys.device, dtype=torch.float32)
+        pooled = torch.empty((B, D) if pool else (0,), device=keys.device, dtype=torch.float32)
+        check(lib.dr_din_attn_fwd(keys.data_ptr(), query.data_ptr(), w1.data_ptr(), _ptr(b1), w2.data_ptr(), _ptr(b2),
+                                  B, T, D, U, interact, act, score.data_ptr(), pooled.data_ptr() if pool else None,
+                                  _stream()), "dr_din_attn_fwd")
+        ctx.interact, ctx.act = interact, act
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(keys, query, w1, b1, w2, b2)
+        if not pool:
+            ctx.mark_non_differentiable(pooled)
+        return pooled, score
+
+    @staticmethod
+    def backward(ctx, g_pooled, g_score):
+        lib = _lib.load()
+        keys, query, w1, b1, w2, b2 = ctx.saved_tensors
+        B, T, D = keys.shape
+        U = w1.shape[-1]
+        g_pooled = None if (g_pooled is None or g_pooled.numel() == 0) else _f32(g_pooled, "g_pooled")
+        g_score = None if g_score is None else _f32(g_score, "g_score")
+        if g_pooled is None and g_score is None:
+            return (None,) * 9
+        g_keys = torch.empty_like(keys)
+        g_query = torch.empty_like(query)
+        gw1 = torch.empty_like(w1)
+        gw2 = torch.empty_like(w2)
+        gb1 = None if b1 is None else torch.empty_like(b1)
+        gb2 = None if b2 is None else torch.empty_like(b2)
+        check(lib.dr_din_attn_bwd(keys.data_ptr(), query.data_ptr(), w1.data_ptr(), _ptr(b1), w2.data_ptr(), _ptr(b2),
+                                  _ptr(g_pooled), _ptr(g_score), B, T, D, U, ctx.interact, ctx.act,
+                                  g_keys.data_ptr(), g_query.data_ptr(), gw1.data_ptr(), _ptr(gb1), gw2.data_ptr(),
+                                  _ptr(gb2), _stream()), "dr_din_attn_bwd")
+        return g_keys, g_query, gw1, gb1, gw2, gb2, None, None, None
+
+
+class DiceFn(torch.autograd.Function):
+    """y [N, U] = Dice(x [N, U]; alpha [U], epsilon): see dr_dice_fwd."""
+
+    @staticmethod
+    def forward(ctx, x, alpha, eps: float):
+        lib = _lib.load()
+        x = _f32(x, "x")
+        alpha = _f32(alpha, "alpha")
+        if x.dim() != 2 or alpha.numel() != x.shape[1]:
+            raise ValueError(f"Dice: x must be [N, U] with alpha [U], got {tuple(x.shape)} and {tuple(alpha.shape)}")
+        N, U = x.shape
+        y = torch.empty_like(x)
+        check(lib.dr_dice_fwd(x.data_ptr(), alpha.data_ptr(), N, U, float(eps), y.data_ptr(), _stream()),
+              "dr_dice_fwd")
+        ctx.eps = float(eps)
+        ctx.save_for_backward(x, alpha)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _lib.load()
+        x, alpha = ctx.saved_tensors
+        N, U = x.shape
+        gy = _f32(gy, "gy")
+        gx = torch.empty_like(x)
+        galpha = torch.empty_like(alpha)
+        check(lib.dr_dice_bwd(x.data_ptr(), alpha.data_ptr(), gy.data_ptr(), N, U, ctx.eps, gx.data_ptr(),
+                              galpha.data_ptr(), _stream()), "dr_dice_bwd")
+        return gx, galpha, None
+
+
+# ------------------------------------------------------------------------------------------
 # Row R: in-batch softmax
 # ------------------------------------------------------------------------------------------
 # Retrieval losses with at least this many scores (nq * nc) run the tensor-core form (score blocks materialised in a

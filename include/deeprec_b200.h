@@ -217,6 +217,54 @@ int dr_cin_bwd(const float* x0, const float* x, const float* w, const float* y, 
                float* g_ws, float* gx0, float* gx, float* gw, float* gb, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Row A: DIN's activation unit as target attention over a behaviour sequence, fused with the
+ * pooling (the [B*T, 3D] unit input and the [B*T, U] hidden activations never reach global memory).
+ *   replaces: keras/models/ranking/din.py:59-71 (ActivationUnit.call) applied at every position
+ *             of a sequence, plus DIN's weighted sum pooling (Zhou et al., KDD 2018).
+ *   keys [B, T, D] (dense rows, e.g. from dr_gather_fwd), query [B, D], w1 = the hidden Dense
+ *   kernel [(2|3)*D, U] whose row blocks multiply [k | q | f(k, q)], b1 [U] (nullable), w2 = the
+ *   Dense(1) kernel [U], b2 [1] (nullable):
+ *     f = none (interact DR_DIN_INTERACT_NONE, w1 has 2D rows), k - q (SUB) or k * q (MUL)
+ *     score[b,t] = act([k | q | f] . w1 + b1) . w2 + b2          act: DR_ACT_*
+ *     pooled[b,:] = sum_t score[b,t] * keys[b,t,:]               (unnormalised: no softmax)
+ *   score and pooled are both nullable (not both); they are written, never accumulated, by one
+ *   kernel in a fixed order (bit-identical from run to run).  Served: 1 <= D <= 128, 1 <= U <= 256,
+ *   T >= 1, B*T < 2^31; larger D or U return DR_ENOTSUP.  B = 0 is a no-op.  Exact fp32 FFMA.
+ *   Padding: a history padded with id -1 gathers a zero key row, which adds nothing to pooled and
+ *   gets no gradient through the score; dr_scatter_add drops its g_keys row.
+ *
+ * dr_din_attn_bwd: no reference lines (TensorFlow autodiff of the above).  g_pooled [B, D] and
+ *   g_score [B, T] are nullable (not both).  h is recomputed per tile, not saved.  Writes
+ *   g_keys [B, T, D] and g_query [B, D] (each element has one owner: deterministic) and
+ *   gw1, gb1, gw2, gb2, which are split across CTAs and summed with floating-point atomics, so
+ *   their last bits can differ from run to run.  gb1 / gb2 are given exactly when b1 / b2 are.
+ *   B = 0 still zeroes the weight gradients.                                                  */
+#define DR_DIN_INTERACT_NONE 0
+#define DR_DIN_INTERACT_SUB 1
+#define DR_DIN_INTERACT_MUL 2
+int dr_din_attn_fwd(const float* keys, const float* query, const float* w1, const float* b1,
+                    const float* w2, const float* b2, int64_t B, int T, int D, int U, int interact,
+                    int act, float* score, float* pooled, void* stream);
+int dr_din_attn_bwd(const float* keys, const float* query, const float* w1, const float* b1,
+                    const float* w2, const float* b2, const float* g_pooled, const float* g_score,
+                    int64_t B, int T, int D, int U, int interact, int act, float* g_keys,
+                    float* g_query, float* gw1, float* gb1, float* gw2, float* gb2, void* stream);
+
+/* Dice activation on a rank-2 input x [N, U].
+ *   replaces: keras/models/ranking/din.py:110-121 (Dice.call).  Per row: mu = mean,
+ *   sigma = population std (reduce_std), p = sigmoid((x - mu) / sqrt(sigma + eps)) (the square
+ *   root of the std, as the reference computes it), a = PReLU(x) with alpha [U],
+ *   y = a > 0 ? p*a : (1 - p)*a (the branch tests the PReLU output, not x).  One warp per row.
+ * dr_dice_bwd: gx [N, U] through PReLU, p, mu and sigma, galpha [U] (column sums, overwritten,
+ *   summed with floating-point atomics).  Deviation: for a constant row (sigma = 0, every row
+ *   when U = 1) the gradient through sigma is 0, where TensorFlow's autodiff gives NaN.
+ *   dr_dice_bwd serves U <= 8192 (DR_ENOTSUP above).                                          */
+int dr_dice_fwd(const float* x, const float* alpha, int64_t N, int U, float eps, float* y,
+                void* stream);
+int dr_dice_bwd(const float* x, const float* alpha, const float* gy, int64_t N, int U, float eps,
+                float* gx, float* galpha, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * Row R (+R1, R2): in-batch softmax loss of the two-tower Retrieval task, fused
  *   Q @ C^T + online log-sum-exp; the [nq, nc] score matrix is never materialised.
  *   replaces: keras/models/retrieval/sbcnm.py:120-151 (Retrieval.call), :78-86
