@@ -8,6 +8,7 @@ import torch
 
 from oracle import farmhash_py as F
 from oracle import reference_np as R
+from deepfm_oracle import _cpu_deepfm_grads
 
 pytestmark = pytest.mark.gpu
 
@@ -241,34 +242,6 @@ def test_topk_rows_rejects_k_larger_than_row():
 
 
 # ---- Adam inside the train step (SURVEY 8f #1) ------------------------------------------------------------------
-def _cpu_deepfm_grads(tables, lins, bias, ws, bs, ids, labels):
-    """float64 torch-CPU autograd of the reference composition (deepfm.py:36-47 + BCE mean): dense gradients."""
-    tt = [torch.tensor(t, dtype=torch.float64, requires_grad=True) for t in tables]
-    tl = [torch.tensor(l, dtype=torch.float64, requires_grad=True) for l in lins]
-    tb = torch.tensor([bias], dtype=torch.float64, requires_grad=True)
-    tw = [torch.tensor(w, dtype=torch.float64, requires_grad=True) for w in ws]
-    tbi = [torch.tensor(b, dtype=torch.float64, requires_grad=True) for b in bs]
-    B = ids.shape[0]
-    cols, lin = [], tb.expand(B)
-    for s, t in enumerate(tt):
-        ok = torch.from_numpy((ids[:, s] >= 0) & (ids[:, s] < t.shape[0]))
-        idx = torch.from_numpy(np.clip(ids[:, s], 0, t.shape[0] - 1))
-        cols.append(t[idx] * ok[:, None])
-        lin = lin + tl[s][idx] * ok
-    st = torch.stack(cols, 1)
-    fm = 0.5 * ((st.sum(1) ** 2) - (st ** 2).sum(1)).sum(1)
-    h = st.reshape(B, -1)
-    for i, (w, b) in enumerate(zip(tw, tbi)):
-        h = h @ w + b
-        if i < len(tw) - 1:
-            h = torch.relu(h)
-    z = lin + fm + h[:, 0]
-    loss = torch.nn.functional.binary_cross_entropy_with_logits(z, torch.from_numpy(labels).double())
-    loss.backward()
-    g = lambda xs: [x.grad.numpy() for x in xs]
-    return float(loss.detach()), g(tt), g(tl), tb.grad.numpy(), g(tw), g(tbi)
-
-
 @pytest.mark.parametrize("optimizer", ["adam", "lazy_adam", "adam_rows"])
 @pytest.mark.parametrize("D", [16, 32])                   # fused 128-B rows / split layout
 @pytest.mark.parametrize("use_graph", [False, True])
