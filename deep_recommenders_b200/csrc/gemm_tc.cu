@@ -195,35 +195,6 @@ __global__ void __launch_bounds__(256) split_tf32_transpose_kernel(const float* 
   }
 }
 
-__device__ __forceinline__ float epi_scalar_tc(const GemmArgs& a, float acc, int64_t m, int64_t n) {
-  const int64_t off = m * a.ldc + n;
-  switch (a.epi) {
-    case EPI_BIAS_ACT: return act_apply(acc + (a.bias ? __ldg(a.bias + n) : 0.f), a.act);
-    case EPI_ACTGRAD: return acc * act_grad_from_y(__ldg(a.aux0 + off), a.act);
-    case EPI_CROSS: {
-      const float x = __ldg(a.aux1 + off);
-      float u = acc + (a.bias ? __ldg(a.bias + n) : 0.f);
-      if (a.alpha != 0.f) u = u + a.alpha * x;
-      if (a.out2) a.out2[off] = u;
-      return __ldg(a.aux0 + off) * u + x;
-    }
-    case EPI_CROSS_DX: {
-      float v = acc + __ldg(a.aux1 + off);
-      if (a.alpha != 0.f) v += a.alpha * __ldg(a.aux0 + off);
-      return v;
-    }
-    case EPI_SCORES: {
-      float v = acc;
-      if (a.bias) v = v - logf(__ldg(a.bias + n));
-      if (a.cand_ids && m + a.row0 != n && m + a.row0 < a.N && __ldg(a.cand_ids + n) == __ldg(a.cand_ids + m + a.row0))
-        v = v + (-FLT_MAX / 100.0f);
-      return v;
-    }
-    default: return acc;
-  }
-}
-
-
 // Splitter pass over one staged operand tile of ROWS x 32 floats: hi = top 19 bits, lo = v - hi (exact), both written in
 // the K-major SWIZZLE_128B layout (16-B chunk c of row r at r * 128 + ((c ^ (r & 7)) << 4)).
 //   K-major raw tile: TMA staged it in that very layout, so the pass is elementwise on 16-B chunks;
@@ -274,14 +245,175 @@ __device__ __forceinline__ TcItem tc_decode(int64_t item, int64_t n_tiles, int64
   return t;
 }
 
-// Fused epilogue of one warpgroup's 64 x BN accumulator.  Fragment layout of wgmma's D: warp w of the warpgroup owns rows
-// 16 w .. 16 w + 15; d[4 j + {0, 1}] are columns 8 j + 2 (lane % 4) + {0, 1} of row lane / 4, d[4 j + {2, 3}] the same
-// columns of row lane / 4 + 8.  Four lanes write one whole 32-B sector of a row.
-// ACC (EPI_CROSS_DX_ACC, C += acc + alpha*aux0 + aux1) is a compile-time form with kernels of its own (gemm_tc_acc_kernel),
-// so that the kernels of every other epilogue compile exactly as they do without it.
-template <int BN, bool ACC>
+// Two adjacent columns n, n + 1 (n even) of a row-major operand: one 8-B access when VEC (base 8-B aligned, even pitch),
+// else two scalar ones, the second only when `two` (n + 1 < N).
+template <bool VEC>
+__device__ __forceinline__ float2 ld_pair(const float* p, const bool two) {
+  if constexpr (VEC) return __ldg(reinterpret_cast<const float2*>(p));
+  else return make_float2(__ldg(p), two ? __ldg(p + 1) : 0.f);
+}
+template <bool VEC>
+__device__ __forceinline__ void st_pair(float* p, const float2 v, const bool two) {
+  if constexpr (VEC) {
+    *reinterpret_cast<float2*>(p) = v;
+  } else {
+    p[0] = v.x;
+    if (two) p[1] = v.y;
+  }
+}
+
+// Fused epilogue of one warpgroup's 64 x BN accumulator in one epilogue mode EPI (and activation ACT), both fixed at
+// compile time, so the whole fragment is straight-line code.  Fragment layout of wgmma's D: warp w of the warpgroup owns
+// rows 16 w .. 16 w + 15; d[4 j + {0, 1}] are columns 8 j + 2 (lane % 4) + {0, 1} of row lane / 4, d[4 j + {2, 3}] the
+// same columns of row lane / 4 + 8.  Four lanes write one whole 32-B sector of a row.
+// The fragment is walked in groups of G column pairs: the group's bias pair (shared by both rows) and aux pairs are all
+// loaded before any arithmetic on it, so their latencies overlap; G is small enough that the loads fit beside the
+// accumulators without spilling.  Each element's arithmetic is that of the FFMA kernel's epi_scalar (gemm.cu), operation
+// for operation, so both kernels round alike.
+template <int BN, int EPI, int ACT, bool VEC>
+__device__ __forceinline__ void tc_epilogue_mode(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw,
+                                                 const int64_t n0, const int lane) {
+  constexpr int G = (EPI == EPI_CROSS || EPI == EPI_CROSS_DX || EPI == EPI_SCORES) ? 2 : 4;
+  constexpr bool BIAS = EPI == EPI_BIAS_ACT || EPI == EPI_CROSS || EPI == EPI_SCORES;
+  constexpr bool AUX0 = EPI == EPI_ACTGRAD || EPI == EPI_CROSS || EPI == EPI_CROSS_DX;
+  constexpr bool AUX1 = EPI == EPI_CROSS || EPI == EPI_CROSS_DX;
+  static_assert((BN / 8) % G == 0, "column groups must tile the fragment");
+  const int64_t nl = n0 + 2 * (lane & 3);
+  int64_t m[2], row[2];
+  bool row_ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    m[h] = mw + (lane >> 2) + 8 * h;
+    row_ok[h] = m[h] < a.M;
+    row[h] = m[h] * a.ldc + nl;
+  }
+  // EPI_SCORES: candidate id of each row's positive, loaded only where epi_scalar_tc reads it
+  int64_t rid[2] = {0, 0};
+  bool rmask[2] = {false, false};
+  if constexpr (EPI == EPI_SCORES) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      rmask[h] = a.cand_ids && row_ok[h] && m[h] + a.row0 < a.N;
+      if (rmask[h]) rid[h] = __ldg(a.cand_ids + m[h] + a.row0);
+    }
+  }
+#pragma unroll
+  for (int j0 = 0; j0 < BN / 8; j0 += G) {
+    float2 bv[G], x0[2][G], x1[2][G];
+    int64_t cid[G][2];
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      const int64_t n = nl + 8 * (j0 + g);
+      const bool col_ok = n < a.N, two = n + 1 < a.N;
+      bv[g] = make_float2(0.f, 0.f);
+      if constexpr (BIAS) {
+        if (a.bias && col_ok) bv[g] = ld_pair<VEC>(a.bias + n, two);
+      }
+      if constexpr (EPI == EPI_SCORES) {
+        cid[g][0] = (rmask[0] || rmask[1]) && col_ok ? __ldg(a.cand_ids + n) : 0;
+        cid[g][1] = (rmask[0] || rmask[1]) && two ? __ldg(a.cand_ids + n + 1) : 0;
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if constexpr (AUX0) x0[h][g] = row_ok[h] && col_ok ? ld_pair<VEC>(a.aux0 + row[h] + 8 * (j0 + g), two)
+                                                           : make_float2(0.f, 0.f);
+        if constexpr (AUX1) x1[h][g] = row_ok[h] && col_ok ? ld_pair<VEC>(a.aux1 + row[h] + 8 * (j0 + g), two)
+                                                           : make_float2(0.f, 0.f);
+      }
+    }
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      const int j = j0 + g;
+      const int64_t n = nl + 8 * j;
+      if (n >= a.N) continue;
+      const bool two = n + 1 < a.N;
+      float2 lp = make_float2(0.f, 0.f);   // EPI_SCORES: log p of the column pair, shared by both rows
+      if constexpr (EPI == EPI_SCORES) {
+        if (a.bias) lp = make_float2(logf(bv[g].x), two ? logf(bv[g].y) : 0.f);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!row_ok[h]) continue;
+        const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+        const int64_t off = row[h] + 8 * j;
+        float* c = a.C + off;
+        float2 r = make_float2(v0, v1);
+        if constexpr (EPI == EPI_ATOMIC) {
+          red_add_f32(c, v0);
+          if (two) red_add_f32(c + 1, v1);
+          continue;
+        } else if constexpr (EPI == EPI_BIAS_ACT) {
+          r = make_float2(act_apply(v0 + bv[g].x, ACT), act_apply(v1 + bv[g].y, ACT));
+        } else if constexpr (EPI == EPI_ACTGRAD) {
+          r = make_float2(v0 * act_grad_from_y(x0[h][g].x, ACT), v1 * act_grad_from_y(x0[h][g].y, ACT));
+        } else if constexpr (EPI == EPI_CROSS) {
+          float2 u = make_float2(v0 + bv[g].x, v1 + bv[g].y);
+          if (a.alpha != 0.f) {
+            u.x = u.x + a.alpha * x1[h][g].x;
+            u.y = u.y + a.alpha * x1[h][g].y;
+          }
+          if (a.out2) st_pair<VEC>(a.out2 + off, u, two);
+          r = make_float2(x0[h][g].x * u.x + x1[h][g].x, x0[h][g].y * u.y + x1[h][g].y);
+        } else if constexpr (EPI == EPI_CROSS_DX) {
+          r = make_float2(v0 + x1[h][g].x, v1 + x1[h][g].y);
+          if (a.alpha != 0.f) {
+            r.x += a.alpha * x0[h][g].x;
+            r.y += a.alpha * x0[h][g].y;
+          }
+        } else if constexpr (EPI == EPI_SCORES) {
+          if (a.bias) {
+            r.x = r.x - lp.x;
+            r.y = r.y - lp.y;
+          }
+          const int64_t q = m[h] + a.row0;
+          if (rmask[h] && q != n && cid[g][0] == rid[h]) r.x = r.x + (-FLT_MAX / 100.0f);
+          if (rmask[h] && q != n + 1 && cid[g][1] == rid[h]) r.y = r.y + (-FLT_MAX / 100.0f);
+        }
+        st_pair<VEC>(c, r, two);
+      }
+    }
+  }
+}
+
+template <int BN, int EPI, int ACT>
+__device__ __forceinline__ void tc_epilogue_vec(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw,
+                                                const int64_t n0, const int lane, const bool vec_ok) {
+  if (vec_ok) tc_epilogue_mode<BN, EPI, ACT, true>(a, d, mw, n0, lane);
+  else tc_epilogue_mode<BN, EPI, ACT, false>(a, d, mw, n0, lane);
+}
+
+template <int BN, int EPI>
+__device__ __forceinline__ void tc_epilogue_act(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw,
+                                                const int64_t n0, const int lane, const bool vec_ok) {
+  switch (a.act) {
+    case DR_ACT_RELU: tc_epilogue_vec<BN, EPI, DR_ACT_RELU>(a, d, mw, n0, lane, vec_ok); return;
+    case DR_ACT_SIGMOID: tc_epilogue_vec<BN, EPI, DR_ACT_SIGMOID>(a, d, mw, n0, lane, vec_ok); return;
+    case DR_ACT_TANH: tc_epilogue_vec<BN, EPI, DR_ACT_TANH>(a, d, mw, n0, lane, vec_ok); return;
+    default: tc_epilogue_vec<BN, EPI, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
+  }
+}
+
+// The epilogue mode (and the activation, where it matters) is chosen once per tile, not once per element.
+// `vec_ok`: C, every auxiliary operand and the bias are 8-B aligned and ldc and N are even, so every column pair is one
+// float2 access.
+template <int BN>
 __device__ __forceinline__ void tc_epilogue(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw, const int64_t n0,
                                             const int lane, const bool vec_ok) {
+  switch (a.epi) {
+    case EPI_BIAS_ACT: tc_epilogue_act<BN, EPI_BIAS_ACT>(a, d, mw, n0, lane, vec_ok); return;
+    case EPI_ATOMIC: tc_epilogue_mode<BN, EPI_ATOMIC, DR_ACT_NONE, false>(a, d, mw, n0, lane); return;
+    case EPI_ACTGRAD: tc_epilogue_act<BN, EPI_ACTGRAD>(a, d, mw, n0, lane, vec_ok); return;
+    case EPI_CROSS: tc_epilogue_vec<BN, EPI_CROSS, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
+    case EPI_CROSS_DX: tc_epilogue_vec<BN, EPI_CROSS_DX, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
+    case EPI_SCORES: tc_epilogue_vec<BN, EPI_SCORES, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
+    default: tc_epilogue_vec<BN, EPI_STORE, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
+  }
+}
+
+// EPI_CROSS_DX_ACC (C += acc + alpha*aux0 + aux1) is a compile-time form with kernels of its own (gemm_tc_acc_kernel).
+template <int BN>
+__device__ __forceinline__ void tc_epilogue_acc(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw,
+                                                const int64_t n0, const int lane) {
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
     const int64_t m = mw + (lane >> 2) + 8 * half;
@@ -292,19 +424,9 @@ __device__ __forceinline__ void tc_epilogue(const GemmArgs& a, const float (&d)[
       if (n >= a.N) continue;
       const float v0 = d[4 * j + 2 * half], v1 = d[4 * j + 2 * half + 1];
       float* c = a.C + m * a.ldc + n;
-      if constexpr (ACC) {
-        const int64_t off = m * a.ldc + n;
-        c[0] += v0 + a.alpha * __ldg(a.aux0 + off) + __ldg(a.aux1 + off);
-        if (n + 1 < a.N) c[1] += v1 + a.alpha * __ldg(a.aux0 + off + 1) + __ldg(a.aux1 + off + 1);
-      } else if (a.epi == EPI_ATOMIC) {
-        red_add_f32(c, v0);
-        if (n + 1 < a.N) red_add_f32(c + 1, v1);
-      } else if (vec_ok && n + 1 < a.N) {
-        *reinterpret_cast<float2*>(c) = make_float2(epi_scalar_tc(a, v0, m, n), epi_scalar_tc(a, v1, m, n + 1));
-      } else {
-        c[0] = epi_scalar_tc(a, v0, m, n);
-        if (n + 1 < a.N) c[1] = epi_scalar_tc(a, v1, m, n + 1);
-      }
+      const int64_t off = m * a.ldc + n;
+      c[0] += v0 + a.alpha * __ldg(a.aux0 + off) + __ldg(a.aux1 + off);
+      if (n + 1 < a.N) c[1] += v1 + a.alpha * __ldg(a.aux0 + off + 1) + __ldg(a.aux1 + off + 1);
     }
   }
 }
@@ -399,7 +521,10 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
   } else {
     // ===== consumer warpgroups: rows [64 wg, 64 wg + 64) of the tile =====
     const int wg = warp >> 2;
-    const bool vec_ok = ((a.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 7u) == 0);
+    const bool vec_ok = ((a.ldc & 1) == 0) && ((a.N & 1) == 0) &&
+                        (((reinterpret_cast<uintptr_t>(a.C) | reinterpret_cast<uintptr_t>(a.bias) |
+                           reinterpret_cast<uintptr_t>(a.aux0) | reinterpret_cast<uintptr_t>(a.aux1) |
+                           reinterpret_cast<uintptr_t>(a.out2)) & 7u) == 0);
     uint32_t it = 0;
     for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
       const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
@@ -428,13 +553,14 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
       }
       wgmma_wait<0>();
       mbar_arrive(&pl_empty[(it - 1) % TC_PLANE_STAGES]);
-      tc_epilogue<BN, ACC>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane, vec_ok);
+      if constexpr (ACC) tc_epilogue_acc<BN>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane);
+      else tc_epilogue<BN>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane, vec_ok);
     }
   }
 }
 
 // Registers are allocated to warps in groups of four, so 13 warps count as 16: 65536 / 512 = 128 registers per thread.
-// The BN = 128 instantiations hold 64 accumulators and spill one 4-byte value (8 bytes of stack) at that cap.
+// The BN = 128 instantiations hold 64 accumulators and use all 128 without spilling.
 template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
