@@ -54,6 +54,13 @@ _SIGS = {
     "dr_din_attn_bwd": [_p, _p, _p, _p, _p, _p, _p, _p, _i64, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p],
     "dr_dice_fwd": [_p, _p, _i64, _i, _f, _p, _p],
     "dr_dice_bwd": [_p, _p, _p, _i64, _i, _f, _p, _p, _p],
+    "dr_mha_attn_fwd": [_p, _p, _p, _p, _i64, _i, _i, _i, _i, _i64, _i, _f, C.c_uint64, _p, _p, _p],
+    "dr_mha_attn_bwd": [_p, _p, _p, _p, _p, _p, _p, _i64, _i, _i, _i, _i, _i64, _i, _f, C.c_uint64, _p, _p, _p,
+                        _p],
+    "dr_add_layernorm_fwd": [_p, _p, _p, _p, _i64, _i, _f, _p, _p],
+    "dr_add_layernorm_bwd": [_p, _p, _p, _p, _i64, _i, _f, _p, _p, _p, _p],
+    "dr_softmax_rows_fwd": [_p, _i64, _i, _p, _p],
+    "dr_softmax_rows_bwd": [_p, _p, _i64, _i, _p, _p],
     "dr_inbatch_softmax_fwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p],
     "dr_inbatch_softmax_bwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p, _p, _p],
     "dr_inbatch_softmax_fwd_ws": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _i64, _p, _p, _p],

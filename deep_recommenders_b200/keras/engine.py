@@ -28,8 +28,15 @@ def mean_squared_error(y_true: torch.Tensor, y_pred: torch.Tensor) -> torch.Tens
     return ((y_pred - y_true) ** 2).mean(dim=-1)
 
 
+def categorical_crossentropy(y_true: torch.Tensor, y_pred: torch.Tensor) -> torch.Tensor:
+    """tf.keras.losses.categorical_crossentropy on probabilities: y_pred is renormalised over the last axis, clipped
+    to [eps, 1 - eps] (eps = 1e-7), and -sum(y_true * log(y_pred)) is taken over that axis."""
+    p = (y_pred / y_pred.sum(dim=-1, keepdim=True)).clamp(1e-7, 1.0 - 1e-7)
+    return -(y_true * torch.log(p)).sum(dim=-1)
+
+
 _LOSSES = {"binary_crossentropy": binary_crossentropy, "mse": mean_squared_error,
-           "mean_squared_error": mean_squared_error}
+           "mean_squared_error": mean_squared_error, "categorical_crossentropy": categorical_crossentropy}
 
 
 # ---- tf.keras.optimizers ------------------------------------------------------------------------------------------
@@ -136,6 +143,32 @@ class EarlyStopping:
         return False
 
 
+class _OptimizerHandle:
+    """``model.optimizer`` as callbacks see it: ``lr`` reads and writes the learning rate of the optimizer spec and,
+    once the torch optimizer is built (after the first forward), of each of its parameter groups."""
+
+    def __init__(self, model):
+        self._model = model
+
+    @property
+    def lr(self) -> float:
+        opt = self._model._optimizer
+        return float(opt.param_groups[0]["lr"]) if opt is not None else float(self._model._optimizer_spec.kw["lr"])
+
+    @lr.setter
+    def lr(self, value: float) -> None:
+        self._model._optimizer_spec.kw["lr"] = float(value)
+        if self._model._optimizer is not None:
+            for group in self._model._optimizer.param_groups:
+                group["lr"] = float(value)
+
+    learning_rate = lr
+
+
+def _hook(cb, name: str):
+    return getattr(cb, name, None)
+
+
 # ---- the loop -----------------------------------------------------------------------------------------------------
 def _batches(data) -> Iterable:
     """`data`: an iterable / generator of (features, labels) batches, or a zero-argument callable returning one (the
@@ -157,6 +190,12 @@ class TrainingLoopMixin:
         self._optimizer = None
         self._metrics = list(metrics or [])
         return self
+
+    @property
+    def optimizer(self) -> _OptimizerHandle:
+        if not hasattr(self, "_optimizer_spec"):
+            raise RuntimeError("call compile() before reading the optimizer")
+        return _OptimizerHandle(self)
 
     def _step_loss(self, x, y):
         pred = self(x)
@@ -198,6 +237,13 @@ class TrainingLoopMixin:
             x = [(x, y)] * (steps_per_epoch or 1) * epochs
         stream = iter(_batches(x))
         history: dict = {}
+        callbacks = list(callbacks or [])
+        for cb in callbacks:                         # Keras callbacks reach the model through `self.model`
+            if _hook(cb, "on_train_begin") or _hook(cb, "on_batch_end"):
+                cb.model = self
+        for cb in callbacks:
+            if _hook(cb, "on_train_begin"):
+                cb.on_train_begin({})
         for epoch in range(epochs):
             for m in self._metrics:
                 m.reset_state()
@@ -210,6 +256,9 @@ class TrainingLoopMixin:
                 loss.backward()
                 self._optimizer.step()
                 tot = loss.detach().double() if tot is None else tot + loss.detach().double()
+                for cb in callbacks:
+                    if _hook(cb, "on_batch_end"):
+                        cb.on_batch_end(n, {})
                 n += 1
                 for m in self._metrics:
                     m.update_state(yt, pred.detach())
@@ -223,7 +272,7 @@ class TrainingLoopMixin:
                 history.setdefault(k, []).append(v)
             if verbose:
                 print(f"epoch {epoch + 1}/{epochs} " + " ".join(f"{k}={v:.4f}" for k, v in logs.items()), flush=True)
-            if any(cb.on_epoch_end(epoch, logs) for cb in (callbacks or [])):
+            if any(cb.on_epoch_end(epoch, logs) for cb in callbacks):
                 break
         self.history = history
         return history

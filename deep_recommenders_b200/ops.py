@@ -442,6 +442,157 @@ class DiceFn(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------
+# Row T: multi-head attention, LayerNorm of a sum, row softmax
+# ------------------------------------------------------------------------------------------
+class MHAttentionFn(torch.autograd.Function):
+    """out [B, Lq, H*dh] = MHAttentionFn(q [B, Lq, H*dh], k, v [B, Lk, H*dh], mask [Bm, Lk] or None, H, causal, rate,
+    seed): scaled dot-product attention per head (see dr_mha_attn_fwd).  Saves out and the float64 log-sum-exp; the
+    backward regenerates the dropout mask from (seed, rate)."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, mask, H: int, causal: bool, rate: float, seed: int):
+        lib = _lib.load()
+        q, k, v = _f32(q, "queries"), _f32(k, "keys"), _f32(v, "values")
+        mask = None if mask is None else _f32(mask, "masks")
+        if q.dim() != 3 or k.dim() != 3 or v.shape != k.shape or q.shape[0] != k.shape[0] or q.shape[2] != k.shape[2]:
+            raise ValueError(f"attention: queries [B, Lq, H*dh], keys and values [B, Lk, H*dh] expected, got "
+                             f"{tuple(q.shape)}, {tuple(k.shape)}, {tuple(v.shape)}")
+        B, Lq, HD = q.shape
+        Lk = k.shape[1]
+        if HD % H:
+            raise ValueError(f"attention: width {HD} is not a multiple of {H} heads")
+        Bm = 0
+        if mask is not None:
+            if mask.dim() != 2 or mask.shape[1] != Lk or mask.shape[0] == 0 or (H * B) % mask.shape[0]:
+                raise ValueError(f"attention: masks must be [Bm, {Lk}] with Bm dividing {H * B}, got "
+                                 f"{tuple(mask.shape)}")
+            Bm = mask.shape[0]
+        out = torch.empty_like(q)
+        lse = torch.empty((H * B, Lq), device=q.device, dtype=torch.float64)
+        seed = int(seed) % (1 << 64)
+        check(lib.dr_mha_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), _ptr(mask), B, H, Lq, Lk, HD // H, Bm,
+                                  int(bool(causal)), float(rate), seed, out.data_ptr(), lse.data_ptr(), _stream()),
+              "dr_mha_attn_fwd")
+        ctx.meta = (H, bool(causal), float(rate), seed, Bm)
+        ctx.save_for_backward(q, k, v, mask, out, lse)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        lib = _lib.load()
+        q, k, v, mask, out, lse = ctx.saved_tensors
+        H, causal, rate, seed, Bm = ctx.meta
+        B, Lq, HD = q.shape
+        Lk = k.shape[1]
+        g = _f32(g, "g_out")
+        gq, gk, gv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        check(lib.dr_mha_attn_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), _ptr(mask), out.data_ptr(), lse.data_ptr(),
+                                  g.data_ptr(), B, H, Lq, Lk, HD // H, Bm, int(causal), rate, seed, gq.data_ptr(),
+                                  gk.data_ptr(), gv.data_ptr(), _stream()), "dr_mha_attn_bwd")
+        return gq, gk, gv, None, None, None, None, None
+
+
+class AddLayerNormFn(torch.autograd.Function):
+    """y [..., C] = gamma * normalize(x + residual) + beta (residual may be None): see dr_add_layernorm_fwd."""
+
+    @staticmethod
+    def forward(ctx, x, residual, gamma, beta, eps: float):
+        lib = _lib.load()
+        x = _f32(x, "inputs")
+        residual = None if residual is None else _f32(residual, "residual")
+        gamma, beta = _f32(gamma, "gamma"), _f32(beta, "beta")
+        C = x.shape[-1]
+        if (residual is not None and residual.shape != x.shape) or gamma.numel() != C or beta.numel() != C:
+            raise ValueError(f"LayerNormalization: inputs {tuple(x.shape)}, residual "
+                             f"{None if residual is None else tuple(residual.shape)}, gamma {tuple(gamma.shape)} and "
+                             f"beta {tuple(beta.shape)} do not match")
+        N = x.numel() // C
+        y = torch.empty_like(x)
+        check(lib.dr_add_layernorm_fwd(x.data_ptr(), _ptr(residual), gamma.data_ptr(), beta.data_ptr(), N, C,
+                                       float(eps), y.data_ptr(), _stream()), "dr_add_layernorm_fwd")
+        ctx.eps = float(eps)
+        ctx.has_res = residual is not None
+        ctx.save_for_backward(x, residual, gamma)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _lib.load()
+        x, residual, gamma = ctx.saved_tensors
+        C = x.shape[-1]
+        gy = _f32(gy, "gy")
+        gx = torch.empty_like(x)
+        ggamma, gbeta = torch.empty_like(gamma), torch.empty_like(gamma)
+        check(lib.dr_add_layernorm_bwd(x.data_ptr(), _ptr(residual), gamma.data_ptr(), gy.data_ptr(), x.numel() // C,
+                                       C, ctx.eps, gx.data_ptr(), ggamma.data_ptr(), gbeta.data_ptr(), _stream()),
+              "dr_add_layernorm_bwd")
+        return gx, (gx if ctx.has_res else None), ggamma, gbeta, None
+
+
+class SoftmaxRowsFn(torch.autograd.Function):
+    """softmax over the last axis (dr_softmax_rows_fwd / _bwd)."""
+
+    @staticmethod
+    def forward(ctx, x):
+        lib = _lib.load()
+        x = _f32(x, "inputs")
+        V = x.shape[-1]
+        y = torch.empty_like(x)
+        check(lib.dr_softmax_rows_fwd(x.data_ptr(), x.numel() // V, V, y.data_ptr(), _stream()), "dr_softmax_rows_fwd")
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _lib.load()
+        (y,) = ctx.saved_tensors
+        V = y.shape[-1]
+        gy = _f32(gy, "gy")
+        gx = torch.empty_like(y)
+        check(lib.dr_softmax_rows_bwd(y.data_ptr(), gy.data_ptr(), y.numel() // V, V, gx.data_ptr(), _stream()),
+              "dr_softmax_rows_bwd")
+        return gx
+
+
+class TiedProjectionFn(torch.autograd.Function):
+    """logits [M, V] = x [M, d] @ table [V, d]^T without a transposed copy of the table:
+    forward dr_scores_fwd(x, table); gx = G @ table (dr_dense_fwd, table as a [V, d] weight);
+    gtable = G^T @ x (the weight-gradient half of dr_dense_bwd, act NONE)."""
+
+    @staticmethod
+    def forward(ctx, x, table):
+        lib = _lib.load()
+        x, table = _f32(x, "inputs"), _f32(table, "embeddings")
+        if x.dim() != 2 or table.dim() != 2 or x.shape[1] != table.shape[1]:
+            raise ValueError(f"tied projection: x [M, d] and table [V, d] expected, got {tuple(x.shape)}, "
+                             f"{tuple(table.shape)}")
+        M, d = x.shape
+        V = table.shape[0]
+        _lib.ensure_gemm_workspace(M, d, V, x.device)
+        out = torch.empty((M, V), device=x.device, dtype=torch.float32)
+        check(lib.dr_scores_fwd(x.data_ptr(), table.data_ptr(), None, None, M, V, d, out.data_ptr(), _stream()),
+              "dr_scores_fwd")
+        ctx.save_for_backward(x, table)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        lib = _lib.load()
+        x, table = ctx.saved_tensors
+        M, d = x.shape
+        V = table.shape[0]
+        g = _f32(g, "g")
+        gx = torch.empty_like(x)
+        gt = torch.empty_like(table)
+        _lib.ensure_gemm_workspace(M, V, d, x.device)
+        check(lib.dr_dense_fwd(g.data_ptr(), table.data_ptr(), None, M, V, d, 0, gx.data_ptr(), _stream()),
+              "dr_dense_fwd")
+        check(lib.dr_dense_bwd(g.data_ptr(), table.data_ptr(), None, x.data_ptr(), M, V, d, 0, None, None,
+                               gt.data_ptr(), None, _stream()), "dr_dense_bwd")
+        return gx, gt
+
+
+# ------------------------------------------------------------------------------------------
 # Row R: in-batch softmax
 # ------------------------------------------------------------------------------------------
 # Retrieval losses with at least this many scores (nq * nc) run the tensor-core form (score blocks materialised in a

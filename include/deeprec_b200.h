@@ -265,6 +265,67 @@ int dr_dice_bwd(const float* x, const float* alpha, const float* gy, int64_t N, 
                 float* gx, float* galpha, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Row T: multi-head scaled dot-product attention, fused (the [H*B, Lq, Lk] score matrix never
+ * reaches global memory: keys stream through shared memory with an online softmax).
+ *   replaces: keras/models/nlp/multi_head_attention.py:72-84 (ScaledDotProductAttention.call),
+ *             :45-58 (mask, future_mask) and :134-147 (MultiHeadAttention's head split / merge).
+ *   q [B, Lq, H*dh], k and v [B, Lk, H*dh], out [B, Lq, H*dh]: head h is the column block
+ *   h*dh .. (h+1)*dh, so split / concat are strides.  Logical row r = h*B + b (head-major, as the
+ *   reference's concat(split(x, H, axis=2), axis=0)).  The standalone layer is H = 1.
+ *     s   = (q . k) / fl32(sqrt(dh))                         (a division, as TF does)
+ *     s   = s + mask[r % Bm, j] * C      C = fl32(-2^32+1) = -4294967296.0f, added, not -inf;
+ *                                        mask [Bm, Lk] float, nullable, Bm divides H*B (K.tile)
+ *     s   = C where j > i                (causal != 0: replaced, as tf.where; needs Lq == Lk)
+ *     p   = softmax_j(s);  with rate > 0: p * keep(r,i,j) * fl32(1 / (1 - rate))
+ *     out = p . v
+ *   So a row whose keys are all padding gets uniform weights (the mean of v), and with causal
+ *   masking and key 0 padded, row 0 gets uniform weights over all Lk keys, future ones included.
+ *   Dropout: rate in [0, 1), 64-bit seed.  keep(r,i,j) is a stateless splitmix64 finalizer:
+ *     c = (r*Lq + i)*Lk + j;  z = seed + (c + 1) * 0x9E3779B97F4A7C15   (mod 2^64)
+ *     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;
+ *     z ^= z >> 31;  keep = (z >> 40) >= (uint32)(rate * 2^24)     (rate widened to double)
+ *   rate = 0 takes a path with no hashing.
+ *   lse [H*B, Lq] float64 (saved for the backward): m + log(l).  float64 because a fully padded
+ *   row has lse = C + log(Lk), which fp32 (ulp 512 at 2^32) rounds back to C.
+ *   Served: 1 <= dh <= 128 (DR_ENOTSUP above), any Lq, Lk >= 1, H*B*max(Lq, Lk) < 2^31.
+ *   B = 0 is a no-op.  Exact fp32 FFMA; every output element has one owner (bit-identical reruns).
+ *
+ * dr_mha_attn_bwd: no reference lines (TensorFlow autodiff of the above).  Recomputes p from lse;
+ *   D_i = rowsum(g_out * out); ds = p * (dp - D_i), passed through the mask add and zero where the
+ *   causal rule replaced the score; d(q . k) = ds * fl32(1 / fl32(sqrt(dh))) (within an ulp of the
+ *   division TF's autodiff does).  Writes gq, gk, gv (overwritten; gk / gv from a CTA per key
+ *   block looping over queries, gq from a CTA per query block: deterministic).  The dropout mask
+ *   is regenerated from (seed, rate).                                                         */
+int dr_mha_attn_fwd(const float* q, const float* k, const float* v, const float* mask, int64_t B,
+                    int H, int Lq, int Lk, int dh, int64_t Bm, int causal, float rate, uint64_t seed,
+                    float* out, double* lse, void* stream);
+int dr_mha_attn_bwd(const float* q, const float* k, const float* v, const float* mask,
+                    const float* out, const double* lse, const float* g_out, int64_t B, int H,
+                    int Lq, int Lk, int dh, int64_t Bm, int causal, float rate, uint64_t seed,
+                    float* gq, float* gk, float* gv, void* stream);
+
+/* LayerNormalization of x + residual (the Transformer's Add & Norm), rows of width C.
+ *   replaces: keras/models/nlp/transformer.py:109-113 (LayerNormalization.call) applied to the sum
+ *   of :212-213, :218-219, :245-246, :253-254, :260-261.  residual is nullable.  Per row of
+ *   s = x + residual: mu = mean, var = mean((s - mu)^2) (population, tf.nn.moments),
+ *   y = gamma * ((s - mu) / (var + eps) ** 0.5) + beta.  One warp per row.
+ * dr_add_layernorm_bwd: gx [N, C] (the gradient of both x and residual), ggamma and gbeta [C]
+ *   (column sums, overwritten, summed with floating-point atomics: their last bits can differ
+ *   from run to run).  Serves C <= 4096 (DR_ENOTSUP above).                                    */
+int dr_add_layernorm_fwd(const float* x, const float* residual, const float* gamma,
+                         const float* beta, int64_t N, int C, float eps, float* y, void* stream);
+int dr_add_layernorm_bwd(const float* x, const float* residual, const float* gamma,
+                         const float* gy, int64_t N, int C, float eps, float* gx, float* ggamma,
+                         float* gbeta, void* stream);
+
+/* Row softmax over x [N, V]: y = exp(x - max) / sum.
+ *   replaces: keras/models/nlp/transformer.py:264-265 (K.softmax over the vocabulary).
+ * dr_softmax_rows_bwd: gx = y * (gy - sum(gy * y)) from the saved y.  One warp per row.       */
+int dr_softmax_rows_fwd(const float* x, int64_t N, int V, float* y, void* stream);
+int dr_softmax_rows_bwd(const float* y, const float* gy, int64_t N, int V, float* gx,
+                        void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * Row R (+R1, R2): in-batch softmax loss of the two-tower Retrieval task, fused
  *   Q @ C^T + online log-sum-exp; the [nq, nc] score matrix is never materialised.
  *   replaces: keras/models/retrieval/sbcnm.py:120-151 (Retrieval.call), :78-86
