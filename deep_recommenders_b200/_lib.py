@@ -45,6 +45,8 @@ _SIGS = {
     "dr_dense_fwd": [_p, _p, _p, _i64, _i, _i, _i, _p, _p],
     "dr_dense_bwd": [_p, _p, _p, _p, _i64, _i, _i, _i, _p, _p, _p, _p, _p],
     "dr_dense_bwd_chain": [_p, _p, _p, _p, _i64, _i, _i, _i, _p, _p, _p, _p, _p, _i, _p],
+    "dr_dense_grouped_fwd": [_p, _p, _p, _i64, _i, _i, _i, _i, _p, _p],
+    "dr_dense_grouped_bwd": [_p, _p, _p, _p, _i64, _i, _i, _i, _i, _p, _p, _p, _p, _p],
     "dr_cross_fwd": [_p, _p, _p, _p, _p, _p, _f, _i64, _i, _i, _p, _p, _p, _p],
     "dr_cross_bwd": [_p, _p, _p, _p, _p, _f, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p],
     "dr_cross_bwd_acc": [_p, _p, _p, _p, _p, _f, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p],
@@ -61,6 +63,8 @@ _SIGS = {
     "dr_add_layernorm_bwd": [_p, _p, _p, _p, _i64, _i, _f, _p, _p, _p, _p],
     "dr_softmax_rows_fwd": [_p, _i64, _i, _p, _p],
     "dr_softmax_rows_bwd": [_p, _p, _i64, _i, _p, _p],
+    "dr_moe_mix_fwd": [_p, _p, _i64, _i, _i, _i, _p, _p, _p],
+    "dr_moe_mix_bwd": [_p, _p, _p, _i64, _i, _i, _i, _p, _p, _p],
     "dr_inbatch_softmax_fwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p],
     "dr_inbatch_softmax_bwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p, _p, _p],
     "dr_inbatch_softmax_fwd_ws": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _i64, _p, _p, _p],

@@ -249,11 +249,12 @@ static GemmArgs mk(const float* A, const float* B, float* C, int64_t M, int64_t 
   return a;
 }
 
-// gW[Kw,N] = X^T[Kw,M] @ G[M,N] (split-K over the batch, atomics into zeroed gW)
+// gW[Kw,N] = X^T[Kw,M] @ G[M,N] (split-K over the batch, atomics into zeroed gW); ldx / ldg: row pitches of X and G
+// (0 = packed)
 static int gemm_xt_g(const float* X, const float* G, float* gW, int64_t M, int64_t Kw, int64_t N,
-                     cudaStream_t st, bool accumulate = false) {
+                     cudaStream_t st, bool accumulate = false, int64_t ldx = 0, int64_t ldg = 0) {
   if (!accumulate) DR_CUDA_CALL(cudaMemsetAsync(gW, 0, sizeof(float) * Kw * N, st));
-  GemmArgs a = mk(X, G, gW, Kw, N, M, Kw, N, N, EPI_ATOMIC);
+  GemmArgs a = mk(X, G, gW, Kw, N, M, ldx ? ldx : Kw, ldg ? ldg : N, N, EPI_ATOMIC);
   a.splitk = splitk_for(Kw, N, M);
   a.stages = g_tune_tc_dw_stages;
   a.share = g_tune_tc_dw_share;
@@ -347,6 +348,61 @@ extern "C" int dr_dense_bwd_chain(const float* x, const float* w, const float* y
   DR_REQUIRE(act == DR_ACT_NONE || (y && gz_ws), DR_EINVAL, "dr_dense_bwd_chain: activation needs y and gz_ws");
   DR_REQUIRE(prev_act == DR_ACT_NONE || (prev_y && gx), DR_EINVAL, "dr_dense_bwd_chain: prev_act needs prev_y and gx");
   return dense_bwd_impl(x, w, y, gy, M, K, N, act, gz_ws, gx, gw, gb, prev_y, prev_act, (cudaStream_t)stream);
+}
+
+// G Dense layers of one shape on column blocks: x [M, G*K], w [G, K, N], b [G, N], y [M, G*N].  Group g is the plain
+// Dense call on x[:, g*K ..] and y[:, g*N ..], run as one strided GEMM per group (the TMA path takes the strides when
+// it can, the eligibility check sends the others to FFMA).
+extern "C" int dr_dense_grouped_fwd(const float* x, const float* w, const float* b, int64_t M, int G, int K, int N,
+                                    int act, float* y, void* stream) {
+  DR_REQUIRE(x && w && y, DR_EINVAL, "dr_dense_grouped_fwd: null pointer");
+  DR_REQUIRE(M >= 0 && G >= 1 && K >= 1 && N >= 1, DR_EINVAL, "dr_dense_grouped_fwd: bad shape");
+  DR_REQUIRE((int64_t)G * K < ((int64_t)1 << 31) && (int64_t)G * N < ((int64_t)1 << 31), DR_EINVAL,
+             "dr_dense_grouped_fwd: G*K and G*N must stay below 2^31");
+  DR_REQUIRE(act >= DR_ACT_NONE && act <= DR_ACT_TANH, DR_EINVAL, "dr_dense_grouped_fwd: unknown activation %d", act);
+  const int64_t ldx = (int64_t)G * K, ldy = (int64_t)G * N;
+  for (int g = 0; g < G; ++g) {
+    GemmArgs a = mk(x + (int64_t)g * K, w + (int64_t)g * K * N, y + (int64_t)g * N, M, N, K, ldx, N, ldy, EPI_BIAS_ACT);
+    a.bias = b ? b + (int64_t)g * N : nullptr; a.act = act;
+    if (int rc = gemm_launch(a, false, false, (cudaStream_t)stream)) return rc;
+  }
+  return DR_OK;
+}
+
+// Backward: one activation-gradient + column-sum pass over the whole [M, G*N] block (elementwise, so the Dense pass
+// with N' = G*N writes gb [G, N] directly), then per group the strided dX GEMM and the split-K dW GEMM.
+extern "C" int dr_dense_grouped_bwd(const float* x, const float* w, const float* y, const float* gy, int64_t M, int G,
+                                    int K, int N, int act, float* gz_ws, float* gx, float* gw, float* gb, void* stream) {
+  DR_REQUIRE(x && w && gy && (gw || gx), DR_EINVAL, "dr_dense_grouped_bwd: null pointer");
+  DR_REQUIRE(M >= 0 && G >= 1 && K >= 1 && N >= 1, DR_EINVAL, "dr_dense_grouped_bwd: bad shape");
+  DR_REQUIRE((int64_t)G * K < ((int64_t)1 << 31) && (int64_t)G * N < ((int64_t)1 << 31), DR_EINVAL,
+             "dr_dense_grouped_bwd: G*K and G*N must stay below 2^31");
+  DR_REQUIRE(act >= DR_ACT_NONE && act <= DR_ACT_TANH, DR_EINVAL, "dr_dense_grouped_bwd: unknown activation %d", act);
+  DR_REQUIRE(act == DR_ACT_NONE || (y && gz_ws), DR_EINVAL, "dr_dense_grouped_bwd: activation needs y and gz_ws");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t ldx = (int64_t)G * K, ldy = (int64_t)G * N;
+  if (gb) DR_CUDA_CALL(cudaMemsetAsync(gb, 0, sizeof(float) * ldy, st));
+  if (M == 0) {
+    if (gw) DR_CUDA_CALL(cudaMemsetAsync(gw, 0, sizeof(float) * (size_t)G * K * N, st));
+    return DR_OK;
+  }
+  const float* gz = gy;
+  if (act != DR_ACT_NONE || gb) {
+    if (int rc = launch_actgrad_colsum(gy, y, act, M, ldy, rows_per_cta_for(M), gz_ws, gb, st)) return rc;
+    if (act != DR_ACT_NONE) gz = gz_ws;
+  }
+  for (int g = 0; g < G; ++g) {
+    const float* gz_g = gz + (int64_t)g * N;
+    const float* w_g = w + (int64_t)g * K * N;
+    if (gx) {
+      GemmArgs a = mk(gz_g, w_g, gx + (int64_t)g * K, M, K, N, ldy, N, ldx, EPI_STORE);   // gx_g = gz_g @ W_g^T
+      if (int rc = gemm_launch(a, false, true, st)) return rc;
+    }
+    if (gw) {
+      if (int rc = gemm_xt_g(x + (int64_t)g * K, gz_g, gw + (int64_t)g * K * N, M, K, N, st, false, ldx, ldy)) return rc;
+    }
+  }
+  return DR_OK;
 }
 
 extern "C" int dr_cross_fwd(const float* x0, const float* x, const float* w, const float* uk, const float* vk,

@@ -651,6 +651,9 @@ bool gemm_tc_eligible(const GemmArgs& a, bool ta, bool tb) {
   // operands already K-major are split in place with float4 accesses
   if (!ta && ((a.lda & 3) || !aligned16(a.A))) return false;
   if (tb && ((a.ldb & 3) || !aligned16(a.B))) return false;
+  // that flat split reads rows * ld floats from the operand's first element: a K-major operand whose pitch is wider than
+  // K (a column block of a wider matrix, as the grouped Dense passes) would be read past its last row, so it goes to FFMA
+  if ((!ta && a.lda != a.K) || (tb && a.ldb != a.K)) return false;
   if (!g_ws_ptr) return false;
   size_t ae, be;
   plane_elems(a, ta, tb, &ae, &be);

@@ -105,6 +105,68 @@ def indicator_column(categorical_column: CategoricalColumn) -> IndicatorColumn:
     return IndicatorColumn(categorical_column)
 
 
+@dataclass(frozen=True)
+class NumericColumn:
+    """tf.feature_column.numeric_column: the feature's values, reshaped to [batch, prod(shape)] and cast to float32."""
+    key: str
+    shape: Tuple = (1,)
+    dtype: str = "float32"
+
+    @property
+    def name(self) -> str:
+        return self.key
+
+    @property
+    def width(self) -> int:
+        w = 1
+        for s in self.shape:
+            w *= int(s)
+        return w
+
+
+def numeric_column(key: str, shape=(1,), dtype: str = "float32") -> NumericColumn:
+    shape = (int(shape),) if isinstance(shape, int) else tuple(int(s) for s in shape)
+    if not shape or any(s < 1 for s in shape):
+        raise ValueError(f"shape dimensions must be greater than 0. shape: {shape}, key: {key}")
+    if dtype not in ("float32", "float64", "float16", "int32", "int64"):
+        raise ValueError(f"dtype must be convertible to float. dtype: {dtype}, key: {key}")
+    return NumericColumn(key, shape, dtype)
+
+
+def input_layer(features, feature_columns, device=None):
+    """tf.feature_column.input_layer for numeric columns: the columns concatenated in order of their names (as
+    TensorFlow sorts them, so C10 comes before C2) into one float32 [batch, sum of widths] CUDA tensor.  Host
+    features are concatenated on the host and copied to the device once per batch."""
+    import numpy as np
+    import torch
+
+    cols = list(feature_columns) if isinstance(feature_columns, (list, tuple)) else [feature_columns]
+    if not cols:
+        raise ValueError("feature_columns must not be empty")
+    for c in cols:
+        if not isinstance(c, NumericColumn):
+            raise NotImplementedError(f"input_layer serves numeric columns only; got {type(c).__name__} "
+                                      f"{getattr(c, 'name', c)!r} (categorical columns go through the embedding "
+                                      "models' own lookup)")
+    cols = sorted(cols, key=lambda c: c.name)
+    parts = []
+    for c in cols:
+        if c.key not in features:
+            raise KeyError(f"feature {c.key!r} of numeric_column {c.name!r} is missing from the features")
+        v = features[c.key]
+        n = v.shape[0]
+        if int(np.prod(v.shape[1:], dtype=np.int64)) != c.width:
+            raise ValueError(f"feature {c.key!r} has shape {tuple(v.shape)}, numeric_column expects "
+                             f"[batch, {', '.join(map(str, c.shape))}]")
+        parts.append(v.reshape(n, c.width))
+    dev = torch.device(device) if device is not None else torch.device("cuda")
+    if all(isinstance(p, torch.Tensor) and p.is_cuda for p in parts):
+        return torch.cat([p.to(torch.float32) for p in parts], dim=1)
+    host = np.concatenate([p.detach().cpu().numpy() if isinstance(p, torch.Tensor) else np.asarray(p)
+                           for p in parts], axis=1).astype(np.float32, copy=False)
+    return torch.from_numpy(np.ascontiguousarray(host)).to(dev)
+
+
 def embedding_column(categorical_column: CategoricalColumn, dimension: int, combiner: str = "mean",
                      initializer_stddev: Optional[float] = None) -> EmbeddingColumn:
     if dimension is None or dimension < 1:

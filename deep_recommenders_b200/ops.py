@@ -232,6 +232,85 @@ class DenseFn(torch.autograd.Function):
         return (gx.view(*ctx.lead, K) if need_x else None), gw, gb, None
 
 
+class GroupedDenseFn(torch.autograd.Function):
+    """y [M, G*N] = GroupedDenseFn(x [M, G*K], w [G, K, N], b [G, N] or None, act): G Dense layers of one shape on
+    column blocks (dr_dense_grouped_fwd / _bwd)."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, act: int):
+        lib = _lib.load()
+        x = _f32(x, "x")
+        w = _f32(w, "kernel")
+        b = None if b is None else _f32(b, "bias")
+        if w.dim() != 3 or x.dim() != 2 or x.shape[1] != w.shape[0] * w.shape[1] or (
+                b is not None and tuple(b.shape) != (w.shape[0], w.shape[2])):
+            raise ValueError(f"grouped Dense: x [M, G*K], kernel [G, K, N], bias [G, N] expected, got {tuple(x.shape)}, "
+                             f"{tuple(w.shape)}, {None if b is None else tuple(b.shape)}")
+        G, K, N = w.shape
+        M = x.shape[0]
+        _lib.ensure_gemm_workspace(M, G * K, G * N, x.device)
+        y = torch.empty((M, G * N), device=x.device, dtype=torch.float32)
+        check(lib.dr_dense_grouped_fwd(x.data_ptr(), w.data_ptr(), _ptr(b), M, G, K, N, act, y.data_ptr(), _stream()),
+              "dr_dense_grouped_fwd")
+        ctx.act = act
+        ctx.has_bias = b is not None
+        ctx.save_for_backward(x, w, y)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _lib.load()
+        x, w, y = ctx.saved_tensors
+        G, K, N = w.shape
+        M = x.shape[0]
+        gy = _f32(gy, "gy")
+        gz_ws = torch.empty_like(gy) if ctx.act != 0 else None
+        gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        gw = torch.empty_like(w)
+        gb = torch.empty((G, N), device=gy.device, dtype=torch.float32) if ctx.has_bias else None
+        check(lib.dr_dense_grouped_bwd(x.data_ptr(), w.data_ptr(), y.data_ptr(), gy.data_ptr(), M, G, K, N, ctx.act,
+                                       _ptr(gz_ws), _ptr(gx), gw.data_ptr(), _ptr(gb), _stream()),
+              "dr_dense_grouped_bwd")
+        return gx, gw, gb, None
+
+
+class MoEMixFn(torch.autograd.Function):
+    """out [B, T*H] = MoEMixFn(experts [B, E*H], logits [B, T*E], T): per task t, softmax(logits[:, t*E:(t+1)*E]) mixes
+    the E expert blocks (dr_moe_mix_fwd / _bwd).  Saves the gates."""
+
+    @staticmethod
+    def forward(ctx, experts, logits, T: int):
+        lib = _lib.load()
+        experts, logits = _f32(experts, "experts"), _f32(logits, "logits")
+        T = int(T)
+        if experts.dim() != 2 or logits.dim() != 2 or logits.shape[0] != experts.shape[0] or T < 1 or \
+                logits.shape[1] < T or logits.shape[1] % T or experts.shape[1] % (logits.shape[1] // T) or \
+                experts.shape[1] == 0:
+            raise ValueError(f"mixture of experts: experts [B, E*H] and logits [B, T*E] with T = {T} expected, got "
+                             f"{tuple(experts.shape)} and {tuple(logits.shape)}")
+        B = experts.shape[0]
+        E = logits.shape[1] // T
+        H = experts.shape[1] // E
+        gates = torch.empty_like(logits)
+        out = torch.empty((B, T * H), device=experts.device, dtype=torch.float32)
+        check(lib.dr_moe_mix_fwd(experts.data_ptr(), logits.data_ptr(), B, E, T, H, gates.data_ptr(), out.data_ptr(),
+                                 _stream()), "dr_moe_mix_fwd")
+        ctx.shape = (E, T, H)
+        ctx.save_for_backward(experts, gates)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        lib = _lib.load()
+        experts, gates = ctx.saved_tensors
+        E, T, H = ctx.shape
+        g = _f32(g, "g_out")
+        g_experts, g_logits = torch.empty_like(experts), torch.empty_like(gates)
+        check(lib.dr_moe_mix_bwd(experts.data_ptr(), gates.data_ptr(), g.data_ptr(), experts.shape[0], E, T, H,
+                                 g_experts.data_ptr(), g_logits.data_ptr(), _stream()), "dr_moe_mix_bwd")
+        return g_experts, g_logits, None
+
+
 # ------------------------------------------------------------------------------------------
 # Row X: Cross
 # ------------------------------------------------------------------------------------------

@@ -152,6 +152,20 @@ int dr_dense_bwd_chain(const float* x, const float* w, const float* y, const flo
                        int64_t M, int K, int N, int act,
                        float* gz_ws, float* gx, float* gw, float* gb,
                        const float* prev_y, int prev_act, void* stream);
+/* G independent Dense layers of one shape (the expert and task towers of MMoE, ESMM's two towers):
+ *   replaces: the per-tower tf.layers.dense calls of estimator/models/feature_interaction/dnn.py:17-29 as called
+ *             by estimator/models/multi_task_learning/mixture_of_experts.py:64-68, :86-90 and esmm.py:38-55.
+ *   x [M, G*K] (group g reads column block g*K), w [G, K, N], b [G, N] (nullable), y [M, G*N] (group g writes
+ *   column block g*N).  Per group exactly dr_dense_fwd / dr_dense_bwd: same activations, gz_ws [M, G*N],
+ *   gx [M, G*K] (NULL = skip), gw [G, K, N] and gb [G, N] OVERWRITTEN.  One strided GEMM per group; the backward's
+ *   activation-gradient + column-sum pass runs once over the whole [M, G*N] block.  G = 1: y and gx are
+ *   bit-identical to dr_dense_fwd / dr_dense_bwd; gw and gb are summed with split-K / column atomics, so their last
+ *   bits depend on the summation order (as in dr_dense_bwd).  Served: any G, K, N >= 1 with G*K, G*N < 2^31.  */
+int dr_dense_grouped_fwd(const float* x, const float* w, const float* b, int64_t M, int G, int K, int N,
+                         int act, float* y, void* stream);
+int dr_dense_grouped_bwd(const float* x, const float* w, const float* y, const float* gy,
+                         int64_t M, int G, int K, int N, int act,
+                         float* gz_ws, float* gx, float* gw, float* gb, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Row X: Cross layer (DCN-v2 matrix form).
@@ -324,6 +338,26 @@ int dr_add_layernorm_bwd(const float* x, const float* residual, const float* gam
 int dr_softmax_rows_fwd(const float* x, int64_t N, int V, float* y, void* stream);
 int dr_softmax_rows_bwd(const float* y, const float* gy, int64_t N, int V, float* gx,
                         void* stream);
+
+/* Multi-gate mixture of experts: every task's gate softmax and expert mixture in one pass.
+ *   replaces: estimator/models/multi_task_learning/mixture_of_experts.py:46-53 (gating softmax), :69 (tf.stack of the
+ *   experts), :73-78 (per gate: expand_dims, [B,1,E] @ [B,E,H] matmul, squeeze).  The reference builds num_experts
+ *   gates and uses the first num_tasks; this serves exactly T gates.
+ *   experts [B, E*H] (expert e = column block e*H), logits [B, T*E] (task t's gate logits = column block t*E).
+ *   gates [B, T*E] (saved): gates[b,t,:] = softmax(logits[b,t,:]) -- max subtracted, expf, divided by the sum.
+ *   out [B, T*H]: out[b, t*H + h] = sum_e gates[b,t,e] * experts[b, e*H + h]   (e ascending, fp32 fmaf onto an
+ *   accumulator that starts at -0.0, so the first step is exactly the first product).  E = 1: the gate is exactly 1
+ *   and out equals the expert bit for bit, signed zeros included (a NaN expert gives a NaN, not its payload).
+ * dr_moe_mix_bwd: no reference lines (TensorFlow autodiff of the above).
+ *   g_experts[b,e,h] = sum_t gates[b,t,e] * g_out[b,t,h];  dg[b,t,e] = sum_h g_out[b,t,h] * experts[b,e,h];
+ *   g_logits[b,t,e] = gates[b,t,e] * (dg[b,t,e] - sum_e' gates[b,t,e'] * dg[b,t,e'])   (both overwritten).
+ *   One warp owns a row; sums are per-lane in a fixed order plus a fixed butterfly: no atomics, every output element
+ *   has one owner, reruns are bit-identical.
+ *   Served: 1 <= E <= 32, 1 <= T <= 16, any H >= 1 with E*H, T*H < 2^31 (DR_ENOTSUP outside).  B = 0 is a no-op. */
+int dr_moe_mix_fwd(const float* experts, const float* logits, int64_t B, int E, int T, int H, float* gates,
+                   float* out, void* stream);
+int dr_moe_mix_bwd(const float* experts, const float* gates, const float* g_out, int64_t B, int E, int T, int H,
+                   float* g_experts, float* g_logits, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Row R (+R1, R2): in-batch softmax loss of the two-tower Retrieval task, fused
