@@ -7,20 +7,24 @@
 // TF32/BF16) at 3 tensor-core products per k-step.
 //
 // Structure (one 128 x BN output tile per work item, persistent grid, 416 threads, sm_90a only):
-//   warps 0-7   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async.m64n{BN}k8.tf32 (both operands from
-//               shared memory, accumulator in registers) x 4 k-steps x 3 products per k-block, then the fused epilogue
-//               (gemm.cuh Epi modes) straight from the accumulator registers (float2 stores / split-K reductions)
-//   warps 8-11  splitters: turn every staged raw fp32 tile into its hi and lo planes in the layout wgmma reads
+//   warps 0-7   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async.m64n{BN}k8.tf32 (accumulator in
+//               registers) x 4 k-steps x 3 products per k-block, then the fused epilogue (gemm.cuh Epi modes) straight
+//               from the accumulator registers (float2 stores / split-K reductions).  Variant 2: each thread loads its
+//               A-fragment elements from the raw A tile, splits them in registers and passes them to wgmma as a
+//               register fragment; B comes from the plane ring.  Variant 1: both operands from the plane ring.
+//   warps 8-11  splitters (variant 2): turn every staged raw fp32 B tile into its hi and lo planes in the layout wgmma
+//               reads
 //   warp 12     TMA producer: cp.async.bulk.tensor into the raw ring, completion on "full" mbarriers (expect_tx)
-// wgmma reads 32-bit operands from shared memory K-major only (canonical SWIZZLE_128B layout, 32 tf32 = 128 B per row).
-// An operand stored K-major (row-major [rows, K]) is staged by TMA in exactly that layout and split chunk by chunk; an
-// operand stored MN-major ([K, rows] row-major: the weight of a forward layer, both operands of a weight gradient) is
-// staged as stored and TRANSPOSED by the same splitter pass, which has to touch every element anyway.
-// Two rings decouple the stages: raw tiles (TMA -> splitters), planes (splitters -> wgmma), each with full / empty
-// mbarriers; fence.proxy.async orders the splitters' generic stores before wgmma's reads.
-// Variant 1 (g_tune_gemm_variant == 1, PRESPLIT): the hi/lo planes are produced K-major in caller-provided workspace
-// (dr_set_workspace) by split_tf32_kernel / split_tf32_transpose_kernel and TMA loads them straight into the plane
-// ring; variant 2 (the default) needs no workspace and no pre-pass.
+// wgmma reads 32-bit B operands from shared memory K-major only (canonical SWIZZLE_128B layout, 32 tf32 = 128 B per
+// row).  A B operand stored K-major (row-major [N, K]) is staged by TMA in exactly that layout and split chunk by chunk;
+// one stored MN-major ([K, N] row-major: the weight of a forward layer, gZ in a weight gradient) is staged as stored and
+// TRANSPOSED by the same splitter pass, which has to touch every element anyway.  A is staged as stored (K-major in
+// SWIZZLE_128B, MN-major unswizzled) and read element by element by the consumers, so either layout needs no transpose.
+// Two rings decouple the stages: raw tiles (TMA -> splitters and consumers), B planes (splitters -> wgmma), each with
+// full / empty mbarriers; fence.proxy.async orders the splitters' generic stores before wgmma's reads.
+// Variant 1 (g_tune_gemm_variant == 1, PRESPLIT): the hi/lo planes of both operands are produced K-major in
+// caller-provided workspace (dr_set_workspace) by split_tf32_kernel / split_tf32_transpose_kernel and TMA loads them
+// straight into the plane ring; variant 2 (the default) needs no workspace and no pre-pass.
 #include "gemm.cuh"
 #include <cuda.h>
 #include <float.h>
@@ -150,6 +154,57 @@ __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t da, uin
       : "l"(da), "l"(db), "r"(1));
 }
 
+// D[64 x N] += A[64 x 8] * B[8 x N] with A from registers: the thread's four elements of the .tf32 m64nNk8 A fragment
+// (warp w of the warpgroup owns rows 16 w .. 16 w + 15; a[0] is row lane / 4, column lane % 4 of the k-step, a[1] row
+// lane / 4 + 8, a[2] and a[3] the same rows at column lane % 4 + 4), B from shared memory by descriptor.
+template <int N>
+__device__ __forceinline__ void wgmma_tf32_ra(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db);
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<64>(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<128>(float (&d)[64], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
+}
+
 __global__ void __launch_bounds__(256) split_tf32_kernel(const float* __restrict__ x, int64_t n4,
                                                           float* __restrict__ hi, float* __restrict__ lo) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -195,7 +250,7 @@ __global__ void __launch_bounds__(256) split_tf32_transpose_kernel(const float* 
   }
 }
 
-// Splitter pass over one staged operand tile of ROWS x 32 floats: hi = top 19 bits, lo = v - hi (exact), both written in
+// Splitter pass over one staged B tile of ROWS x 32 floats: hi = top 19 bits, lo = v - hi (exact), both written in
 // the K-major SWIZZLE_128B layout (16-B chunk c of row r at r * 128 + ((c ^ (r & 7)) << 4)).
 //   K-major raw tile: TMA staged it in that very layout, so the pass is elementwise on 16-B chunks;
 //   MN-major raw tile: [32 k-rows][ROWS] as stored; a thread gathers 4 consecutive k of one row (the lanes of a warp read
@@ -431,17 +486,54 @@ __device__ __forceinline__ void tc_epilogue_acc(const GemmArgs& a, const float (
   }
 }
 
+// Shared-memory stages of one tile width.  The plane ring holds [Ah | Al | Bh | Bl] in variant 1 and [Bh | Bl] in
+// variant 2, whose consumers split A in registers; the raw ring (variant 2 only) holds [A raw | B raw].
+template <int BN, bool PRESPLIT>
+struct TcSmem {
+  static constexpr int A_TILE = TC_BM * TC_BK * 4;   // 16 KB
+  static constexpr int B_TILE = BN * TC_BK * 4;
+  static constexpr int PLANE_STAGE = (PRESPLIT ? 2 * A_TILE : 0) + 2 * B_TILE;
+  static constexpr int RAW_STAGE = PRESPLIT ? 0 : A_TILE + B_TILE;
+  static constexpr size_t bytes(int raw_stages) {   // + 1024: the ring base is rounded up to 1024 B
+    return (size_t)TC_PLANE_STAGES * PLANE_STAGE + (size_t)raw_stages * RAW_STAGE + 1024;
+  }
+};
+
+// A consumer thread's A-fragment elements in the raw A stage.  `a_frag_base`: byte offset of element 0 of k-step 0 (row
+// r = the thread's fragment row, column lane % 4); `a_frag_ld`: element e of k-step ks, at that offset from the stage.
+//   K-major: SWIZZLE_128B rows of 32 floats, 16-B chunk c of row r at chunk c ^ (r & 7).  The stage is 1024-B aligned, so
+//   bits 4-6 of (stage + base) are r & 7 and chunk c of the same row is (stage + base) ^ (c << 4); row r + 8 is 1024 B
+//   further.  A warp's 8 rows x 4 consecutive k hit 32 distinct banks.
+//   MN-major: [32 k][128 rows] as stored, element (r, k) at (k * 128 + r) * 4.
+// The lane index is re-read from %laneid on every call: held in a register instead, the offset would stay live across
+// the epilogue, which needs all 128 registers at BN = 128.
+template <bool A_MN>
+__device__ __forceinline__ uint32_t a_frag_base(const int warp_row0) {
+  uint32_t lane;
+  asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
+  const int row = warp_row0 + (int)(lane >> 2), col = (int)(lane & 3);
+  if constexpr (A_MN) return (uint32_t)(col * TC_BM + row) * 4u;
+  else return (uint32_t)(row * TC_BK + ((row & 7) << 2) + col) * 4u;
+}
+template <bool A_MN>
+__device__ __forceinline__ float a_frag_ld(const uint32_t at, const int ks, const int e) {
+  uint32_t p;
+  if constexpr (A_MN) p = at + (uint32_t)((8 * ks + 4 * (e >> 1)) * TC_BM + 8 * (e & 1)) * 4u;
+  else p = (at ^ (uint32_t)((2 * ks + (e >> 1)) << 4)) + (uint32_t)(e & 1) * 1024u;
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(p));   // volatile: stays after the raw_full wait
+  return v;
+}
+
 // Persistent, warp-specialised.  `raw_stages` (run-time: 2 or 3) is the depth of the raw ring; the plane ring is two deep.
-// Shared memory: planes 2 x [Ah | Al | Bh | Bl], then (variant 2) raw_stages x [A raw | B raw].
+// Shared memory: planes 2 x TcSmem::PLANE_STAGE, then (variant 2) raw_stages x [A raw | B raw].
 template <int BN, bool A_MN, bool B_MN, bool PRESPLIT, bool ACC>
 __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUtensorMap& tmAl, const CUtensorMap& tmBh,
                                              const CUtensorMap& tmBl, const GemmArgs& a, const int raw_stages,
                                              const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
                                              const int64_t total_items) {
-  constexpr int A_TILE = TC_BM * TC_BK * 4;   // 16 KB
-  constexpr int B_TILE = BN * TC_BK * 4;
-  constexpr int PLANE_STAGE = 2 * A_TILE + 2 * B_TILE;
-  constexpr int RAW_STAGE = A_TILE + B_TILE;
+  using S = TcSmem<BN, PRESPLIT>;
+  constexpr int A_TILE = S::A_TILE, B_TILE = S::B_TILE, PLANE_STAGE = S::PLANE_STAGE, RAW_STAGE = S::RAW_STAGE;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* planes = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* raws = planes + TC_PLANE_STAGES * PLANE_STAGE;
@@ -454,7 +546,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_MAX_RAW_STAGES; ++s) {
       mbar_init(&raw_full[s], 1);                    // the producer's expect_tx arrival
-      mbar_init(&raw_empty[s], TC_SPLITTERS);        // every splitter thread arrives
+      mbar_init(&raw_empty[s], TC_SPLITTERS + TC_CONSUMERS);   // every splitter (B) and consumer (A) thread arrives
     }
     for (int s = 0; s < TC_PLANE_STAGES; ++s) {
       mbar_init(&pl_full[s], PRESPLIT ? 1 : TC_SPLITTERS);
@@ -498,7 +590,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
       }
     }
   } else if (threadIdx.x >= TC_CONSUMERS) {
-    // ===== splitter warps: raw fp32 tile -> TF32 hi / lo planes, K-major =====
+    // ===== splitter warps: raw fp32 B tile -> TF32 hi / lo planes, K-major =====
     if (!PRESPLIT) {
       const int tid = (int)threadIdx.x - TC_CONSUMERS;
       uint32_t it = 0;
@@ -510,8 +602,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
           mbar_wait(&pl_empty[p], ((it / TC_PLANE_STAGES) & 1u) ^ 1u);      // wgmma has finished reading the planes
           const uint8_t* rw = raws + (size_t)s * RAW_STAGE;
           uint8_t* pl = planes + (size_t)p * PLANE_STAGE;
-          split_tile<TC_BM, A_MN>(rw, pl, pl + A_TILE, tid);
-          split_tile<BN, B_MN>(rw + A_TILE, pl + 2 * A_TILE, pl + 2 * A_TILE + B_TILE, tid);
+          split_tile<BN, B_MN>(rw + A_TILE, pl, pl + B_TILE, tid);
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to wgmma
           mbar_arrive(&pl_full[p]);
           mbar_arrive(&raw_empty[s]);
@@ -534,21 +625,56 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
       for (int i = 0; i < t.nkb; ++i, ++it) {
         const int p = (int)(it % TC_PLANE_STAGES);
         mbar_wait(&pl_full[p], (it / TC_PLANE_STAGES) & 1u);
-        const uint32_t sa = smem_u32(planes + (size_t)p * PLANE_STAGE) + (uint32_t)wg * (64u * 128u);
-        const uint32_t sb = smem_u32(planes + (size_t)p * PLANE_STAGE) + 2 * A_TILE;
-        wgmma_fence();
+        if constexpr (PRESPLIT) {
+          const uint32_t sa = smem_u32(planes + (size_t)p * PLANE_STAGE) + (uint32_t)wg * (64u * 128u);
+          const uint32_t sb = smem_u32(planes + (size_t)p * PLANE_STAGE) + 2 * A_TILE;
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < TC_BK / 8; ++k) {
-          const uint64_t dAh = make_smem_desc(sa + k * 32), dAl = make_smem_desc(sa + A_TILE + k * 32);
-          const uint64_t dBh = make_smem_desc(sb + k * 32), dBl = make_smem_desc(sb + B_TILE + k * 32);
-          wgmma_tf32<BN>(d, dAl, dBh);   // small cross terms first
-          wgmma_tf32<BN>(d, dAh, dBl);
-          wgmma_tf32<BN>(d, dAh, dBh);
-        }
-        wgmma_commit();
-        if (i > 0) {                     // the previous k-block has retired: its planes may be overwritten
-          wgmma_wait<1>();
-          mbar_arrive(&pl_empty[p ^ 1]);
+          for (int k = 0; k < TC_BK / 8; ++k) {
+            const uint64_t dAh = make_smem_desc(sa + k * 32), dAl = make_smem_desc(sa + A_TILE + k * 32);
+            const uint64_t dBh = make_smem_desc(sb + k * 32), dBl = make_smem_desc(sb + B_TILE + k * 32);
+            wgmma_tf32<BN>(d, dAl, dBh);   // small cross terms first
+            wgmma_tf32<BN>(d, dAh, dBl);
+            wgmma_tf32<BN>(d, dAh, dBh);
+          }
+          wgmma_commit();
+          if (i > 0) {                     // the previous k-block has retired: its planes may be overwritten
+            wgmma_wait<1>();
+            mbar_arrive(&pl_empty[p ^ 1]);
+          }
+        } else {
+          // A straight from the raw stage: each thread splits its own fragment elements as split_tile does and feeds
+          // them to wgmma from registers, one commit group per k-step.  The fragment is rewritten only after the
+          // previous k-step has retired (wait_group 0); the other consumer warpgroup keeps the tensor cores busy
+          // meanwhile, and each k-step's loads are issued before its wait.  A two-buffer form (wait_group 1 after each
+          // commit) compiles to the same 128 registers, measured no faster on H100, and produced wrong dX values in
+          // the full-size Dense test (K = 32, N = 256), for a reason not yet found.
+          const int s = (int)(it % (uint32_t)raw_stages);
+          mbar_wait(&raw_full[s], (it / (uint32_t)raw_stages) & 1u);
+          const uint32_t at = smem_u32(raws + (size_t)s * RAW_STAGE) + a_frag_base<A_MN>(wg * 64 + (warp & 3) * 16);
+          const uint32_t sb = smem_u32(planes + (size_t)p * PLANE_STAGE);
+#pragma unroll
+          for (int k = 0; k < TC_BK / 8; ++k) {
+            float v[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) v[e] = a_frag_ld<A_MN>(at, k, e);
+            wgmma_wait<0>();
+            if (k == 0 && i > 0) mbar_arrive(&pl_empty[p ^ 1]);   // k-block i - 1 has retired: its B planes are free
+            uint32_t ah[4], al[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float h = __uint_as_float(__float_as_uint(v[e]) & 0xFFFFE000u);
+              ah[e] = __float_as_uint(h);
+              al[e] = __float_as_uint(v[e] - h);
+            }
+            if (k + 1 == TC_BK / 8) mbar_arrive(&raw_empty[s]);   // every A element of the stage is in registers
+            const uint64_t dBh = make_smem_desc(sb + k * 32), dBl = make_smem_desc(sb + B_TILE + k * 32);
+            wgmma_fence();
+            wgmma_tf32_ra<BN>(d, al, dBh);   // small cross terms first, as in variant 1
+            wgmma_tf32_ra<BN>(d, ah, dBl);
+            wgmma_tf32_ra<BN>(d, ah, dBh);
+            wgmma_commit();
+          }
         }
       }
       wgmma_wait<0>();
@@ -560,7 +686,8 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
 }
 
 // Registers are allocated to warps in groups of four, so 13 warps count as 16: 65536 / 512 = 128 registers per thread.
-// The BN = 128 instantiations hold 64 accumulators and use all 128 without spilling.
+// The BN = 128 instantiations hold 64 accumulators and use all 128.  The variant-2 ones (A split in registers) spill one
+// 4-byte value: stored once before the consumers' tile loop and reloaded once after it, outside the k-loop.
 template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
@@ -668,9 +795,9 @@ int g_tune_tc_pair = 1;      // accepted and read back for callers that set it; 
 
 template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
 static int launch_tc(const CUtensorMap* tms, const GemmArgs& a, int raw_stages, cudaStream_t st) {
-  constexpr int PLANE_STAGE = 2 * TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4;
-  const size_t smem = (size_t)TC_PLANE_STAGES * PLANE_STAGE + (PRESPLIT ? 0 : (size_t)raw_stages * (PLANE_STAGE / 2)) + 1024;
-  static_assert((size_t)TC_PLANE_STAGES * PLANE_STAGE + 3 * (PLANE_STAGE / 2) + 1024 + 256 <= 232448,
+  using S = TcSmem<BN, PRESPLIT>;
+  const size_t smem = S::bytes(raw_stages);
+  static_assert(S::bytes(TC_MAX_RAW_STAGES) + 256 <= 232448,
                 "plane ring + raw ring exceed the 227 KB of shared memory per CTA");
   auto k = gemm_tc_kernel<BN, A_MN, B_MN, PRESPLIT>;
   if constexpr (!A_MN && !B_MN && BN <= 64) {
