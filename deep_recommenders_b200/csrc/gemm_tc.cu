@@ -25,6 +25,12 @@
 // Variant 1 (g_tune_gemm_variant == 1, PRESPLIT): the hi/lo planes of both operands are produced K-major in
 // caller-provided workspace (dr_set_workspace) by split_tf32_kernel / split_tf32_transpose_kernel and TMA loads them
 // straight into the plane ring; variant 2 (the default) needs no workspace and no pre-pass.
+// Weight planes (gemm_tc_wplanes_kernel, variant 2 with the plane cache on, A K-major, B small against A): B's K-major
+// hi/lo planes are split once per step into the workspace and TMA loads them beside the raw A tile into one ring
+// [A raw | Bh | Bl]; A is split in registers as in variant 2.  No splitter warps, no plane ring: 288 threads, and a stage
+// is released once its k-block's MMAs have retired.  A tile whose valid width is at most 32 or 64 columns runs
+// m64n32k8 / m64n64k8 MMAs into the leading accumulators.
+// In every kernel a consumer warpgroup whose 64 rows all lie past M issues no loads, MMAs or epilogue for that tile.
 #include "gemm.cuh"
 #include <cuda.h>
 #include <float.h>
@@ -56,8 +62,10 @@ constexpr int TC_BK = 32;          // 32 tf32 = 128 bytes = one SWIZZLE_128B row
 constexpr int TC_CONSUMERS = 256;  // two warpgroups
 constexpr int TC_SPLITTERS = 128;
 constexpr int TC_THREADS = TC_CONSUMERS + TC_SPLITTERS + 32;
+constexpr int TC_WP_THREADS = TC_CONSUMERS + 32;   // weight-plane kernel: consumers + TMA warp
 constexpr int TC_PLANE_STAGES = 2;
 constexpr int TC_MAX_RAW_STAGES = 4;
+constexpr int TC_WP_STAGES = 4;                    // ring depth of the weight-plane kernel
 
 // ---- small PTX wrappers ----------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -487,13 +495,14 @@ __device__ __forceinline__ void tc_epilogue_acc(const GemmArgs& a, const float (
 }
 
 // Shared-memory stages of one tile width.  The plane ring holds [Ah | Al | Bh | Bl] in variant 1 and [Bh | Bl] in
-// variant 2, whose consumers split A in registers; the raw ring (variant 2 only) holds [A raw | B raw].
-template <int BN, bool PRESPLIT>
+// variant 2, whose consumers split A in registers; the raw ring (variant 2 only) holds [A raw | B raw], or
+// [A raw | Bh | Bl] in the weight-plane kernel, which has no plane ring.
+template <int BN, bool PRESPLIT, bool WPLANES = false>
 struct TcSmem {
   static constexpr int A_TILE = TC_BM * TC_BK * 4;   // 16 KB
   static constexpr int B_TILE = BN * TC_BK * 4;
-  static constexpr int PLANE_STAGE = (PRESPLIT ? 2 * A_TILE : 0) + 2 * B_TILE;
-  static constexpr int RAW_STAGE = PRESPLIT ? 0 : A_TILE + B_TILE;
+  static constexpr int PLANE_STAGE = WPLANES ? 0 : (PRESPLIT ? 2 * A_TILE : 0) + 2 * B_TILE;
+  static constexpr int RAW_STAGE = PRESPLIT ? 0 : A_TILE + (WPLANES ? 2 : 1) * B_TILE;
   static constexpr size_t bytes(int raw_stages) {   // + 1024: the ring base is rounded up to 1024 B
     return (size_t)TC_PLANE_STAGES * PLANE_STAGE + (size_t)raw_stages * RAW_STAGE + 1024;
   }
@@ -525,15 +534,22 @@ __device__ __forceinline__ float a_frag_ld(const uint32_t at, const int ks, cons
   return v;
 }
 
-// Persistent, warp-specialised.  `raw_stages` (run-time: 2 or 3) is the depth of the raw ring; the plane ring is two deep.
+template <int N>
+struct TcWidth { static constexpr int value = N; };
+
+// Persistent, warp-specialised.  `raw_stages` (run-time: 2 to 4) is the depth of the raw ring; the plane ring is two deep.
 // Shared memory: planes 2 x TcSmem::PLANE_STAGE, then (variant 2) raw_stages x [A raw | B raw].
-template <int BN, bool A_MN, bool B_MN, bool PRESPLIT, bool ACC>
+// WPLANES (A and B K-major, !PRESPLIT): the ring is raw_stages x [A raw | Bh | Bl] with B's planes loaded by TMA
+// (tmBh / tmBl); the threads are the consumers and the TMA warp only.
+template <int BN, bool A_MN, bool B_MN, bool PRESPLIT, bool ACC, bool WPLANES = false>
 __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUtensorMap& tmAl, const CUtensorMap& tmBh,
                                              const CUtensorMap& tmBl, const GemmArgs& a, const int raw_stages,
                                              const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
                                              const int64_t total_items) {
-  using S = TcSmem<BN, PRESPLIT>;
+  static_assert(!WPLANES || (!PRESPLIT && !A_MN && !B_MN && !ACC), "weight planes: K-major A split in registers");
+  using S = TcSmem<BN, PRESPLIT, WPLANES>;
   constexpr int A_TILE = S::A_TILE, B_TILE = S::B_TILE, PLANE_STAGE = S::PLANE_STAGE, RAW_STAGE = S::RAW_STAGE;
+  constexpr int PRODUCER_WARP = (TC_CONSUMERS + (WPLANES ? 0 : TC_SPLITTERS)) / 32;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* planes = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* raws = planes + TC_PLANE_STAGES * PLANE_STAGE;
@@ -546,7 +562,8 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_MAX_RAW_STAGES; ++s) {
       mbar_init(&raw_full[s], 1);                    // the producer's expect_tx arrival
-      mbar_init(&raw_empty[s], TC_SPLITTERS + TC_CONSUMERS);   // every splitter (B) and consumer (A) thread arrives
+      // every splitter (B) and consumer (A) thread arrives; with weight planes, every consumer once the stage has retired
+      mbar_init(&raw_empty[s], (WPLANES ? 0 : TC_SPLITTERS) + TC_CONSUMERS);
     }
     for (int s = 0; s < TC_PLANE_STAGES; ++s) {
       mbar_init(&pl_full[s], PRESPLIT ? 1 : TC_SPLITTERS);
@@ -557,11 +574,12 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
   }
   __syncthreads();
 
-  if (warp == (TC_CONSUMERS + TC_SPLITTERS) / 32) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       // ===== TMA producer =====
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAh) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBh) : "memory");
+      if (WPLANES) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBl) : "memory");
       uint32_t it = 0;
       for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
         const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
@@ -585,13 +603,14 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
             else tma_load_2d(st, &tmAh, &raw_full[s], (int)t.m0, k);
             if (!B_MN) tma_load_2d(st + A_TILE, &tmBh, &raw_full[s], k, (int)t.n0);
             else tma_load_2d(st + A_TILE, &tmBh, &raw_full[s], (int)t.n0, k);
+            if (WPLANES) tma_load_2d(st + A_TILE + B_TILE, &tmBl, &raw_full[s], k, (int)t.n0);
           }
         }
       }
     }
   } else if (threadIdx.x >= TC_CONSUMERS) {
     // ===== splitter warps: raw fp32 B tile -> TF32 hi / lo planes, K-major =====
-    if (!PRESPLIT) {
+    if (!PRESPLIT && !WPLANES) {
       const int tid = (int)threadIdx.x - TC_CONSUMERS;
       uint32_t it = 0;
       for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
@@ -619,13 +638,73 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
     uint32_t it = 0;
     for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
       const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
+      if (t.m0 + wg * 64 >= a.M) {
+        // M tail: none of this warpgroup's rows is in range.  It only makes the arrivals the other warps' waits count,
+        // each after the wait that opens its phase, so that no arrival lands in an earlier phase.
+        for (int i = 0; i < t.nkb; ++i, ++it) {
+          const int p = (int)(it % TC_PLANE_STAGES);
+          if (!WPLANES) mbar_wait(&pl_full[p], (it / TC_PLANE_STAGES) & 1u);
+          if (!PRESPLIT) {   // variant 1 has no raw ring (raw_stages = 0)
+            const int s = (int)(it % (uint32_t)raw_stages);
+            mbar_wait(&raw_full[s], (it / (uint32_t)raw_stages) & 1u);
+            mbar_arrive(&raw_empty[s]);
+          }
+          if (!WPLANES) mbar_arrive(&pl_empty[p]);
+        }
+        continue;
+      }
       float d[BN / 2];
 #pragma unroll
       for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
-      for (int i = 0; i < t.nkb; ++i, ++it) {
-        const int p = (int)(it % TC_PLANE_STAGES);
-        mbar_wait(&pl_full[p], (it / TC_PLANE_STAGES) & 1u);
-        if constexpr (PRESPLIT) {
+      // k-blocks of the in-register A split, NW-wide MMAs into the leading NW / 2 accumulators (NW < BN: the tile's
+      // valid columns all lie in the first NW, the other accumulators stay zero)
+      auto kblocks_ra = [&](auto width) {
+        constexpr int NW = decltype(width)::value;
+        float (&dn)[NW / 2] = reinterpret_cast<float (&)[NW / 2]>(d);
+        for (int i = 0; i < t.nkb; ++i, ++it) {
+          // A straight from the raw stage: each thread splits its own fragment elements as split_tile does and feeds
+          // them to wgmma from registers, one commit group per k-step.  The fragment is rewritten only after the
+          // previous k-step has retired (wait_group 0); the other consumer warpgroup keeps the tensor cores busy
+          // meanwhile, and each k-step's loads are issued before its wait.  A two-buffer form (wait_group 1 after each
+          // commit) compiles to the same 128 registers, measured no faster on H100, and produced wrong dX values in
+          // the full-size Dense test (K = 32, N = 256), for a reason not yet found.
+          const int s = (int)(it % (uint32_t)raw_stages), p = (int)(it % TC_PLANE_STAGES);
+          if (!WPLANES) mbar_wait(&pl_full[p], (it / TC_PLANE_STAGES) & 1u);
+          mbar_wait(&raw_full[s], (it / (uint32_t)raw_stages) & 1u);
+          const uint32_t at = smem_u32(raws + (size_t)s * RAW_STAGE) + a_frag_base<A_MN>(wg * 64 + (warp & 3) * 16);
+          const uint32_t sb = WPLANES ? smem_u32(raws + (size_t)s * RAW_STAGE) + A_TILE
+                                      : smem_u32(planes + (size_t)p * PLANE_STAGE);
+#pragma unroll
+          for (int k = 0; k < TC_BK / 8; ++k) {
+            float v[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) v[e] = a_frag_ld<A_MN>(at, k, e);
+            wgmma_wait<0>();
+            if (k == 0 && i > 0) {   // k-block i - 1 has retired: its B planes (its whole stage, WPLANES) are free
+              if (WPLANES) mbar_arrive(&raw_empty[(it - 1) % (uint32_t)raw_stages]);
+              else mbar_arrive(&pl_empty[p ^ 1]);
+            }
+            uint32_t ah[4], al[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float h = __uint_as_float(__float_as_uint(v[e]) & 0xFFFFE000u);
+              ah[e] = __float_as_uint(h);
+              al[e] = __float_as_uint(v[e] - h);
+            }
+            if (!WPLANES && k + 1 == TC_BK / 8) mbar_arrive(&raw_empty[s]);   // every A element of the stage is in registers
+            const uint64_t dBh = make_smem_desc(sb + k * 32), dBl = make_smem_desc(sb + B_TILE + k * 32);
+            wgmma_fence();
+            wgmma_tf32_ra<NW>(dn, al, dBh);   // small cross terms first, as in variant 1
+            wgmma_tf32_ra<NW>(dn, ah, dBl);
+            wgmma_tf32_ra<NW>(dn, ah, dBh);
+            wgmma_commit();
+          }
+        }
+      };
+      if constexpr (PRESPLIT) {
+        for (int i = 0; i < t.nkb; ++i, ++it) {
+          const int p = (int)(it % TC_PLANE_STAGES);
+          mbar_wait(&pl_full[p], (it / TC_PLANE_STAGES) & 1u);
           const uint32_t sa = smem_u32(planes + (size_t)p * PLANE_STAGE) + (uint32_t)wg * (64u * 128u);
           const uint32_t sb = smem_u32(planes + (size_t)p * PLANE_STAGE) + 2 * A_TILE;
           wgmma_fence();
@@ -642,43 +721,20 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
             wgmma_wait<1>();
             mbar_arrive(&pl_empty[p ^ 1]);
           }
-        } else {
-          // A straight from the raw stage: each thread splits its own fragment elements as split_tile does and feeds
-          // them to wgmma from registers, one commit group per k-step.  The fragment is rewritten only after the
-          // previous k-step has retired (wait_group 0); the other consumer warpgroup keeps the tensor cores busy
-          // meanwhile, and each k-step's loads are issued before its wait.  A two-buffer form (wait_group 1 after each
-          // commit) compiles to the same 128 registers, measured no faster on H100, and produced wrong dX values in
-          // the full-size Dense test (K = 32, N = 256), for a reason not yet found.
-          const int s = (int)(it % (uint32_t)raw_stages);
-          mbar_wait(&raw_full[s], (it / (uint32_t)raw_stages) & 1u);
-          const uint32_t at = smem_u32(raws + (size_t)s * RAW_STAGE) + a_frag_base<A_MN>(wg * 64 + (warp & 3) * 16);
-          const uint32_t sb = smem_u32(planes + (size_t)p * PLANE_STAGE);
-#pragma unroll
-          for (int k = 0; k < TC_BK / 8; ++k) {
-            float v[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) v[e] = a_frag_ld<A_MN>(at, k, e);
-            wgmma_wait<0>();
-            if (k == 0 && i > 0) mbar_arrive(&pl_empty[p ^ 1]);   // k-block i - 1 has retired: its B planes are free
-            uint32_t ah[4], al[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float h = __uint_as_float(__float_as_uint(v[e]) & 0xFFFFE000u);
-              ah[e] = __float_as_uint(h);
-              al[e] = __float_as_uint(v[e] - h);
-            }
-            if (k + 1 == TC_BK / 8) mbar_arrive(&raw_empty[s]);   // every A element of the stage is in registers
-            const uint64_t dBh = make_smem_desc(sb + k * 32), dBl = make_smem_desc(sb + B_TILE + k * 32);
-            wgmma_fence();
-            wgmma_tf32_ra<BN>(d, al, dBh);   // small cross terms first, as in variant 1
-            wgmma_tf32_ra<BN>(d, ah, dBl);
-            wgmma_tf32_ra<BN>(d, ah, dBh);
-            wgmma_commit();
-          }
         }
+      } else if constexpr (WPLANES && BN > 32) {
+        // N tail: the last n-tile of N = 416 at BN = 128 has 32 valid columns.  One MMA width per tile, each with a
+        // k-loop of its own, so the loop carries no width test.
+        const int64_t w = a.N - t.n0;
+        if (w <= 32) kblocks_ra(TcWidth<32>{});
+        else if (BN > 64 && w <= 64) kblocks_ra(TcWidth<64>{});
+        else kblocks_ra(TcWidth<BN>{});
+      } else {
+        kblocks_ra(TcWidth<BN>{});
       }
       wgmma_wait<0>();
-      mbar_arrive(&pl_empty[(it - 1) % TC_PLANE_STAGES]);
+      if (WPLANES) mbar_arrive(&raw_empty[(it - 1) % (uint32_t)raw_stages]);
+      else mbar_arrive(&pl_empty[(it - 1) % TC_PLANE_STAGES]);
       if constexpr (ACC) tc_epilogue_acc<BN>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane);
       else tc_epilogue<BN>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane, vec_ok);
     }
@@ -705,6 +761,18 @@ gemm_tc_acc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
                    const int raw_stages, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
                    const int64_t total_items) {
   gemm_tc_body<BN, false, false, PRESPLIT, true>(tmAh, tmAl, tmBh, tmBl, a, raw_stages, m_tiles, n_tiles, per, total_items);
+}
+
+// Weight planes: K-major raw A (tmAh) split in registers, B's K-major hi / lo planes (tmBh / tmBl) from the workspace.
+// 9 warps count as 12 for register allocation: up to 168 registers per thread, so the BN = 128 epilogue does not spill.
+template <int BN>
+__global__ void __launch_bounds__(TC_WP_THREADS, 1)
+gemm_tc_wplanes_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+                       const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
+                       const GemmArgs a, const int raw_stages, const int64_t m_tiles, const int64_t n_tiles,
+                       const int64_t per, const int64_t total_items) {
+  gemm_tc_body<BN, false, false, false, false, true>(tmAh, tmAl, tmBh, tmBl, a, raw_stages, m_tiles, n_tiles, per,
+                                                     total_items);
 }
 
 // ---- host side ---------------------------------------------------------------------------------------
@@ -793,14 +861,15 @@ bool gemm_tc_eligible(const GemmArgs& a, bool ta, bool tb) {
 int g_tune_tc_stages = 0;    // 0 = three raw stages; 2 = two (32 KB less shared memory at the widest tile)
 int g_tune_tc_pair = 1;      // accepted and read back for callers that set it; H100 has no two-CTA MMA, so it selects nothing
 
-template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
+template <int BN, bool A_MN, bool B_MN, bool PRESPLIT, bool WPLANES = false>
 static int launch_tc(const CUtensorMap* tms, const GemmArgs& a, int raw_stages, cudaStream_t st) {
-  using S = TcSmem<BN, PRESPLIT>;
+  using S = TcSmem<BN, PRESPLIT, WPLANES>;
   const size_t smem = S::bytes(raw_stages);
   static_assert(S::bytes(TC_MAX_RAW_STAGES) + 256 <= 232448,
                 "plane ring + raw ring exceed the 227 KB of shared memory per CTA");
   auto k = gemm_tc_kernel<BN, A_MN, B_MN, PRESPLIT>;
-  if constexpr (!A_MN && !B_MN && BN <= 64) {
+  if constexpr (WPLANES) k = gemm_tc_wplanes_kernel<BN>;
+  if constexpr (!A_MN && !B_MN && BN <= 64 && !WPLANES) {
     if (a.epi == EPI_CROSS_DX_ACC) k = gemm_tc_acc_kernel<BN, PRESPLIT>;
   }
   DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -810,7 +879,8 @@ static int launch_tc(const CUtensorMap* tms, const GemmArgs& a, int raw_stages, 
   const int64_t splits = (kblocks + per - 1) / per;          // every split owns >= 1 k-block
   const int64_t total = m_tiles * n_tiles * splits;
   const int64_t ctas = total < (int64_t)num_sms() ? total : (int64_t)num_sms();
-  k<<<(unsigned)ctas, TC_THREADS, smem, st>>>(tms[0], tms[1], tms[2], tms[3], a, raw_stages, m_tiles, n_tiles, per, total);
+  k<<<(unsigned)ctas, WPLANES ? TC_WP_THREADS : TC_THREADS, smem, st>>>(tms[0], tms[1], tms[2], tms[3], a, raw_stages,
+                                                                         m_tiles, n_tiles, per, total);
   DR_CUDA_LAUNCH_CHECK("gemm_tc");
   return DR_OK;
 }
@@ -852,6 +922,46 @@ int gemm_tc_launch(const GemmArgs& a0, bool ta, bool tb, cudaStream_t st) {
   // fit the 128-register cap without spilling, so it runs 128 x 64 tiles at most
   if (a.epi == EPI_CROSS_DX_ACC && bn == 128) bn = 64;
   CUtensorMap tms[4];
+  size_t ae, be;
+  plane_elems(a, ta, tb, &ae, &be);
+  auto planes = [&](const float* src, size_t elems, bool transposed, int64_t rows, int64_t ld, float** hi, float** lo,
+                    int64_t* pitch) -> int {
+    if (g_cache_on)
+      if (const PlaneEntry* e = plane_cached(src, transposed, rows, a.K, ld)) {
+        *hi = e->hi; *lo = e->lo; *pitch = e->pitch;
+        return DR_OK;
+      }
+    DR_REQUIRE(g_ws_ptr && (g_bump + 2 * elems) * sizeof(float) <= g_ws_bytes, DR_EINVAL,
+               "gemm_tc: workspace exhausted (%zu B registered)", g_ws_bytes);
+    *hi = reinterpret_cast<float*>(g_ws_ptr) + g_bump;
+    *lo = *hi + elems;
+    g_bump += 2 * elems;
+    if (int rc = make_planes(src, !transposed, rows, a.K, ld, *hi, *lo, pitch, st)) return rc;
+    if (g_cache_on && g_nplanes < 64)
+      g_planes[g_nplanes++] = PlaneEntry{src, transposed, rows, a.K, ld, *hi, *lo, *pitch};
+    return DR_OK;
+  };
+  // Weight planes: inside a train step (plane cache on) B is split once and read by every m-tile, instead of being split
+  // again by every tile's splitters.  Taken when B is small against A (N <= M / 16: the forward and dX of a Dense layer
+  // over a batch, where each plane element is reused by at least M / 128 >= N / 8 tiles and the split pass over B moves
+  // at most 3/16 of A's bytes) and A is K-major.  Only for 128-wide tiles (N > 64) with more than one k-block (K > 32):
+  // on H100 the 256 -> 32 layer's forward (N = 32) and dX (K = 32), where the splitters do little per tile, measured
+  // about 1 us slower with the extra split launch than without.  A K-major B is split flat over rows x ldb floats, so its
+  // pitch must be K.  The dW (A transposed) and the accumulating Cross dX keep the splitter kernels.
+  if (g_tune_gemm_variant == 2 && g_cache_on && !ta && a.epi != EPI_CROSS_DX_ACC && a.N * 16 <= a.M && a.N > 64 &&
+      a.K > TC_BK && (!tb || a.ldb == a.K) &&
+      (plane_cached(a.B, !tb, a.N, a.K, a.ldb) || (g_ws_ptr && (g_bump + 2 * be) * sizeof(float) <= g_ws_bytes))) {
+    float *Bh, *Bl;
+    int64_t pb = 0;
+    if (int rc = planes(a.B, be, !tb, a.N, a.ldb, &Bh, &Bl, &pb)) return rc;
+    if (int rc = make_map(&tms[0], a.A, a.K, a.M, a.lda, TC_BK, TC_BM, true)) return rc;
+    if (int rc = make_map(&tms[2], Bh, a.K, a.N, pb, TC_BK, bn, true)) return rc;
+    if (int rc = make_map(&tms[3], Bl, a.K, a.N, pb, TC_BK, bn, true)) return rc;
+    tms[1] = tms[0];
+    if (bn == 32) return launch_tc<32, false, false, false, true>(tms, a, TC_WP_STAGES, st);
+    if (bn == 64) return launch_tc<64, false, false, false, true>(tms, a, TC_WP_STAGES, st);
+    return launch_tc<128, false, false, false, true>(tms, a, TC_WP_STAGES, st);
+  }
   if (g_tune_gemm_variant == 2) {
     // Variant 2: tensor maps straight on the source operands (staged as stored), split in shared memory.
     const bool A_MN = ta, B_MN = !tb;
@@ -882,26 +992,7 @@ int gemm_tc_launch(const GemmArgs& a0, bool ta, bool tb, cudaStream_t st) {
   }
   // Variant 1: K-major hi/lo planes in the workspace.  A(m,k): !ta -> stored [M,K] (flat split), ta -> stored [K,M]
   // (transposing split); B(k,n): tb -> stored [N,K] (flat), !tb -> stored [K,N] (transposing).
-  size_t ae, be;
-  plane_elems(a, ta, tb, &ae, &be);
   if (!g_cache_on) g_bump = 0;
-  auto planes = [&](const float* src, size_t elems, bool transposed, int64_t rows, int64_t ld, float** hi, float** lo,
-                    int64_t* pitch) -> int {
-    if (g_cache_on)
-      if (const PlaneEntry* e = plane_cached(src, transposed, rows, a.K, ld)) {
-        *hi = e->hi; *lo = e->lo; *pitch = e->pitch;
-        return DR_OK;
-      }
-    DR_REQUIRE(g_ws_ptr && (g_bump + 2 * elems) * sizeof(float) <= g_ws_bytes, DR_EINVAL,
-               "gemm_tc: workspace exhausted (%zu B registered)", g_ws_bytes);
-    *hi = reinterpret_cast<float*>(g_ws_ptr) + g_bump;
-    *lo = *hi + elems;
-    g_bump += 2 * elems;
-    if (int rc = make_planes(src, !transposed, rows, a.K, ld, *hi, *lo, pitch, st)) return rc;
-    if (g_cache_on && g_nplanes < 64)
-      g_planes[g_nplanes++] = PlaneEntry{src, transposed, rows, a.K, ld, *hi, *lo, *pitch};
-    return DR_OK;
-  };
   float *Ah, *Al, *Bh, *Bl;
   int64_t pa = 0, pb = 0;
   if (int rc = planes(a.A, ae, ta, a.M, a.lda, &Ah, &Al, &pa)) return rc;

@@ -9,7 +9,12 @@ Then the layer-0 forward (M = 65536, N = 256, 128 x 128 tiles) is swept over K u
 dr_debug_gemm) and under bias + relu (EPI_BIAS_ACT, through dr_dense_fwd).  Every CTA of the persistent grid owns the
 same number of tiles, so time = tiles per CTA x (fixed cost per tile + K / 32 x cost per k-block): the least-squares
 line through (k-blocks, time) gives the fixed per-tile cost as its intercept and the per-k-block cost as its slope.
-usage: bench_gemm_shapes.py [KEY=VALUE ...]   -> one JSON line per shape, one per swept epilogue, one for the card"""
+
+cache=1 times every GEMM as a train step runs it: the plane cache is switched on (and emptied) before each call, so the
+forward and dX take B's hi / lo planes from the workspace (gemm_tc_wplanes_kernel) and each call pays for its own split of
+B, as the step pays once per layout of each weight.  cache=0 (the default) is the in-kernel split of every call.
+usage: bench_gemm_shapes.py [cache=0|1] [KEY=VALUE ...]   -> one JSON line per shape, one per swept epilogue, one for
+the card"""
 import json
 import os
 import subprocess
@@ -21,11 +26,14 @@ import torch
 from deep_recommenders_b200 import _lib
 from deep_recommenders_b200._lib import check
 
-knobs = [a for a in sys.argv[1:] if "=" in a]
+knobs = [a for a in sys.argv[1:] if "=" in a and not a.startswith("cache=")]
+CACHE = any(a == "cache=1" for a in sys.argv[1:])
 for kv in knobs:
     k, v = kv.split("=")
     _lib.tune(k, int(v))
 lib = _lib.load()
+if CACHE:
+    _lib.set_workspace(256 << 20)
 dev = torch.device("cuda", 0)
 SHAPES = [(65536, 416, 256), (65536, 256, 32), (8192, 3328, 512), (16384, 3328, 512), (65536, 3328, 512),
           (8192, 512, 256)]
@@ -45,6 +53,12 @@ def card():
 
 
 def timed(fn, iters=6):
+    if CACHE:
+        fn0 = fn
+
+        def fn(i):
+            check(lib.dr_gemm_plane_cache(1), "plane cache")   # empty: this call splits its own B
+            fn0(i)
     for i in range(2):
         fn(i)
     torch.cuda.synchronize()
@@ -57,7 +71,7 @@ def timed(fn, iters=6):
     return e0.elapsed_time(e1) / iters * 1e3
 
 
-print(json.dumps({"card": card(), "knobs": knobs}), flush=True)
+print(json.dumps({"card": card(), "knobs": knobs, "cache": CACHE}), flush=True)
 st = torch.cuda.current_stream().cuda_stream
 for M, K, N in SHAPES:
     xs = [torch.randn(M, K, device=dev).relu_() for _ in range(R)]     # a layer's input is the relu output below it
@@ -78,7 +92,7 @@ for M, K, N in SHAPES:
                                           None, gw.data_ptr(), None, st), "dw")
     t = {"fwd_us": timed(fwd), "dx_us": timed(dx), "dx_chain_us": timed(dx_chain), "dw_us": timed(dw)}
     fl = 2.0 * M * K * N
-    print(json.dumps({"M": M, "K": K, "N": N, "knobs": knobs, **{k: round(v, 1) for k, v in t.items()},
+    print(json.dumps({"M": M, "K": K, "N": N, "knobs": knobs, "cache": CACHE, **{k: round(v, 1) for k, v in t.items()},
                       **{k.replace("_us", "_tflops"): round(fl / v / 1e6, 1) for k, v in t.items()}}), flush=True)
     del xs, gys, ys, gxs
     torch.cuda.empty_cache()
@@ -108,9 +122,11 @@ for epi in ("store", "bias_relu"):
     kb = np.array(SWEEP_K, dtype=np.float64) / 32
     slope, icpt = np.polyfit(kb, np.array(times), 1)
     t_full = times[SWEEP_K.index(416)]
-    print(json.dumps({"sweep": "layer0_fwd", "epi": epi, "M": M, "N": N, "K": SWEEP_K,
+    print(json.dumps({"sweep": "layer0_fwd", "epi": epi, "cache": CACHE, "M": M, "N": N, "K": SWEEP_K,
                       "us": [round(v, 1) for v in times], "tiles_per_cta": tiles_per_cta,
                       "intercept_us": round(icpt, 1), "slope_us_per_kblock": round(slope, 2),
                       "per_tile_fixed_us": round(icpt / tiles_per_cta, 2),
                       "per_kblock_per_tile_us": round(slope / tiles_per_cta, 3),
                       "intercept_share_of_K416": round(icpt / t_full, 3)}), flush=True)
+if CACHE:
+    check(lib.dr_gemm_plane_cache(0), "plane cache")
