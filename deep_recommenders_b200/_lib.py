@@ -63,6 +63,8 @@ _SIGS = {
     "dr_add_layernorm_bwd": [_p, _p, _p, _p, _i64, _i, _f, _p, _p, _p, _p],
     "dr_softmax_rows_fwd": [_p, _i64, _i, _p, _p],
     "dr_softmax_rows_bwd": [_p, _p, _i64, _i, _p, _p],
+    "dr_spmm_csr_fwd": [_p, _p, _p, _i64, _i64, _i64, _p, _i, _p, _p, _i, _p, _p, _p],
+    "dr_act_bwd_colsum": [_p, _p, _i64, _i, _i, _p, _p, _p],
     "dr_moe_mix_fwd": [_p, _p, _i64, _i, _i, _i, _p, _p, _p],
     "dr_moe_mix_bwd": [_p, _p, _p, _i64, _i, _i, _i, _p, _p, _p],
     "dr_inbatch_softmax_fwd": [_p, _p, _p, _p, _p, _f, _i64, _i64, _i, _p, _p, _p],

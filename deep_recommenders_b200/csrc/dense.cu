@@ -350,6 +350,20 @@ extern "C" int dr_dense_bwd_chain(const float* x, const float* w, const float* y
   return dense_bwd_impl(x, w, y, gy, M, K, N, act, gz_ws, gx, gw, gb, prev_y, prev_act, (cudaStream_t)stream);
 }
 
+// The activation-gradient and bias-gradient pass of dense_bwd_impl on its own, for an epilogue fused into a kernel other
+// than the GEMM (the SpMM of spmm.cu), whose backward needs this pass and no GEMM.
+extern "C" int dr_act_bwd_colsum(const float* y, const float* gy, int64_t M, int N, int act, float* gz, float* gb,
+                                 void* stream) {
+  DR_REQUIRE(M >= 0 && N >= 1, DR_EINVAL, "dr_act_bwd_colsum: bad shape M=%lld N=%d", (long long)M, N);
+  DR_REQUIRE(act >= DR_ACT_NONE && act <= DR_ACT_TANH, DR_EINVAL, "dr_act_bwd_colsum: unknown activation %d", act);
+  DR_REQUIRE(M == 0 || gy, DR_EINVAL, "dr_act_bwd_colsum: null pointer");
+  DR_REQUIRE(act == DR_ACT_NONE || M == 0 || (y && gz), DR_EINVAL, "dr_act_bwd_colsum: activation needs y and gz");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (gb) DR_CUDA_CALL(cudaMemsetAsync(gb, 0, sizeof(float) * N, st));
+  if (M == 0 || (act == DR_ACT_NONE && !gb)) return DR_OK;
+  return launch_actgrad_colsum(gy, y, act, M, N, rows_per_cta_for(M), gz, gb, st);
+}
+
 // G Dense layers of one shape on column blocks: x [M, G*K], w [G, K, N], b [G, N], y [M, G*N].  Group g is the plain
 // Dense call on x[:, g*K ..] and y[:, g*N ..], run as one strided GEMM per group (the TMA path takes the strides when
 // it can, the eligibility check sends the others to FFMA).

@@ -120,6 +120,32 @@ class Recall(_Confusion):
         return 0.0 if self.tp is None else float(self.tp[0] / (self.tp[0] + self.fn[0]).clamp_min(1e-12))
 
 
+class WeightedAccuracy:
+    """The "acc" of ``compile(weighted_metrics=["acc"])``: sum(w * correct) / sum(w) over the rows seen, where
+    correct is argmax agreement under categorical cross-entropy (Keras's categorical accuracy) and agreement of the
+    0.5-thresholded prediction otherwise (binary accuracy).  w is the sample weight (1 when none is given)."""
+
+    def __init__(self, name: str = "acc", categorical: bool = True):
+        self.name, self.categorical = name, categorical
+        self.reset_state()
+
+    def reset_state(self):
+        self.hits = self.total = None
+
+    def update_state(self, y_true, y_pred, sample_weight=None):
+        if self.categorical:
+            correct = (y_pred.argmax(dim=-1) == y_true.argmax(dim=-1)).double()
+        else:
+            correct = ((y_pred > 0.5) == (y_true > 0.5)).double().reshape(y_pred.shape[0], -1).mean(dim=-1)
+        w = correct.new_ones(correct.shape) if sample_weight is None else sample_weight.double().reshape(-1)
+        add = lambda old, new: new if old is None else old + new
+        self.hits = add(self.hits, (w * correct).sum())
+        self.total = add(self.total, w.sum())
+
+    def result(self) -> float:
+        return 0.0 if self.total is None or float(self.total) == 0.0 else float(self.hits / self.total)
+
+
 # ---- tf.keras.callbacks -------------------------------------------------------------------------------------------
 class EarlyStopping:
     """tf.keras.callbacks.EarlyStopping(monitor="val_loss", patience=0, min_delta=0): stop when the monitored value
@@ -181,15 +207,53 @@ def _labels(y, device) -> torch.Tensor:
     return t.to(device=device, dtype=torch.float32).reshape(t.shape[0], -1)
 
 
+def _weights(w, device) -> Optional[torch.Tensor]:
+    if w is None:
+        return None
+    t = w if isinstance(w, torch.Tensor) else torch.as_tensor(np.asarray(w, dtype=np.float32))
+    return t.to(device=device, dtype=torch.float32).reshape(-1)
+
+
+def _whole_array_batch(x, y, sample_weight, batch_size):
+    """Whole-array input is one full batch (GCN is full-batch): there is nothing to shuffle, and a smaller batch is
+    not served."""
+    rows = y.shape[0] if hasattr(y, "shape") else len(y)
+    if batch_size is not None and batch_size < rows:
+        raise NotImplementedError(f"batch_size={batch_size} < {rows} rows: whole-array input runs as one full batch")
+    return (x, y, sample_weight)
+
+
+def _unpack(batch):
+    """(features, labels) or (features, labels, sample_weight)."""
+    return (batch[0], batch[1], batch[2] if len(batch) > 2 else None)
+
+
 class TrainingLoopMixin:
     """compile / fit / evaluate for `Model` (keras/layers/base.py)."""
 
-    def compile(self, loss="binary_crossentropy", optimizer="adam", metrics: Optional[List] = None, **kwargs):
+    def compile(self, loss="binary_crossentropy", optimizer="adam", metrics: Optional[List] = None,
+                weighted_metrics: Optional[List] = None, **kwargs):
+        """weighted_metrics: "acc" / "accuracy" (categorical accuracy under categorical cross-entropy, else binary),
+        weighted by the sample weight given to fit / evaluate."""
         self._loss_fn: Callable = _LOSSES[loss] if isinstance(loss, str) else loss
         self._optimizer_spec = _OPTIMIZERS[optimizer]() if isinstance(optimizer, str) else optimizer
         self._optimizer = None
         self._metrics = list(metrics or [])
+        self._weighted_metrics = []
+        for m in weighted_metrics or []:
+            if m not in ("acc", "accuracy"):
+                raise ValueError(f"unsupported weighted metric {m!r}; supported: 'acc', 'accuracy'")
+            self._weighted_metrics.append(WeightedAccuracy(m, categorical=loss == "categorical_crossentropy"))
         return self
+
+    def _all_metrics(self) -> list:
+        return self._metrics + getattr(self, "_weighted_metrics", [])
+
+    def _update_metrics(self, yt, pred, w):
+        for m in self._metrics:
+            m.update_state(yt, pred)
+        for m in getattr(self, "_weighted_metrics", []):
+            m.update_state(yt, pred, w)
 
     @property
     def optimizer(self) -> _OptimizerHandle:
@@ -197,44 +261,65 @@ class TrainingLoopMixin:
             raise RuntimeError("call compile() before reading the optimizer")
         return _OptimizerHandle(self)
 
-    def _step_loss(self, x, y):
+    def _step_loss(self, x, y, sample_weight=None):
+        """Keras's SUM_OVER_BATCH_SIZE: mean over the rows of w * loss (w = 1 without a sample weight)."""
         pred = self(x)
         yt = _labels(y, pred.device)
-        loss = self._loss_fn(yt, pred).mean()
+        w = _weights(sample_weight, pred.device)
+        per_row = self._loss_fn(yt, pred)
+        loss = per_row.mean() if w is None else (per_row.reshape(-1) * w).sum() / per_row.numel()
         reg = [l for l in getattr(self, "losses", [])] if hasattr(self, "losses") else []
         for r in reg:
             loss = loss + r
-        return pred, yt, loss
+        return pred, yt, w, loss
 
-    def evaluate(self, data, steps: Optional[int] = None) -> dict:
+    def evaluate(self, x, y=None, steps: Optional[int] = None, sample_weight=None, batch_size: Optional[int] = None,
+                 verbose: int = 0) -> dict:
+        """`x`: an iterable (or a callable returning one) of (features, labels[, sample_weight]) batches, of which
+        `steps` are read; or, with labels `y`, whole arrays evaluated as one batch with an optional `sample_weight`.
+        An int second argument is `steps` (the batch form `evaluate(data, steps)`).  Returns a dict of logs."""
         if not hasattr(self, "_loss_fn"):
             raise RuntimeError("call compile() before evaluate()")
-        for m in self._metrics:
+        if isinstance(y, int) and not isinstance(y, bool) and steps is None:
+            y, steps = None, y
+        data = [_whole_array_batch(x, y, sample_weight, batch_size)] if y is not None else _batches(x)
+        metrics = self._all_metrics()
+        for m in metrics:
             m.reset_state()
         tot, n = None, 0
         was = self.training
         self.eval()
         with torch.no_grad():
-            for x, y in itertools.islice(_batches(data), steps):
-                pred, yt, loss = self._step_loss(x, y)
+            for batch in itertools.islice(data, steps):
+                pred, yt, w, loss = self._step_loss(*_unpack(batch))
                 tot = loss.detach().double() if tot is None else tot + loss.detach().double()
                 n += 1
-                for m in self._metrics:
-                    m.update_state(yt, pred)
+                self._update_metrics(yt, pred, w)
         self.train(was)
         logs = {"loss": float(tot / max(n, 1)) if tot is not None else float("nan")}
-        logs.update({m.name: m.result() for m in self._metrics})
+        logs.update({m.name: m.result() for m in metrics})
         return logs
 
     def fit(self, x, y=None, epochs: int = 1, steps_per_epoch: Optional[int] = None, validation_data=None,
-            validation_steps: Optional[int] = None, callbacks: Optional[List] = None, verbose: int = 0):
+            validation_steps: Optional[int] = None, callbacks: Optional[List] = None, verbose: int = 0,
+            sample_weight=None, batch_size: Optional[int] = None, shuffle: bool = True):
         """`x`: iterable (or callable returning one) of (features, labels) batches that is consumed ACROSS epochs, as
-        the reference's repeated tf.data pipeline is; `steps_per_epoch` batches make one epoch.  Returns a dict of
-        per-epoch logs (`history`)."""
+        the reference's repeated tf.data pipeline is; `steps_per_epoch` batches make one epoch.  With labels `y`, `x`
+        and `y` are whole arrays trained as one full batch per step, weighted by `sample_weight` when it is given;
+        `batch_size` below the number of rows raises NotImplementedError, and `shuffle` has no effect on a single
+        full batch.  With `batch_size` given (Keras's whole-array form) and no `steps_per_epoch`, an epoch is one pass
+        over the arrays: one step.  `validation_data` is then `(x, y)` or `(x, y, sample_weight)`; without `y` it is a batch iterable
+        (or callable) read for `validation_steps` batches.  Returns a dict of per-epoch logs (`history`)."""
         if not hasattr(self, "_loss_fn"):
             raise RuntimeError("call compile() before fit()")
         if y is not None:
-            x = [(x, y)] * (steps_per_epoch or 1) * epochs
+            if batch_size is not None and steps_per_epoch is None:
+                steps_per_epoch = 1
+            x = [_whole_array_batch(x, y, sample_weight, batch_size)] * (steps_per_epoch or 1) * epochs
+            if validation_data is not None:
+                vx, vy, vw = _unpack(validation_data)
+                validation_data = [_whole_array_batch(vx, vy, vw, None)]
+                validation_steps = 1
         stream = iter(_batches(x))
         history: dict = {}
         callbacks = list(callbacks or [])
@@ -245,11 +330,11 @@ class TrainingLoopMixin:
             if _hook(cb, "on_train_begin"):
                 cb.on_train_begin({})
         for epoch in range(epochs):
-            for m in self._metrics:
+            for m in self._all_metrics():
                 m.reset_state()
             tot, n = None, 0
-            for xb, yb in itertools.islice(stream, steps_per_epoch):
-                pred, yt, loss = self._step_loss(xb, yb)
+            for batch in itertools.islice(stream, steps_per_epoch):
+                pred, yt, w, loss = self._step_loss(*_unpack(batch))
                 if self._optimizer is None:        # parameters of lazily built layers exist after the first forward
                     self._optimizer = self._optimizer_spec.build([p for p in self.parameters() if p.requires_grad])
                 self._optimizer.zero_grad(set_to_none=True)
@@ -260,14 +345,13 @@ class TrainingLoopMixin:
                     if _hook(cb, "on_batch_end"):
                         cb.on_batch_end(n, {})
                 n += 1
-                for m in self._metrics:
-                    m.update_state(yt, pred.detach())
+                self._update_metrics(yt, pred.detach(), w)
             if n == 0:
                 break                                # input exhausted
             logs = {"loss": float(tot / n)}
-            logs.update({m.name: m.result() for m in self._metrics})
+            logs.update({m.name: m.result() for m in self._all_metrics()})
             if validation_data is not None:
-                logs.update({"val_" + k: v for k, v in self.evaluate(validation_data, validation_steps).items()})
+                logs.update({"val_" + k: v for k, v in self.evaluate(validation_data, steps=validation_steps).items()})
             for k, v in logs.items():
                 history.setdefault(k, []).append(v)
             if verbose:

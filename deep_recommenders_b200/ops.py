@@ -312,6 +312,144 @@ class MoEMixFn(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------
+# GCN: CSR sparse x dense product (dr_spmm_csr_fwd)
+# ------------------------------------------------------------------------------------------
+ACT_SOFTMAX = 4          # DR_ACT_SOFTMAX: served by the SpMM epilogue only
+SPMM_SOFTMAX_MAX_F = 1024
+
+
+class CSRAdjacency:
+    """A constant sparse matrix A [n_rows, n_cols] prepared once on the device: the int32 CSR of A and of A^T.
+
+    Build it from a scipy sparse matrix (anything with ``tocsr()``), a torch sparse COO or CSR tensor, or CSR arrays.
+    The arrays are validated once on the host (``ValueError`` for a malformed ``indptr``, an index out of range or
+    non-float values).  Entries keep their stored order: duplicates are summed where they stand, and a COO tensor is
+    grouped by row without coalescing.  A^T is a stable sort of the entries by column, so each transposed row lists
+    its entries in ascending original row, and the backward sums in a fixed order.  The values are an input, not a
+    parameter: no gradient reaches them (TensorFlow would give a SparseTensor's values one)."""
+
+    def __init__(self, indptr, indices, values, shape, device=None):
+        import numpy as np
+        indptr = np.asarray(indptr)
+        indices = np.asarray(indices)
+        values = np.asarray(values)
+        n_rows, n_cols = int(shape[0]), int(shape[1])
+        if n_rows < 0 or n_cols < 0 or indptr.ndim != 1 or indptr.shape[0] != n_rows + 1:
+            raise ValueError(f"CSR: indptr must have n_rows + 1 = {n_rows + 1} entries, got shape {indptr.shape}")
+        if indices.ndim != 1 or values.shape != indices.shape:
+            raise ValueError(f"CSR: indices {indices.shape} and values {values.shape} must be 1-D of one length")
+        if not (np.issubdtype(indptr.dtype, np.integer) and np.issubdtype(indices.dtype, np.integer)):
+            raise ValueError("CSR: indptr and indices must be integers")
+        if not np.issubdtype(values.dtype, np.floating):
+            raise ValueError(f"CSR: values must be floating point, got {values.dtype}")
+        nnz = indices.shape[0]
+        if max(n_rows, n_cols, nnz) >= 2 ** 31:
+            raise ValueError(f"CSR: n_rows, n_cols and nnz must stay below 2^31, got {n_rows}, {n_cols}, {nnz}")
+        if indptr[0] != 0 or indptr[-1] != nnz or (n_rows and np.any(np.diff(indptr) < 0)):
+            raise ValueError(f"CSR: indptr must start at 0, never decrease and end at nnz = {nnz}")
+        if nnz and (indices.min() < 0 or indices.max() >= n_cols):
+            raise ValueError(f"CSR: column index out of range [0, {n_cols})")
+        dev = torch.device(device if device is not None else "cuda")
+        self.shape = (n_rows, n_cols)
+        self.nnz = nnz
+        self.indptr = torch.from_numpy(indptr.astype(np.int32)).to(dev)
+        self.indices = torch.from_numpy(indices.astype(np.int32)).to(dev)
+        self.values = torch.from_numpy(values.astype(np.float32)).to(dev)
+        rows = torch.repeat_interleave(torch.arange(n_rows, device=dev, dtype=torch.int32),
+                                       (self.indptr[1:] - self.indptr[:-1]).long())
+        order = torch.sort(self.indices, stable=True).indices
+        counts = torch.bincount(self.indices.long(), minlength=n_cols)
+        self.t_indptr = torch.zeros(n_cols + 1, dtype=torch.int32, device=dev)
+        self.t_indptr[1:] = torch.cumsum(counts, 0).to(torch.int32)
+        self.t_indices = rows[order].contiguous()
+        self.t_values = self.values[order].contiguous()
+
+    @classmethod
+    def from_any(cls, adj, device=None) -> "CSRAdjacency":
+        """A prepared adjacency from a scipy sparse matrix (duck-typed through ``tocsr()``) or a torch sparse tensor."""
+        if isinstance(adj, CSRAdjacency):
+            return adj
+        if isinstance(adj, torch.Tensor):
+            if adj.layout == torch.sparse_csr:
+                return cls(adj.crow_indices().cpu().numpy(), adj.col_indices().cpu().numpy(),
+                           adj.values().detach().cpu().numpy(), adj.shape, device or adj.device)
+            if adj.layout == torch.sparse_coo:
+                idx = adj._indices().cpu()
+                vals = adj._values().detach().cpu()
+                order = torch.sort(idx[0], stable=True).indices
+                counts = torch.bincount(idx[0], minlength=adj.shape[0])
+                indptr = torch.cat([torch.zeros(1, dtype=torch.int64), torch.cumsum(counts, 0)])
+                return cls(indptr.numpy(), idx[1][order].numpy(), vals[order].numpy(), adj.shape,
+                           device or (adj.device if adj.is_cuda else None))
+            raise ValueError(f"CSRAdjacency: a torch tensor must be sparse COO or CSR, got layout {adj.layout}")
+        if hasattr(adj, "tocsr"):
+            csr = adj.tocsr()
+            return cls(csr.indptr, csr.indices, csr.data, csr.shape, device)
+        raise TypeError(f"CSRAdjacency: expected a scipy sparse matrix or a torch sparse tensor, got {type(adj).__name__}")
+
+    def spmm(self, x, bias=None, residual=None, act: int = 0, transpose: bool = False):
+        """act(A @ x + bias) (+ residual), or A^T @ x with transpose=True, as raw tensors (no autograd)."""
+        lib = _lib.load()
+        n_rows, n_cols = self.shape[::-1] if transpose else self.shape
+        indptr, indices, values = ((self.t_indptr, self.t_indices, self.t_values) if transpose
+                                   else (self.indptr, self.indices, self.values))
+        if x.dim() != 2 or x.shape[0] != n_cols or x.shape[1] < 1:
+            raise ValueError(f"SpMM: x must be [{n_cols}, F], got {tuple(x.shape)}")
+        F = x.shape[1]
+        if bias is not None and tuple(bias.shape) != (F,):
+            raise ValueError(f"SpMM: bias must be [{F}], got {tuple(bias.shape)}")
+        if residual is not None and tuple(residual.shape) != (n_rows, F):
+            raise ValueError(f"SpMM: residual must be [{n_rows}, {F}], got {tuple(residual.shape)}")
+        y = torch.empty((n_rows, F), device=x.device, dtype=torch.float32)
+        out = torch.empty_like(y) if residual is not None else None
+        check(lib.dr_spmm_csr_fwd(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), n_rows, n_cols,
+                                  self.nnz, x.data_ptr(), F, _ptr(bias), _ptr(residual), act, y.data_ptr(),
+                                  _ptr(out), _stream()), "dr_spmm_csr_fwd")
+        return y, out
+
+
+class SpMMFn(torch.autograd.Function):
+    """SpMMFn(x [n_cols, F], bias [F] or None, residual [n_rows, F] or None, adj: CSRAdjacency, act) =
+    act(A @ x + bias) (+ residual): the plain product with bias None, residual None and act 0, else the fused epilogue
+    (dr_spmm_csr_fwd).  act is a DR_ACT_* code or ACT_SOFTMAX.  Backward: the activation gradient from the saved
+    output (dr_act_bwd_colsum, after dr_softmax_rows_bwd for the softmax), then gx = A^T @ gz on the transposed CSR."""
+
+    @staticmethod
+    def forward(ctx, x, bias, residual, adj, act: int):
+        x = _f32(x, "x")
+        bias = None if bias is None else _f32(bias, "bias")
+        residual = None if residual is None else _f32(residual, "residual")
+        y, out = adj.spmm(x, bias, residual, act)
+        ctx.adj, ctx.act = adj, act
+        ctx.has_bias, ctx.has_res = bias is not None, residual is not None
+        ctx.save_for_backward(y)
+        return out if residual is not None else y
+
+    @staticmethod
+    def backward(ctx, g):
+        lib = _lib.load()
+        (y,) = ctx.saved_tensors
+        g = _f32(g, "g")
+        M, F = y.shape
+        act = ctx.act
+        gb = torch.empty((F,), device=g.device, dtype=torch.float32) if ctx.has_bias else None
+        gz = g
+        if act == ACT_SOFTMAX:
+            gz = torch.empty_like(y)
+            check(lib.dr_softmax_rows_bwd(y.data_ptr(), g.data_ptr(), M, F, gz.data_ptr(), _stream()),
+                  "dr_softmax_rows_bwd")
+            act = 0
+        elif act != 0:
+            gz = torch.empty_like(y)
+        if act != 0 or gb is not None:
+            check(lib.dr_act_bwd_colsum(_ptr(y) if act else None, gz.data_ptr() if act == 0 else g.data_ptr(), M, F,
+                                        act, gz.data_ptr() if act else None, _ptr(gb), _stream()),
+                  "dr_act_bwd_colsum")
+        gx = ctx.adj.spmm(gz, transpose=True)[0] if ctx.needs_input_grad[0] else None
+        return gx, gb, (g if ctx.has_res else None), None, None
+
+
+# ------------------------------------------------------------------------------------------
 # Row X: Cross
 # ------------------------------------------------------------------------------------------
 class CrossFn(torch.autograd.Function):

@@ -52,6 +52,7 @@ extern "C" {
 #define DR_ACT_RELU 1
 #define DR_ACT_SIGMOID 2
 #define DR_ACT_TANH 3
+#define DR_ACT_SOFTMAX 4   /* dr_spmm_csr_fwd only: softmax over the output row */
 
 /* ABI version (major*10000 + minor*100 + patch) and last error string. */
 int dr_version(void);
@@ -338,6 +339,32 @@ int dr_add_layernorm_bwd(const float* x, const float* residual, const float* gam
 int dr_softmax_rows_fwd(const float* x, int64_t N, int V, float* y, void* stream);
 int dr_softmax_rows_bwd(const float* y, const float* gy, int64_t N, int V, float* gx,
                         void* stream);
+
+/* GCN aggregation: CSR sparse (adjacency) times dense (features) with a fused epilogue.
+ *   replaces: keras/models/retrieval/gcn.py:45-55 (tf.sparse.sparse_dense_matmul(adj, features), the Dense's bias
+ *   and activation when the layer multiplies by the kernel first, and `outputs += features`).
+ *   A [n_rows, n_cols] in CSR: indptr int32 [n_rows + 1], indices int32 [nnz], values fp32 [nnz]; x [n_cols, F].
+ *   y[r, f] = act(sum_{p = indptr[r]}^{indptr[r+1]-1} values[p] * x[indices[p], f] + bias[f])
+ *     the sum is fp32 fmaf in ascending p, from +0.0; duplicate column indices are summed, unsorted rows are summed in
+ *     their stored order; an empty row gives act(bias); an index outside [0, n_cols) contributes nothing and is never
+ *     dereferenced.  act: DR_ACT_NONE/RELU/SIGMOID/TANH, or DR_ACT_SOFTMAX (max subtracted, expf, divided by the sum
+ *     over the row's F values; served for F <= 1024, DR_ENOTSUP above).
+ *   out = y + residual (residual [n_rows, F]): written only when residual != NULL, and y is still written (the
+ *     backward needs act' of y).  bias [F] and residual are nullable; out must be given with a residual.
+ *   One owner (a group of 1..32 lanes) per output row, no atomics: reruns are bit-identical.
+ *   Served: n_rows, n_cols, nnz < 2^31 (DR_ENOTSUP outside), any F >= 1.  n_rows = 0 is a no-op.
+ *   The backward is this entry on the transposed CSR (entries of each transposed row in ascending original row) with
+ *   act = DR_ACT_NONE and no bias; the CSR arrays are inputs only, so the values get no gradient.               */
+int dr_spmm_csr_fwd(const int* indptr, const int* indices, const float* values, int64_t n_rows, int64_t n_cols,
+                    int64_t nnz, const float* x, int F, const float* bias, const float* residual, int act, float* y,
+                    float* out, void* stream);
+/* Activation gradient and bias gradient of a fused epilogue such as the one above:
+ *   gz = gy * act'(y) (act'(y) from the saved output y; gz may alias gy), gb[n] = sum_m gz[m, n] (OVERWRITTEN).
+ *   act: DR_ACT_NONE/RELU/SIGMOID/TANH; with DR_ACT_NONE gz is gy and is not written (y and gz may be NULL).
+ *   gb is nullable; it is summed with floating-point atomics, so its last bits can differ from run to run, as the
+ *   gb of dr_dense_bwd can.  The same pass dr_dense_bwd runs before its GEMMs, without them.                     */
+int dr_act_bwd_colsum(const float* y, const float* gy, int64_t M, int N, int act, float* gz, float* gb,
+                      void* stream);
 
 /* Multi-gate mixture of experts: every task's gate softmax and expert mixture in one pass.
  *   replaces: estimator/models/multi_task_learning/mixture_of_experts.py:46-53 (gating softmax), :69 (tf.stack of the
