@@ -100,6 +100,11 @@ _SIGS = {
     "dr_hash_bucket_bytes_host": [_p, _p, _i64, _i64, _p],
     "dr_fingerprint64_host": [_p, _i64],
     "dr_vocab_lookup_i64": [_p, _i64, _p, _p, _i64, _i64, _p, _p],
+    "dr_cross_hash": [_i, _p, _p, _p, _i64, C.c_uint64, _i64, _p, _p, _p],
+    "dr_cross_hash_host": [_i, _p, _p, _p, _i64, C.c_uint64, _i64, _p, _p],
+    "dr_wide_fwd": [_p, _i64, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _p, _p],
+    "dr_wide_bwd": [_p, _i64, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _p, _p],
+    "dr_wide_ftrl": [_p, _i64, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _f, _f, _f, _p],
     "dr_embed_bag_fwd": [_p, _i64, _i64, _p, _i, _p, _i64, _i, _i, _p, _i64, _p],
     "dr_embed_bag_bwd": [_p, _i, _p, _i64, _i, _i, _p, _i64, _i64, _i64, _p, _f, _p],
     "dr_crc32c_host": [_p, _i64],

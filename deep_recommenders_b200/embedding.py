@@ -125,13 +125,16 @@ class EmbeddingCollection(nn.Module):
         second_order=False: logit = bias + linear only (xDeepFM's linear unit), from the same fused kernel.
 
         bags: {slot: (flat_ids [nnz], row_splits [B+1])} for multi-valued slots (mean-combined embedding,
-        summed first-order weights); the matching columns of `ids` are ignored.
+        summed first-order weights); the matching columns of `ids` are ignored.  A collection without first-order
+        weights serves bags with want_logit=False.
         """
         if ids.dim() != 2 or ids.shape[1] != self.num_slots:
             raise ValueError(f"ids must be [B, {self.num_slots}], got {tuple(ids.shape)}")
         if bags:
             if not second_order:
                 raise ValueError("second_order=False is not served with multi-valued slots (bags)")
+            if want_logit and not self.with_linear:
+                raise ValueError("EmbedFMMixed needs a collection with the first-order term (with_linear=True)")
             bad = [s for s in bags if not (0 <= s < self.num_slots)]
             if bad:
                 raise ValueError(f"bags: slot indices {bad} outside [0, {self.num_slots})")
@@ -141,3 +144,59 @@ class EmbeddingCollection(nn.Module):
         stack, logit = ops.EmbedFM.apply(ids, self.weight, self.linear if want else None,
                                          self.bias if want else None, self, want, bool(second_order))
         return stack, (logit if want else None)
+
+
+class LinearTable(nn.Module):
+    """The variables of tf.feature_column.linear_model over S indicator / crossed columns (estimator
+    wide_and_deep.py:31-33): one scalar weight per row of each column and one bias, with the two slots
+    tf.train.FtrlOptimizer keeps for them.
+
+    state [total_rows + 1, 4] fp32: row r = {w, z, n, g} -- weight, FTRL linear slot, FTRL accumulator and the
+    gradient of the current batch -- in ONE 16-byte record, so a lookup, its gradient atomic and the update of a row
+    touch one 32-B sector (csrc/wide.cu).  Record total_rows is the bias.  Column s owns rows [off_s, off_s + rows_s).
+    w, z and g start at zero, as linear_model's zeros initializer and FTRL's linear slot do; n starts at
+    initial_accumulator_value, the FTRL optimizer's setting, which ops.FtrlOptimizer checks it matches.  The slots
+    live in the table, so they are saved with it and a new optimizer continues from them.
+    """
+
+    def __init__(self, rows: Sequence[int], device=None, initial_accumulator_value: float = 0.1):
+        super().__init__()
+        self.rows_list = [int(r) for r in rows]
+        if not self.rows_list or any(r < 1 for r in self.rows_list):
+            raise ValueError(f"LinearTable needs at least one column and rows >= 1 per column, got {self.rows_list}")
+        self.num_slots = len(self.rows_list)
+        dev = torch.device(device if device is not None else ("cuda" if torch.cuda.is_available() else "cpu"))
+        offs = [0]
+        for r in self.rows_list:
+            offs.append(offs[-1] + r)
+        self.total_rows = offs[-1]
+        # a Parameter so that autograd runs the backward that accumulates g in place; its .grad stays None
+        if not initial_accumulator_value >= 0.0:
+            raise ValueError(f"initial_accumulator_value {initial_accumulator_value} needs to be positive or zero")
+        self.initial_accumulator_value = float(initial_accumulator_value)
+        state = torch.zeros((self.total_rows + 1, 4), dtype=torch.float32, device=dev)
+        state[:, 2] = self.initial_accumulator_value
+        self.state = nn.Parameter(state)
+        self.register_buffer("_offsets", torch.tensor(offs[:-1], dtype=torch.int64, device=dev), persistent=False)
+        self.register_buffer("_rows", torch.tensor(self.rows_list, dtype=torch.int64, device=dev), persistent=False)
+        self.lookups = None        # (ids, bags) of the last forward: the rows the optimizer updates
+
+    @property
+    def weights(self) -> torch.Tensor:
+        """[total_rows] view of the weights (column s at [off_s, off_s + rows_s))."""
+        return self.state.detach()[:self.total_rows, 0]
+
+    @property
+    def bias(self) -> torch.Tensor:
+        return self.state.detach()[self.total_rows:, 0]
+
+    def weights_of(self, s: int) -> torch.Tensor:
+        o = int(self._offsets[s])
+        return self.weights[o:o + self.rows_list[s]]
+
+    def forward(self, ids: torch.Tensor, bags: Optional[dict] = None) -> torch.Tensor:
+        """ids [B, S] int64 (columns of multi-valued slots ignored), bags {slot: (flat ids, row_splits)} -> logit [B]."""
+        if ids.dim() != 2 or ids.shape[1] != self.num_slots:
+            raise ValueError(f"ids must be [B, {self.num_slots}], got {tuple(ids.shape)}")
+        self.lookups = (ids, bags)
+        return ops.WideLinearFn.apply(self.state, self, ids, bags)

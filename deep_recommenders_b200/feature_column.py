@@ -174,3 +174,59 @@ def embedding_column(categorical_column: CategoricalColumn, dimension: int, comb
     if combiner not in ("mean", "sqrtn", "sum"):
         raise ValueError(f"Invalid combiner {combiner}.")
     return EmbeddingColumn(categorical_column, int(dimension), combiner, initializer_stddev)
+
+
+DEFAULT_CROSS_HASH_KEY = 0xDECAFCAFFE    # TensorFlow's sparse_cross_hashed default hash_key
+
+
+@dataclass(frozen=True)
+class CrossedColumn:
+    """tf.feature_column.crossed_column over raw features: id = FingerprintCat64 chain over the keys' values, mod
+    hash_bucket_size (csrc/cross.cuh).  Strings enter through Fingerprint64 of their bytes, int64 values raw; a
+    single-valued key drops empty strings and -1 (a RaggedFeature keeps every value, as TensorFlow keeps a
+    SparseTensor's); multi-valued keys cross every combination."""
+    keys: Tuple[str, ...]
+    hash_bucket_size: int
+    hash_key: int = DEFAULT_CROSS_HASH_KEY
+
+    @property
+    def key(self) -> str:
+        return self.name
+
+    @property
+    def name(self) -> str:
+        return "_X_".join(sorted(self.keys))
+
+    @property
+    def num_buckets(self) -> int:
+        return self.hash_bucket_size
+
+
+def crossed_column(keys, hash_bucket_size: int, hash_key: Optional[int] = None) -> CrossedColumn:
+    if len(keys) < 2:
+        raise ValueError(f"keys must be a list with length > 1. Given: {keys}")
+    if hash_bucket_size is None or hash_bucket_size < 1:
+        raise ValueError(f"hash_bucket_size must be > 1. hash_bucket_size: {hash_bucket_size}")
+    for k in keys:
+        if not isinstance(k, str):
+            raise NotImplementedError(f"crossed_column serves raw feature names as keys; got {type(k).__name__} "
+                                      f"{getattr(k, 'name', k)!r}")
+    return CrossedColumn(tuple(keys), int(hash_bucket_size),
+                         DEFAULT_CROSS_HASH_KEY if hash_key is None else int(hash_key))
+
+
+def linear_model(features, feature_columns, table):
+    """tf.feature_column.linear_model over indicator columns of categorical or crossed columns: [B, 1] =
+    bias + sum over the columns of the weights of the example's ids (multi-valued features count every value).
+    It owns nothing: `table` (embedding.LinearTable with one slot per column, in this order) holds the weights."""
+    from .hashing import wide_ids
+    cols = list(feature_columns) if isinstance(feature_columns, (list, tuple)) else [feature_columns]
+    for c in cols:
+        if not isinstance(c, IndicatorColumn):
+            raise NotImplementedError(f"linear_model serves indicator columns only; got {type(c).__name__} "
+                                      f"{getattr(c, 'name', c)!r}")
+    if len(cols) != table.num_slots or any(int(c.categorical_column.num_buckets) != r
+                                           for c, r in zip(cols, table.rows_list)):
+        raise ValueError("the table's columns do not match feature_columns")
+    ids, bags = wide_ids([c.categorical_column for c in cols], features, table.state.device)
+    return table(ids, bags).unsqueeze(1)

@@ -176,3 +176,120 @@ def ids_and_bags(keys: Sequence[str], cats: dict, inputs, device):
             B = cols[-1].shape[0]
     cols = [c if c is not None else torch.zeros((B,), dtype=torch.int64, device=device) for c in cols]
     return torch.stack(cols, dim=1), (bags or None)
+
+
+def _cross_key_host(v):
+    """One key's raw feature -> (values, byte offsets or None, row_splits or None) as numpy arrays."""
+    splits = None
+    if isinstance(v, RaggedFeature):
+        rs = v.row_splits
+        splits = np.ascontiguousarray(rs.detach().cpu().numpy() if isinstance(rs, torch.Tensor) else rs,
+                                      dtype=np.int64)
+        v = v.values
+    if isinstance(v, PackedStrings):
+        data, offsets = pack_strings(v)
+        return data, offsets, splits
+    arr = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+    if splits is None:
+        if arr.ndim == 2 and arr.shape[1] == 1:
+            arr = arr[:, 0]
+        if arr.ndim != 1:
+            raise ValueError(f"crossed_column: expected one value per example ([B] or [B, 1]), got shape {arr.shape}; "
+                             "pass multi-valued features as a RaggedFeature")
+    arr = arr.reshape(-1)
+    if arr.dtype.kind in "iu":
+        return np.ascontiguousarray(arr, dtype=np.int64), None, splits
+    data, offsets = pack_strings(arr.tolist())
+    return data, offsets, splits
+
+
+def cross_ids(col, features, device):
+    """crossed_column ids of a batch: [B] int64 (-1 = no cross) when every key is single-valued, else
+    (flat ids, row_splits [B+1]), on `device`.  When some key is a CUDA tensor the crossing runs on the device
+    (host strings are copied there as bytes + offsets); otherwise it runs in the host twin and the ids are copied."""
+    from . import ops
+    for k in col.keys:
+        if k not in features:
+            raise KeyError(f"feature {k!r} of crossed_column {col.name!r} is missing from the features")
+    raw = [features[k] for k in col.keys]
+    on_device = any(isinstance(v.values if isinstance(v, RaggedFeature) else v, torch.Tensor)
+                    and (v.values if isinstance(v, RaggedFeature) else v).is_cuda for v in raw)
+    if on_device:
+        vals, offs, spl = [], [], []
+        for v in raw:
+            rs = v.row_splits if isinstance(v, RaggedFeature) else None
+            x = v.values if isinstance(v, RaggedFeature) else v
+            if isinstance(x, torch.Tensor) and x.is_cuda and x.dtype in (torch.int64, torch.int32):
+                vals.append(x.reshape(-1).to(torch.int64).contiguous())
+                offs.append(None)
+            else:
+                data, o, _ = _cross_key_host(x if rs is None else RaggedFeature(x, rs))
+                vals.append(torch.from_numpy(data.copy()).to(device))
+                offs.append(None if o is None else torch.from_numpy(o).to(device))
+            if rs is not None:
+                rs = rs if isinstance(rs, torch.Tensor) else torch.from_numpy(np.asarray(rs, dtype=np.int64))
+                rs = rs.to(device=device, dtype=torch.int64).contiguous()
+            spl.append(rs)
+        B = next((s.numel() - 1 for s in spl if s is not None), None)
+        B = (vals[0].numel() if offs[0] is None else offs[0].numel() - 1) if B is None else B
+        return ops.cross_hash(vals, offs, spl, B, col.hash_bucket_size, col.hash_key)
+    keys = [_cross_key_host(v) for v in raw]
+    B = next((len(s) - 1 for _, _, s in keys if s is not None), None)
+    B = (keys[0][1].size - 1 if keys[0][1] is not None else keys[0][0].size) if B is None else B
+    ids, splits = cross_hash_host(keys, B, col.hash_bucket_size, col.hash_key)
+    if splits is None:
+        return torch.from_numpy(ids).to(device)
+    return torch.from_numpy(ids).to(device), torch.from_numpy(splits).to(device)
+
+
+def cross_hash_host(keys, B: int, num_buckets: int, hash_key: int):
+    """dr_cross_hash_host on numpy keys [(values, byte offsets or None, row_splits or None)] -> (ids, None) when
+    every key is single-valued (ids [B], -1 = no cross), else (flat ids, row_splits [B+1])."""
+    lib = _lib.load()
+    K = len(keys)
+    for vals, offs, spl in keys:
+        n = (offs.size - 1) if offs is not None else vals.size
+        if (spl is None and n != B) or (spl is not None and (spl.size != B + 1 or spl[-1] > n)):
+            raise ValueError(f"crossed_column: a key has {n} values, which does not fit a batch of {B}")
+    vp = (C.c_void_p * K)(*[k[0].ctypes.data for k in keys])
+    op = (C.c_void_p * K)(*[None if k[1] is None else k[1].ctypes.data for k in keys])
+    sp = (C.c_void_p * K)(*[None if k[2] is None else k[2].ctypes.data for k in keys])
+    hk = int(hash_key) & 0xFFFFFFFFFFFFFFFF
+    if all(k[2] is None for k in keys):
+        out = np.empty(B, dtype=np.int64)
+        _lib.check(lib.dr_cross_hash_host(K, vp, op, sp, B, hk, int(num_buckets), None, out.ctypes.data),
+                   "dr_cross_hash_host")
+        return out, None
+    splits = np.empty(B + 1, dtype=np.int64)
+    _lib.check(lib.dr_cross_hash_host(K, vp, op, sp, B, hk, int(num_buckets), splits.ctypes.data, None),
+               "dr_cross_hash_host")
+    np.cumsum(splits, out=splits)
+    out = np.empty(max(int(splits[-1]), 1), dtype=np.int64)
+    _lib.check(lib.dr_cross_hash_host(K, vp, op, sp, B, hk, int(num_buckets), splits.ctypes.data, out.ctypes.data),
+               "dr_cross_hash_host")
+    return out[:int(splits[-1])], splits
+
+
+def wide_ids(columns, inputs, device):
+    """Categorical / crossed columns -> (ids [B, S] int64 on `device`, {slot: (flat ids, row_splits)} or None), the
+    layout LinearTable takes: single-valued columns fill their column of ids, multi-valued ones go to the bags."""
+    from .feature_column import CrossedColumn
+    cols, bags, B = [], {}, None
+    for s, c in enumerate(columns):
+        if isinstance(c, CrossedColumn):
+            r = cross_ids(c, inputs, device)
+        elif isinstance(c, CategoricalColumn):
+            ids, b = ids_and_bags([c.key], {c.key: c}, inputs, device)
+            r = ids[:, 0] if b is None else b[0]
+        else:
+            raise NotImplementedError(f"column {getattr(c, 'name', c)!r}: linear_model serves categorical and "
+                                      "crossed columns")
+        if isinstance(r, tuple):
+            bags[s] = r
+            cols.append(None)
+            B = r[1].numel() - 1
+        else:
+            cols.append(r)
+            B = r.shape[0]
+    cols = [c if c is not None else torch.full((B,), -1, dtype=torch.int64, device=device) for c in cols]
+    return torch.stack(cols, dim=1), (bags or None)

@@ -984,6 +984,145 @@ def lazy_adam_rows_(ids: torch.Tensor, rows: torch.Tensor, slot_offsets: torch.T
                                 _stream()), "dr_lazy_adam_rows")
 
 
+def _wide_bags(bags, B: int):
+    """{slot: (flat ids, row_splits)} -> (n, host arrays of slots / id pointers / split pointers, kept tensors)."""
+    import ctypes as C
+    slots = sorted(bags) if bags else []
+    keep = []
+    for s in slots:
+        bid, bsp = _ids(bags[s][0], "bag ids").to(torch.int64), _splits(bags[s][1])
+        if bsp.numel() != B + 1:
+            raise ValueError(f"slot {s}: row_splits has {bsp.numel()} entries, expected B+1 = {B + 1}")
+        keep.append((bid, bsp))
+    n = len(slots)
+    return (n, (C.c_int * max(n, 1))(*slots), (C.c_void_p * max(n, 1))(*[k[0].data_ptr() for k in keep]),
+            (C.c_void_p * max(n, 1))(*[k[1].data_ptr() for k in keep]), keep)
+
+
+def _wide_args(table, ids, bags):
+    ids = _ids(ids).to(torch.int64).contiguous()
+    B, S = ids.shape
+    n, bs, bi, bp, keep = _wide_bags(bags, B)
+    return (table.state.data_ptr(), table.total_rows, table._rows.data_ptr(), table._offsets.data_ptr(), ids.data_ptr(),
+            B, S, n, bs, bi, bp), (ids, keep)
+
+
+class WideLinearFn(torch.autograd.Function):
+    """logit [B] = tf.feature_column.linear_model over the LinearTable's columns (dr_wide_fwd).  Backward accumulates
+    the row gradients into the table's records (dr_wide_bwd) for FtrlOptimizer.apply and returns no tensor gradient."""
+
+    @staticmethod
+    def forward(ctx, state, table, ids, bags):
+        lib = _lib.load()
+        _f32(state, "state")
+        args, keep = _wide_args(table, ids, bags)
+        logit = torch.empty((args[5],), device=state.device, dtype=torch.float32)
+        check(lib.dr_wide_fwd(*args, logit.data_ptr(), _stream()), "dr_wide_fwd")
+        ctx.table, ctx.args, ctx.keep = table, args, keep
+        return logit
+
+    @staticmethod
+    def backward(ctx, g_logit):
+        lib = _lib.load()
+        g_logit = _f32(g_logit, "g_logit")
+        with torch.no_grad():
+            check(lib.dr_wide_bwd(*ctx.args, g_logit.data_ptr(), _stream()), "dr_wide_bwd")
+        return None, None, None, None
+
+
+class FtrlOptimizer:
+    """tf.train.FtrlOptimizer(learning_rate, learning_rate_power=-0.5, initial_accumulator_value=0.1,
+    l1_regularization_strength=0.0, l2_regularization_strength=0.0) for the wide part of a model: `apply(table)`
+    updates the rows of a LinearTable the last forward touched, and its bias, with TensorFlow's ApplyFtrl arithmetic
+    (dr_wide_ftrl), after the backward has accumulated their gradients.  Rows the batch did not touch keep their
+    values, which is what TensorFlow's dense update leaves in them (see csrc/wide.cu).
+    Served: learning_rate_power = -0.5 and no l2 shrinkage."""
+
+    def __init__(self, learning_rate, learning_rate_power=-0.5, initial_accumulator_value=0.1,
+                 l1_regularization_strength=0.0, l2_regularization_strength=0.0,
+                 l2_shrinkage_regularization_strength=0.0):
+        if not learning_rate > 0:
+            raise ValueError(f"learning_rate {learning_rate} must be positive")
+        if initial_accumulator_value < 0.0:
+            raise ValueError(f"initial_accumulator_value {initial_accumulator_value} needs to be positive or zero")
+        if learning_rate_power > 0.0:
+            raise ValueError(f"learning_rate_power {learning_rate_power} needs to be negative or zero")
+        if l1_regularization_strength < 0.0:
+            raise ValueError(f"l1_regularization_strength {l1_regularization_strength} needs to be positive or zero")
+        if l2_regularization_strength < 0.0:
+            raise ValueError(f"l2_regularization_strength {l2_regularization_strength} needs to be positive or zero")
+        if l2_shrinkage_regularization_strength < 0.0:
+            raise ValueError("l2_shrinkage_regularization_strength needs to be positive or zero")
+        if learning_rate_power != -0.5:
+            raise NotImplementedError("FtrlOptimizer serves learning_rate_power = -0.5 only")
+        if l2_shrinkage_regularization_strength != 0.0:
+            raise NotImplementedError("FtrlOptimizer does not serve l2_shrinkage_regularization_strength")
+        self.learning_rate = float(learning_rate)
+        self.initial_accumulator_value = float(initial_accumulator_value)
+        self.l1 = float(l1_regularization_strength)
+        self.l2 = float(l2_regularization_strength)
+
+    def apply(self, table) -> None:
+        if table.lookups is None:
+            raise RuntimeError("FtrlOptimizer.apply: the table has not run a forward pass")
+        # the accumulator slot lives in the table (it is initialised there, and saved with it)
+        if table.initial_accumulator_value != self.initial_accumulator_value:
+            raise ValueError(f"FtrlOptimizer.apply: the table's accumulators start at "
+                             f"{table.initial_accumulator_value}, this optimizer's initial_accumulator_value is "
+                             f"{self.initial_accumulator_value}: build the LinearTable with the optimizer's value")
+        lib = _lib.load()
+        args, keep = _wide_args(table, *table.lookups)
+        with torch.no_grad():
+            check(lib.dr_wide_ftrl(*args, self.learning_rate, self.l1, self.l2, _stream()), "dr_wide_ftrl")
+
+
+def cross_hash(values, value_offsets, row_splits, B: int, num_buckets: int, hash_key: int):
+    """crossed_column on the device (dr_cross_hash).  values[k]: CUDA int64 values, or uint8 bytes of strings with
+    value_offsets[k] (CUDA int64 [n+1]); row_splits[k]: CUDA int64 [B+1] or None (one value per example).
+    -> ids [B] (-1: no cross) when every key is single-valued, else (flat ids, row_splits [B+1])."""
+    import ctypes as C
+    lib = _lib.load()
+    K = len(values)
+    dev = values[0].device
+    for t in list(values) + [t for t in value_offsets if t is not None] + [t for t in row_splits if t is not None]:
+        if not t.is_cuda or not t.is_contiguous():
+            raise _lib.DeepRecError("cross_hash: every input must be a contiguous CUDA tensor")
+    # the kernel reads B values (or B + 1 splits) of every key: check the lengths before it runs
+    n = [v.numel() if o is None else o.numel() - 1 for v, o in zip(values, value_offsets)]
+    for k, (nk, s) in enumerate(zip(n, row_splits)):
+        if s is None and nk != B:
+            raise ValueError(f"cross_hash: key {k} is single-valued with {nk} values for a batch of {B}")
+        if s is not None and s.numel() != B + 1:
+            raise ValueError(f"cross_hash: key {k} has {s.numel()} row splits for a batch of {B}")
+    ragged = [k for k, s in enumerate(row_splits) if s is not None]
+    if ragged and B > 0:
+        ends = torch.stack([row_splits[k][-1] for k in ragged]).tolist()
+        for k, e in zip(ragged, ends):
+            if e > n[k]:
+                raise ValueError(f"cross_hash: key {k}'s row splits end at {e}, past its {n[k]} values")
+    # an empty values tensor has no storage; the kernel reads none of it but needs a non-null pointer
+    values = [v if v.numel() else v.new_zeros((1,)) for v in values]
+    vp = (C.c_void_p * K)(*[v.data_ptr() for v in values])
+    op = (C.c_void_p * K)(*[None if o is None else o.data_ptr() for o in value_offsets])
+    sp = (C.c_void_p * K)(*[None if s is None else s.data_ptr() for s in row_splits])
+    hk = int(hash_key) & 0xFFFFFFFFFFFFFFFF
+    if all(s is None for s in row_splits):
+        out = torch.empty((B,), dtype=torch.int64, device=dev)
+        check(lib.dr_cross_hash(K, vp, op, sp, B, hk, int(num_buckets), None, out.data_ptr(), _stream()),
+              "dr_cross_hash")
+        return out
+    splits = torch.empty((B + 1,), dtype=torch.int64, device=dev)
+    check(lib.dr_cross_hash(K, vp, op, sp, B, hk, int(num_buckets), splits.data_ptr(), None, _stream()),
+          "dr_cross_hash")
+    splits = torch.cumsum(splits, 0)
+    out = torch.empty((int(splits[-1]),), dtype=torch.int64, device=dev)
+    if out.numel() == 0:
+        return out, splits
+    check(lib.dr_cross_hash(K, vp, op, sp, B, hk, int(num_buckets), splits.data_ptr(), out.data_ptr(), _stream()),
+          "dr_cross_hash")
+    return out, splits
+
+
 def hash_bucket_i64(values: torch.Tensor, num_buckets: int) -> torch.Tensor:
     """tf.strings.to_hash_bucket_fast(tf.as_string(values), num_buckets) for a CUDA int64 tensor."""
     lib = _lib.load()
@@ -1095,7 +1234,9 @@ class EmbedFMMixed(torch.autograd.Function):
     @staticmethod
     def forward(ctx, ids, weight, linear, bias, meta, bags):
         lib = _lib.load()
-        if not meta.with_linear or bias is None:
+        if not meta.with_linear:
+            return EmbedFMMixed._forward_no_linear(ctx, ids, weight, meta, bags)
+        if bias is None:
             raise ValueError("EmbedFMMixed needs a collection with the first-order term (with_linear=True)")
         ids = _ids(ids).clone()
         B, S = ids.shape
@@ -1140,7 +1281,73 @@ class EmbedFMMixed(torch.autograd.Function):
         return stack, logit
 
     @staticmethod
+    def _forward_no_linear(ctx, ids, weight, meta, bags):
+        """Embeddings only (a collection without first-order weights, e.g. WDL's deep half): the bags are
+        mean-reduced into scratch tables and one dr_embed_fm_fwd without a logit gathers the stack."""
+        lib = _lib.load()
+        ids = _ids(ids).clone()
+        B, S = ids.shape
+        D, RS = meta.dim, meta.row_stride
+        dev = weight.device
+        tp, _, rows = meta.pointers(weight, None)
+        tp, rows = tp.clone(), rows.clone()
+        slots = sorted(bags)
+        scratch = torch.empty((len(slots), B, RS), device=dev, dtype=torch.float32)
+        ar = torch.arange(B, device=dev, dtype=ids.dtype)
+        saved_bags = []
+        for k, s in enumerate(slots):
+            bid, bsp = bags[s]
+            bid, bsp = _ids(bid, "bag ids"), _splits(bsp)
+            if bsp.numel() != B + 1:
+                raise ValueError(f"slot {s}: row_splits has {bsp.numel()} entries, expected B+1 = {B + 1}")
+            off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
+            _bag_fwd(lib, weight.data_ptr() + 4 * off * RS, n_rows, RS, bid, bsp, B, D, "mean", scratch[k].data_ptr(),
+                     RS)
+            tp[s] = scratch[k].data_ptr()
+            rows[s] = B
+            ids[:, s] = ar
+            saved_bags.append((s, bid, bsp))
+        stack = torch.empty((B, S, D), device=dev, dtype=torch.float32)
+        check(lib.dr_embed_fm_fwd(tp.data_ptr(), None, rows.data_ptr(), ids.data_ptr(), ids.element_size(), None,
+                                  B, S, D, RS, meta.lin_stride, 0, stack.data_ptr(), None, None, _stream()),
+              "dr_embed_fm_fwd")
+        ctx.meta, ctx.saved_bags = meta, saved_bags
+        ctx.save_for_backward(ids, stack, None, weight, None, None, rows)
+        dummy = stack.new_zeros((0,))
+        ctx.mark_non_differentiable(dummy)
+        return stack, dummy
+
+    @staticmethod
+    def _backward_no_linear(ctx, g_stack):
+        lib = _lib.load()
+        ids, stack, _, weight, _, _, rows = ctx.saved_tensors
+        meta = ctx.meta
+        if g_stack is None:
+            return None, None, None, None, None, None
+        g_stack = _f32(g_stack, "g_stack")
+        B, S = ids.shape
+        D, RS = meta.dim, meta.row_stride
+        fused_sgd = meta.sparse_lr is not None
+        gw, scale = (weight, -float(meta.sparse_lr)) if fused_sgd else (torch.zeros_like(weight), 1.0)
+        tp, _, _ = meta.pointers(gw, None, cache=False)
+        tp = tp.clone()
+        gscratch = torch.zeros((len(ctx.saved_bags), B, RS), device=weight.device, dtype=torch.float32)
+        for k, (s, _, _) in enumerate(ctx.saved_bags):
+            tp[s] = gscratch[k].data_ptr()
+        with torch.no_grad():
+            check(lib.dr_embed_fm_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(), stack.data_ptr(), None, None,
+                                      g_stack.data_ptr(), B, S, D, RS, meta.lin_stride, 0, tp.data_ptr(), None, None,
+                                      scale, _stream()), "dr_embed_fm_bwd")
+            for k, (s, bid, bsp) in enumerate(ctx.saved_bags):
+                off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
+                _bag_bwd(lib, bid, bsp, B, D, "mean", gscratch[k].data_ptr(), RS, n_rows, RS,
+                         gw.data_ptr() + 4 * off * RS, 1.0)
+        return None, (None if fused_sgd else gw), None, None, None, None
+
+    @staticmethod
     def backward(ctx, g_stack, g_logit):
+        if not ctx.meta.with_linear:
+            return EmbedFMMixed._backward_no_linear(ctx, g_stack)
         lib = _lib.load()
         ids, stack, sum_e, weight, linear, bias, rows = ctx.saved_tensors
         meta = ctx.meta

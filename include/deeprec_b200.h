@@ -626,6 +626,48 @@ uint64_t dr_fingerprint64_host(const uint8_t* s, int64_t len);
  * (TF default -1 => zero embedding row, all-zero indicator).                                            */
 int dr_vocab_lookup_i64(const int64_t* values, int64_t n, const int64_t* keys_sorted, const int64_t* vocab_index,
                         int64_t vocab_size, int64_t default_id, int64_t* out_ids, void* stream);
+/* crossed_column (replaces tf.feature_column.crossed_column = tf.sparse.cross_hashed, example
+ * train_wdl_on_movielens_estimator.py:37-47).  K keys (2 <= K <= 16); values / value_offsets / row_splits are HOST
+ * arrays of K pointers (device pointers for dr_cross_hash, host pointers for the _host twin):
+ *   values[k]         int64 values, or the bytes of strings when value_offsets[k] != NULL ([n+1] byte offsets);
+ *   row_splits[k]     [B+1] splits of a multi-valued key, NULL when the key has one value per example.
+ * A single-valued key drops its ignore values (empty string, -1); a multi-valued key keeps every value, as TensorFlow
+ * keeps a SparseTensor's.  Each combination of one kept value per key (last key fastest)
+ * gives id = (FingerprintCat64 chain from hash_key over Fingerprint64(string) / raw int64) mod num_buckets.
+ *   out_splits == NULL         every key single-valued: out_ids[b] = the cross of b, -1 if a key has no kept value;
+ *   out_splits, out_ids NULL   out_splits[0] = 0, out_splits[b+1] = number of crosses of b (caller takes the cumsum);
+ *   both given                 the crosses of b are written to out_ids[out_splits[b] ..].                        */
+int dr_cross_hash(int K, const void* const* values, const int64_t* const* value_offsets,
+                  const int64_t* const* row_splits, int64_t B, uint64_t hash_key, int64_t num_buckets,
+                  int64_t* out_splits, int64_t* out_ids, void* stream);
+int dr_cross_hash_host(int K, const void* const* values, const int64_t* const* value_offsets,
+                       const int64_t* const* row_splits, int64_t B, uint64_t hash_key, int64_t num_buckets,
+                       int64_t* out_splits, int64_t* out_ids);
+
+/* Wide part of Wide & Deep: tf.feature_column.linear_model over indicator / crossed columns
+ * (estimator/models/ranking/wide_and_deep.py:31-33) and tf.train.FtrlOptimizer on it (train_wdl_on_movielens_estimator.py
+ * :65-69).  state: 16-B aligned [total_rows + 1, 4] records {w, z, n, g} (weight, FTRL linear and accumulator slots,
+ * batch gradient); record total_rows is the bias.  rows / slot_offsets [S] (device): slot s owns rows
+ * [slot_offsets[s], + rows[s]).  ids [B, S] int64 single-valued lookups; n_bags (<= DR_WIDE_MAX_BAGS) multi-valued
+ * slots replace their column of ids: bag_slots / bag_ids / bag_splits are HOST arrays (device pointers to flat ids and
+ * [B+1] splits).  An id outside [0, rows[s]) contributes nothing; duplicates count.
+ *   dr_wide_fwd   logit[b] = bias + sum of w over the lookups of b.
+ *   dr_wide_bwd   g[row] += g_logit[b] per lookup; g[bias] += sum_b g_logit[b] (float atomics).
+ *   dr_wide_ftrl  each touched row (and the bias) applies ApplyFtrl with learning_rate_power = -0.5 once:
+ *                 n' = n + g^2; z += g - (sqrt(n') - sqrt(n)) / lr * w;
+ *                 w = |z| > l1 ? (sign(z) l1 - z) / (sqrt(n') / lr + 2 l2) : 0; n = n'; then g = 0.
+ *                 Untouched rows are not written: equal to TensorFlow's dense update while w is the function of
+ *                 (z, n) the last update wrote (true from w = z = 0).  DR_EINVAL for lr <= 0, l1 < 0 or l2 < 0.   */
+#define DR_WIDE_MAX_BAGS 16
+int dr_wide_fwd(const float* state, int64_t total_rows, const int64_t* rows, const int64_t* slot_offsets,
+                const int64_t* ids, int64_t B, int S, int n_bags, const int* bag_slots, const int64_t* const* bag_ids,
+                const int64_t* const* bag_splits, float* logit, void* stream);
+int dr_wide_bwd(float* state, int64_t total_rows, const int64_t* rows, const int64_t* slot_offsets,
+                const int64_t* ids, int64_t B, int S, int n_bags, const int* bag_slots, const int64_t* const* bag_ids,
+                const int64_t* const* bag_splits, const float* g_logit, void* stream);
+int dr_wide_ftrl(float* state, int64_t total_rows, const int64_t* rows, const int64_t* slot_offsets,
+                 const int64_t* ids, int64_t B, int S, int n_bags, const int* bag_slots, const int64_t* const* bag_ids,
+                 const int64_t* const* bag_splits, float lr, float l1, float l2, void* stream);
 
 /* Multi-valued slot (VarLenFeature, e.g. "Genres" movielens.py:122): ids [nnz] + row_splits [B+1].
  *   out[b, :] = combine_j table[ids[j], :D]  over the VALID ids (0 <= id < rows) of bag b;
