@@ -6,7 +6,7 @@ index r div G.  Shared by the CUDA path (sharded.py) and the gloo CPU protocol t
 """
 from __future__ import annotations
 
-from typing import List, Sequence
+from typing import List, NamedTuple, Sequence
 
 
 def slot_offsets(rows: Sequence[int]) -> List[int]:
@@ -28,6 +28,24 @@ def local_row(row: int, world: int) -> int:
 def local_rows(total_rows: int, rank: int, world: int) -> int:
     """Number of global rows r in [0, total_rows) with r % world == rank."""
     return (total_rows - rank + world - 1) // world if total_rows > rank else 0
+
+
+class P2PLayout(NamedTuple):
+    max_rows: int      # rows allocated on every rank: local_rows(total, 0, world)
+    vdim: int          # floats per row (the row stride)
+    lin_in_row: bool   # first-order weight at float `dim` of the row (flags = DR_EMBED_LIN_IN_ROW)
+    lin_offset: int    # floats from the shard base to the trailing first-order array (0: in the row)
+    numel: int         # floats of the whole symmetric allocation
+
+
+def p2p_layout(total_rows: int, dim: int, world: int) -> P2PLayout:
+    """One rank's shard of the p2p exchange, the same size on every rank.  Narrow rows (dim + 1 <= 32) are
+    [emb | w | pad] in ONE 128-B line; wide rows (dim = 32 ... 128) are exactly `dim` floats (whole lines, no
+    padding), followed by the [max_rows] first-order weights rounded up to 4 floats."""
+    max_rows = local_rows(total_rows, 0, world)
+    if dim + 1 <= 32:
+        return P2PLayout(max_rows, 32, True, 0, max_rows * 32)
+    return P2PLayout(max_rows, dim, False, max_rows * dim, max_rows * dim + (max_rows + 3) // 4 * 4)
 
 
 def capacity(n_lookups: int, world: int, slack: float = 0.04, floor: int = 4096) -> int:

@@ -42,28 +42,26 @@ class ShardedEmbedding:
         self.dim, self.rank, self.world = int(dim), rank, world
         self.total_rows = sum(self.rows_list)
         self.local_rows = shard_plan.local_rows(self.total_rows, rank, world)
-        max_rows = shard_plan.local_rows(self.total_rows, 0, world)       # same size on every rank
-        # narrow rows (D <= 28): [emb | w | pad] = ONE 128-B line, the weight rides in the row (flags = LIN_IN_ROW).
-        # wide rows (BASELINE C3-C5, D = 32 ... 128): rows of exactly D floats (whole lines, no padding) and the
-        # first-order weights as a [max_rows] array trailing the shard in the same symmetric allocation.
-        self.lin_in_row = exchange == "nccl" or self.dim + 1 <= 32
+        # p2p: narrow rows (D <= 28) are [emb | w | pad] = ONE 128-B line, the weight rides in the row
+        # (flags = LIN_IN_ROW); wide rows (BASELINE C3-C5, D = 32 ... 128) are exactly D floats and the first-order
+        # weights a [max_rows] array trailing the shard in the same symmetric allocation (shard_plan.p2p_layout).
         if exchange == "nccl":
             if dim + 4 > 128:
                 raise NotImplementedError("exchange='nccl' moves fused rows of D + 4 <= 128 floats; use exchange='p2p' "
                                           "for wider rows")
-            self.vdim = self.dim + 4
+            self.lin_in_row, self.vdim, self.lin_offset = True, self.dim + 4, 0
         else:
-            self.vdim = 32 if self.lin_in_row else self.dim
+            layout = shard_plan.p2p_layout(self.total_rows, self.dim, world)
+            self.lin_in_row, self.vdim, self.lin_offset = layout.lin_in_row, layout.vdim, layout.lin_offset
         self.flags = 1 if self.lin_in_row else 0
-        self.lin_offset = 0 if self.lin_in_row else max_rows * self.vdim         # floats from the shard base
         self.device = device
         self.handle = None
         self.peer_ptrs = None
         std = 1.0 / self.dim ** 0.5
         if exchange == "p2p":
             import torch.distributed._symmetric_memory as symm_mem
-            numel = max_rows * self.vdim + (0 if self.lin_in_row else (max_rows + 3) // 4 * 4)
-            buf = symm_mem.empty((numel,), dtype=torch.float32, device=device)
+            max_rows = layout.max_rows
+            buf = symm_mem.empty((layout.numel,), dtype=torch.float32, device=device)
             self.handle = symm_mem.rendezvous(buf, group if group is not None else dist.group.WORLD)
             buf.zero_()
             w = buf[:max_rows * self.vdim].view(max_rows, self.vdim)[:self.local_rows]

@@ -18,7 +18,8 @@ the collectives of this step also order every rank's remote reads before any rem
 Towers are the embedding tables themselves (plain DSSM); MLP towers stay single-GPU (TwoTower) in this round.
 
 Tests: the exchange plan by the world-2 gloo test (tests/test_two_tower_protocol_cpu.py); the CUDA step at world 1 by
-tests/test_gpu_zz_next_rows.py and at world 2 by tests/test_gpu_sharded.py (torchrun worker).
+tests/test_gpu_zz_next_rows.py and at world 2 by tests/test_gpu_sharded.py (torchrun worker); its gather / update kernel
+calls at world sizes up to 64, emulated on one GPU, by tests/test_gpu_sharded_emulated.py.
 """
 from __future__ import annotations
 
