@@ -107,6 +107,8 @@ _SIGS = {
     "dr_wide_ftrl": [_p, _i64, _p, _p, _p, _i64, _i, _i, _p, _p, _p, _f, _f, _f, _p],
     "dr_embed_bag_fwd": [_p, _i64, _i64, _p, _i, _p, _i64, _i, _i, _p, _i64, _p],
     "dr_embed_bag_bwd": [_p, _i, _p, _i64, _i, _i, _p, _i64, _i64, _i64, _p, _f, _p],
+    "dr_fnn_input_fwd": [_p, _p, _p, _p, _i, _i64, _i64, _i, _p, _i64, _i, _i, _i64, _p, _p],
+    "dr_fnn_input_bwd": [_p, _i, _p, _p, _i64, _i, _i, _i64, _i64, _i64, _i, _p, _p, _f, _p],
     "dr_crc32c_host": [_p, _i64],
     "dr_masked_crc32c_host": [_p, _i64],
     "dr_tfrecord_index": [_p, _i64, _i, _p, _p, _i64],

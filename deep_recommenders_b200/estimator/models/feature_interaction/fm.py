@@ -48,6 +48,25 @@ class FM(object):
     def parameters(self):
         return self.collection.parameters()
 
+    def export(self, path):
+        """Write the trained tables to `path` as one torch.save file of CPU tensors, keyed by feature name like the two
+        dicts the reference's FNN reads from an FM SavedModel (fnn.py:32-48) -- what ranking.FNN warm-starts from:
+
+            {"format": 1, "bias": [1], "linear": {key: [rows, 1]}, "factorized": {key: [rows, D]}}
+
+        Loadable with torch.load(path, weights_only=True).  The tensors are copies: the file does not share storage
+        with the collection's arena."""
+        coll = self.collection
+
+        def cpu(t):
+            return t.detach().to("cpu", copy=True).contiguous()
+
+        state = {"format": 1, "bias": cpu(coll.bias).reshape(1), "linear": {}, "factorized": {}}
+        for s, key in enumerate(self._keys):
+            state["linear"][key] = cpu(coll.linear_of(s)).reshape(-1, 1)
+            state["factorized"][key] = cpu(coll.table(s))
+        torch.save(state, path)
+
     def __call__(self, *args, **kwargs):
         return self.call(*args, **kwargs)
 

@@ -1218,6 +1218,84 @@ class EmbedBag(torch.autograd.Function):
         return (None if fused else tgt), None, None, None, None, None, None
 
 
+def _reduce_bags(lib, ids, weight, linear, meta, bags):
+    """Reduce every multi-valued slot of `bags` into a per-batch scratch "table" of B rows in the collection's own
+    row layout: embedding columns = mean of the bag's valid rows and, when the collection has first-order weights,
+    first-order entry = SUM of their weights (the indicator column is a multi-hot count vector).  A fused kernel then
+    reads slot s from that scratch with ids 0..B-1.
+
+    Returns (ids, table_ptrs, lin_ptrs, rows, saved_bags, scratch): copies of ids and of the collection's device
+    pointer arrays with the bag slots redirected, the (slot, flat ids, row_splits) list the backward needs, and the
+    scratch tensors, which the caller keeps alive until its kernel is enqueued."""
+    ids = _ids(ids).clone()
+    B, S = ids.shape
+    D, RS = meta.dim, meta.row_stride
+    dev = weight.device
+    with_lin = meta.with_linear
+    fused_rows = meta.layout == "fused"
+    tp, lp, rows = meta.pointers(weight, linear)
+    tp, lp, rows = tp.clone(), lp.clone(), rows.clone()
+    slots = sorted(bags)
+    scratch = torch.zeros((len(slots), B, RS), device=dev, dtype=torch.float32)
+    scratch_lin = None if (fused_rows or not with_lin) else torch.zeros((len(slots), B), device=dev, dtype=torch.float32)
+    ar = torch.arange(B, device=dev, dtype=ids.dtype)
+    saved_bags = []
+    for k, s in enumerate(slots):
+        bid, bsp = bags[s]
+        bid, bsp = _ids(bid, "bag ids"), _splits(bsp)
+        if bsp.numel() != B + 1:
+            raise ValueError(f"slot {s}: row_splits has {bsp.numel()} entries, expected B+1 = {B + 1}")
+        off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
+        base = weight.data_ptr() + 4 * off * RS
+        _bag_fwd(lib, base, n_rows, RS, bid, bsp, B, D, "mean", scratch[k].data_ptr(), RS)
+        if with_lin:
+            if fused_rows:
+                _bag_fwd(lib, base + 4 * D, n_rows, RS, bid, bsp, B, 1, "sum", scratch[k].data_ptr() + 4 * D, RS)
+                lp[s] = scratch[k].data_ptr() + 4 * D
+            else:
+                _bag_fwd(lib, linear.data_ptr() + 4 * off, n_rows, 1, bid, bsp, B, 1, "sum",
+                         scratch_lin[k].data_ptr(), 1)
+                lp[s] = scratch_lin[k].data_ptr()
+        tp[s] = scratch[k].data_ptr()
+        rows[s] = B
+        ids[:, s] = ar
+        saved_bags.append((s, bid, bsp))
+    return ids, tp, lp, rows, saved_bags, (scratch, scratch_lin)
+
+
+def _bag_grad_scratch(meta, tp, lp, saved_bags, B, with_lin, dev):
+    """Backward twin of _reduce_bags: redirect the bag slots of the gradient pointer arrays (tp, lp, modified in
+    place) to zeroed scratch gradient tables of B rows; returns (gscratch, gscratch_lin)."""
+    D, RS = meta.dim, meta.row_stride
+    fused_rows = meta.layout == "fused"
+    nb = len(saved_bags)
+    gscratch = torch.zeros((nb, B, RS), device=dev, dtype=torch.float32)
+    gscratch_lin = None if (fused_rows or not with_lin) else torch.zeros((nb, B), device=dev, dtype=torch.float32)
+    for k, (s, _, _) in enumerate(saved_bags):
+        tp[s] = gscratch[k].data_ptr()
+        if with_lin:
+            lp[s] = gscratch[k].data_ptr() + 4 * D if fused_rows else gscratch_lin[k].data_ptr()
+    return gscratch, gscratch_lin
+
+
+def _spread_bag_grads(lib, meta, gw, gl, saved_bags, gscratch, gscratch_lin, B, with_lin):
+    """Spread each bag slot's scratch gradient over the bag's rows of gw (embedding / count) and of the first-order
+    weights (x 1) with dr_embed_bag_bwd.  The scratch already carries the caller's scale: it is spread with 1."""
+    D, RS = meta.dim, meta.row_stride
+    fused_rows = meta.layout == "fused"
+    for k, (s, bid, bsp) in enumerate(saved_bags):
+        off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
+        base = gw.data_ptr() + 4 * off * RS
+        _bag_bwd(lib, bid, bsp, B, D, "mean", gscratch[k].data_ptr(), RS, n_rows, RS, base, 1.0)
+        if not with_lin:
+            continue
+        if fused_rows:
+            _bag_bwd(lib, bid, bsp, B, 1, "sum", gscratch[k].data_ptr() + 4 * D, RS, n_rows, RS, base + 4 * D, 1.0)
+        else:
+            _bag_bwd(lib, bid, bsp, B, 1, "sum", gscratch_lin[k].data_ptr(), 1, n_rows, 1,
+                     gl.data_ptr() + 4 * off, 1.0)
+
+
 class EmbedFMMixed(torch.autograd.Function):
     """EmbedFM for a collection in which some slots are multi-valued (SURVEY 8f #2).
 
@@ -1226,7 +1304,8 @@ class EmbedFMMixed(torch.autograd.Function):
     indicator column is a multi-hot count vector); the fused gather + FM kernel then reads slot r from that
     scratch with ids 0..B-1, so the whole model is still ONE dr_embed_fm_fwd launch.  Backward mirrors it: the
     fused backward accumulates slot r's per-example gradient in a scratch grad table, dr_embed_bag_bwd spreads
-    it over the bag's rows (embedding / count, first-order x 1).
+    it over the bag's rows (embedding / count, first-order x 1).  The scratch handling is shared with FnnInputFn
+    (_reduce_bags, _bag_grad_scratch, _spread_bag_grads).
 
     ids [B, S]: columns of ragged slots are ignored.  bags: {slot: (flat_ids, row_splits[B+1])}.
     """
@@ -1238,38 +1317,10 @@ class EmbedFMMixed(torch.autograd.Function):
             return EmbedFMMixed._forward_no_linear(ctx, ids, weight, meta, bags)
         if bias is None:
             raise ValueError("EmbedFMMixed needs a collection with the first-order term (with_linear=True)")
-        ids = _ids(ids).clone()
+        ids, tp, lp, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, linear, meta, bags)
         B, S = ids.shape
         D, RS = meta.dim, meta.row_stride
         dev = weight.device
-        fused_rows = meta.layout == "fused"
-        tp, lp, rows = meta.pointers(weight, linear)
-        tp, lp, rows = tp.clone(), lp.clone(), rows.clone()
-        slots = sorted(bags)
-        scratch = torch.zeros((len(slots), B, RS), device=dev, dtype=torch.float32)
-        scratch_lin = None if fused_rows else torch.zeros((len(slots), B), device=dev, dtype=torch.float32)
-        ar = torch.arange(B, device=dev, dtype=ids.dtype)
-        saved_bags = []
-        for k, s in enumerate(slots):
-            bid, bsp = bags[s]
-            bid, bsp = _ids(bid, "bag ids"), _splits(bsp)
-            if bsp.numel() != B + 1:
-                raise ValueError(f"slot {s}: row_splits has {bsp.numel()} entries, expected B+1 = {B + 1}")
-            off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
-            base = weight.data_ptr() + 4 * off * RS
-            _bag_fwd(lib, base, n_rows, RS, bid, bsp, B, D, "mean", scratch[k].data_ptr(), RS)
-            if fused_rows:
-                _bag_fwd(lib, base + 4 * D, n_rows, RS, bid, bsp, B, 1, "sum", scratch[k].data_ptr() + 4 * D, RS)
-                lin_ptr = scratch[k].data_ptr() + 4 * D
-            else:
-                _bag_fwd(lib, linear.data_ptr() + 4 * off, n_rows, 1, bid, bsp, B, 1, "sum",
-                         scratch_lin[k].data_ptr(), 1)
-                lin_ptr = scratch_lin[k].data_ptr()
-            tp[s] = scratch[k].data_ptr()
-            lp[s] = lin_ptr
-            rows[s] = B
-            ids[:, s] = ar
-            saved_bags.append((s, bid, bsp))
         stack = torch.empty((B, S, D), device=dev, dtype=torch.float32)
         sum_e = torch.empty((B, D), device=dev, dtype=torch.float32)
         logit = torch.empty((B,), device=dev, dtype=torch.float32)
@@ -1285,28 +1336,10 @@ class EmbedFMMixed(torch.autograd.Function):
         """Embeddings only (a collection without first-order weights, e.g. WDL's deep half): the bags are
         mean-reduced into scratch tables and one dr_embed_fm_fwd without a logit gathers the stack."""
         lib = _lib.load()
-        ids = _ids(ids).clone()
+        ids, tp, _, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, None, meta, bags)
         B, S = ids.shape
         D, RS = meta.dim, meta.row_stride
         dev = weight.device
-        tp, _, rows = meta.pointers(weight, None)
-        tp, rows = tp.clone(), rows.clone()
-        slots = sorted(bags)
-        scratch = torch.empty((len(slots), B, RS), device=dev, dtype=torch.float32)
-        ar = torch.arange(B, device=dev, dtype=ids.dtype)
-        saved_bags = []
-        for k, s in enumerate(slots):
-            bid, bsp = bags[s]
-            bid, bsp = _ids(bid, "bag ids"), _splits(bsp)
-            if bsp.numel() != B + 1:
-                raise ValueError(f"slot {s}: row_splits has {bsp.numel()} entries, expected B+1 = {B + 1}")
-            off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
-            _bag_fwd(lib, weight.data_ptr() + 4 * off * RS, n_rows, RS, bid, bsp, B, D, "mean", scratch[k].data_ptr(),
-                     RS)
-            tp[s] = scratch[k].data_ptr()
-            rows[s] = B
-            ids[:, s] = ar
-            saved_bags.append((s, bid, bsp))
         stack = torch.empty((B, S, D), device=dev, dtype=torch.float32)
         check(lib.dr_embed_fm_fwd(tp.data_ptr(), None, rows.data_ptr(), ids.data_ptr(), ids.element_size(), None,
                                   B, S, D, RS, meta.lin_stride, 0, stack.data_ptr(), None, None, _stream()),
@@ -1329,19 +1362,14 @@ class EmbedFMMixed(torch.autograd.Function):
         D, RS = meta.dim, meta.row_stride
         fused_sgd = meta.sparse_lr is not None
         gw, scale = (weight, -float(meta.sparse_lr)) if fused_sgd else (torch.zeros_like(weight), 1.0)
-        tp, _, _ = meta.pointers(gw, None, cache=False)
+        tp, lp, _ = meta.pointers(gw, None, cache=False)
         tp = tp.clone()
-        gscratch = torch.zeros((len(ctx.saved_bags), B, RS), device=weight.device, dtype=torch.float32)
-        for k, (s, _, _) in enumerate(ctx.saved_bags):
-            tp[s] = gscratch[k].data_ptr()
+        gscratch, gscratch_lin = _bag_grad_scratch(meta, tp, lp, ctx.saved_bags, B, False, weight.device)
         with torch.no_grad():
             check(lib.dr_embed_fm_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(), stack.data_ptr(), None, None,
                                       g_stack.data_ptr(), B, S, D, RS, meta.lin_stride, 0, tp.data_ptr(), None, None,
                                       scale, _stream()), "dr_embed_fm_bwd")
-            for k, (s, bid, bsp) in enumerate(ctx.saved_bags):
-                off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
-                _bag_bwd(lib, bid, bsp, B, D, "mean", gscratch[k].data_ptr(), RS, n_rows, RS,
-                         gw.data_ptr() + 4 * off * RS, 1.0)
+            _spread_bag_grads(lib, meta, gw, None, ctx.saved_bags, gscratch, gscratch_lin, B, False)
         return None, (None if fused_sgd else gw), None, None, None, None
 
     @staticmethod
@@ -1354,7 +1382,6 @@ class EmbedFMMixed(torch.autograd.Function):
         B, S = ids.shape
         D, RS = meta.dim, meta.row_stride
         dev = weight.device
-        fused_rows = meta.layout == "fused"
         g_stack = None if g_stack is None else _f32(g_stack, "g_stack")
         g_logit = None if g_logit is None else _f32(g_logit, "g_logit")
         if g_stack is None and g_logit is None:
@@ -1371,30 +1398,92 @@ class EmbedFMMixed(torch.autograd.Function):
             scale = 1.0
         tp, lp, _ = meta.pointers(gw, gl, cache=False)
         tp, lp = tp.clone(), lp.clone()
-        nb = len(ctx.saved_bags)
-        gscratch = torch.zeros((nb, B, RS), device=dev, dtype=torch.float32)
-        gscratch_lin = None if fused_rows else torch.zeros((nb, B), device=dev, dtype=torch.float32)
-        for k, (s, _, _) in enumerate(ctx.saved_bags):
-            tp[s] = gscratch[k].data_ptr()
-            lp[s] = gscratch[k].data_ptr() + 4 * D if fused_rows else gscratch_lin[k].data_ptr()
+        gscratch, gscratch_lin = _bag_grad_scratch(meta, tp, lp, ctx.saved_bags, B, True, dev)
         with torch.no_grad():
             check(lib.dr_embed_fm_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(), stack.data_ptr(),
                                       sum_e.data_ptr(), g_logit.data_ptr(), _ptr(g_stack), B, S, D, RS,
                                       meta.lin_stride, meta.flags, tp.data_ptr(), lp.data_ptr(), _ptr(gb), scale,
                                       _stream()), "dr_embed_fm_bwd")
-            for k, (s, bid, bsp) in enumerate(ctx.saved_bags):
-                off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
-                base = gw.data_ptr() + 4 * off * RS
-                # the scratch already carries `scale`: spread it with scale = 1
-                _bag_bwd(lib, bid, bsp, B, D, "mean", gscratch[k].data_ptr(), RS, n_rows, RS, base, 1.0)
-                if fused_rows:
-                    _bag_bwd(lib, bid, bsp, B, 1, "sum", gscratch[k].data_ptr() + 4 * D, RS, n_rows, RS, base + 4 * D, 1.0)
-                else:
-                    _bag_bwd(lib, bid, bsp, B, 1, "sum", gscratch_lin[k].data_ptr(), 1, n_rows, 1,
-                             gl.data_ptr() + 4 * off, 1.0)
+            _spread_bag_grads(lib, meta, gw, gl, ctx.saved_bags, gscratch, gscratch_lin, B, True)
         if fused_sgd:
             return None, None, None, None, None, None
         return None, gw, gl, gb, None, None
+
+
+def fnn_layout(S: int, D: int):
+    """(P, ld) of FNN's tower input row (dr_fnn_input_fwd): P = round_up(1 + S, 4) columns of [bias | w_1..w_S | 0],
+    then the S embeddings; ld = P + S * D is a multiple of 4 whenever D is."""
+    P = (1 + S + 3) // 4 * 4
+    return P, P + S * D
+
+
+class FnnInputFn(torch.autograd.Function):
+    """x [B, ld] = FnnInputFn(ids, weight, linear, bias, meta, bags): FNN's tower input
+    concat([bias, w_1..w_S, e_1..e_S]) in the padded row layout of fnn_layout, written by ONE dr_fnn_input_fwd over
+    the collection `meta` (fused or split layout).  `bias` is a device [1] tensor the kernel reads (a constant of
+    the model: it gets no gradient).  Multi-valued slots (bags, {slot: (flat_ids, row_splits)}) are reduced first
+    into scratch tables as EmbedFMMixed does (embedding = mean, w = sum).
+
+    Backward: dr_fnn_input_bwd scatter-adds the embedding and w columns of g_x into dense gradients of weight /
+    linear (meta.sparse_lr is None), or applies the fused sparse SGD in place (meta.sparse_lr = lr).
+    """
+
+    @staticmethod
+    def forward(ctx, ids, weight, linear, bias, meta, bags=None):
+        lib = _lib.load()
+        if not meta.with_linear:
+            raise ValueError("FnnInputFn needs a collection with first-order weights (with_linear=True)")
+        bias = _f32(bias, "bias")
+        if bias.numel() != 1:
+            raise ValueError(f"FnnInputFn: bias must have one element, got {tuple(bias.shape)}")
+        if bags:
+            ids, tp, lp, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, linear, meta, bags)
+        else:
+            ids = _ids(ids)
+            tp, lp, rows = meta.pointers(weight, linear)
+            saved_bags = []
+        B, S = ids.shape
+        D = meta.dim
+        _, ld = fnn_layout(S, D)
+        x = torch.empty((B, ld), device=weight.device, dtype=torch.float32)
+        check(lib.dr_fnn_input_fwd(tp.data_ptr(), lp.data_ptr(), rows.data_ptr(), ids.data_ptr(), ids.element_size(),
+                                   meta.row_stride, meta.lin_stride, meta.flags, bias.data_ptr(), B, S, D, ld,
+                                   x.data_ptr(), _stream()), "dr_fnn_input_fwd")
+        ctx.meta, ctx.saved_bags = meta, saved_bags
+        ctx.save_for_backward(ids, weight, linear, rows)
+        return x
+
+    @staticmethod
+    def backward(ctx, g_x):
+        lib = _lib.load()
+        ids, weight, linear, rows = ctx.saved_tensors
+        meta = ctx.meta
+        if g_x is None:
+            return None, None, None, None, None, None
+        g_x = _f32(g_x, "g_x")
+        B, S = ids.shape
+        D = meta.dim
+        _, ld = fnn_layout(S, D)
+        fused_sgd = meta.sparse_lr is not None
+        if fused_sgd:
+            gw, gl, scale = weight, linear, -float(meta.sparse_lr)
+        else:
+            gw = torch.zeros_like(weight)
+            gl = None if linear is None else torch.zeros_like(linear)
+            scale = 1.0
+        tp, lp, _ = meta.pointers(gw, gl, cache=fused_sgd)
+        if ctx.saved_bags:
+            tp, lp = tp.clone(), lp.clone()
+            gscratch, gscratch_lin = _bag_grad_scratch(meta, tp, lp, ctx.saved_bags, B, True, weight.device)
+        with torch.no_grad():
+            check(lib.dr_fnn_input_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(), g_x.data_ptr(), B, S, D,
+                                       ld, meta.row_stride, meta.lin_stride, meta.flags, tp.data_ptr(), lp.data_ptr(),
+                                       scale, _stream()), "dr_fnn_input_bwd")
+            if ctx.saved_bags:
+                _spread_bag_grads(lib, meta, gw, gl, ctx.saved_bags, gscratch, gscratch_lin, B, True)
+        if fused_sgd:
+            return None, None, None, None, None, None
+        return None, gw, gl, None, None, None
 
 
 def topk_rows(scores_: torch.Tensor, k: int):

@@ -686,6 +686,26 @@ int dr_embed_bag_bwd(const void* ids, int id_bytes, const int64_t* row_splits, i
                      const float* g_out, int64_t g_stride, int64_t rows, int64_t row_stride, float* grad_table,
                      float scale, void* stream);
 
+/* FNN's tower input (estimator/models/ranking/fnn.py:53-82): concat([bias, w_1 .. w_S, e_1 .. e_S]) in one gather.
+ *   Row layout: P = round_up(1 + S, 4), ld = P + S*D; column 0 = *bias, columns 1..S = w_s, columns 1+S..P-1 = 0,
+ *   embedding s at [P + s*D, P + (s+1)*D).  Every embedding segment starts 16-B aligned and ld % 4 == 0.
+ *   table_ptrs / lin_ptrs / rows / ids / id_bytes / row_stride / lin_stride / flags: as dr_embed_fm_fwd; with
+ *   DR_EMBED_LIN_IN_ROW (the fused row layout) w is float D of the row and lin_ptrs may be NULL, otherwise
+ *   lin_ptrs is required.  An id < 0 or >= rows[s] gives a zero embedding and a zero w.
+ *   bias : device [1], read on the device.  out : [B, ld], 16-B aligned.
+ * bwd: for every valid lookup (b, s): grad_table s [id, :D] += scale * g_x[b, P + s*D ...], and its first-order
+ *   weight (float D of the row, or grad_lin_ptrs[s][id * lin_stride]) += scale * g_x[b, 1 + s].  Column 0 and the
+ *   pad are not read.  scale = 1 with zeroed gradient arenas gives the dense gradient, scale = -lr with the
+ *   pointers aliasing the parameters a fused sparse SGD step.
+ * Both: DR_EINVAL for a null pointer, D % 4 != 0 or D outside [4, 128], ld != P + S*D, bad strides or flags;
+ *   DR_EALIGN for a row buffer (out / g_x) that is not 16-B aligned; DR_ENOTSUP for B*S >= 2^31.  B = 0 is a no-op. */
+int dr_fnn_input_fwd(const float* const* table_ptrs, const float* const* lin_ptrs, const int64_t* rows,
+                     const void* ids, int id_bytes, int64_t row_stride, int64_t lin_stride, int flags,
+                     const float* bias, int64_t B, int S, int D, int64_t ld, float* out, void* stream);
+int dr_fnn_input_bwd(const void* ids, int id_bytes, const int64_t* rows, const float* g_x, int64_t B, int S, int D,
+                     int64_t ld, int64_t row_stride, int64_t lin_stride, int flags, float* const* grad_table_ptrs,
+                     float* const* grad_lin_ptrs, float scale, void* stream);
+
 /* ---- 8(f) #4  input format: TFRecord file of serialized tf.train.Example (datasets/movielens.py:54-62 writer
  * schema, :116-125 tf.io.parse_example reader).  HOST entry points (no GPU needed), the native replacement of
  * tf.data.TFRecordDataset + tf.io.parse_example for this path; their outputs are exactly what the id pipeline above
