@@ -23,7 +23,7 @@ import torch
 
 from . import _lib, ops
 from ._lib import check
-from .training import _WholeStepDriver
+from .training import _WholeStepDriver, flat_params
 
 HEAD_MAX_WIDTH = 4096      # dr_dcn_head_bce_fwd_bwd serves d + n up to this
 
@@ -70,21 +70,7 @@ class DCNTrainStep(_WholeStepDriver):
             params += [c.kernel, c.kernel_u, c.kernel_v, c.bias]
         for l in self.layers + [model.head]:
             params += [l.kernel, l.bias]
-        r4 = lambda n: (n + 3) // 4 * 4      # every parameter starts on a 16-byte boundary
-        total = sum(r4(p.numel()) for p in params if p is not None)
-        self.flat = torch.empty(total, device=dev, dtype=torch.float32)
-        self.gflat = torch.zeros(total, device=dev, dtype=torch.float32)
-        views, o = [], 0
-        with torch.no_grad():
-            for p in params:
-                if p is None:
-                    views.append((None, None))
-                    continue
-                n = p.numel()
-                self.flat[o:o + n].copy_(p.reshape(-1))
-                p.data = self.flat[o:o + n].view_as(p)            # parameters alias the flat buffer
-                views.append((p.data, self.gflat[o:o + n].view_as(p)))
-                o += r4(n)
+        self.flat, self.gflat, views = flat_params(params, dev)
         L, nl = len(self.cross), len(self.layers)
         self.cw = views[:4 * L]                                   # per Cross layer: kernel, kernel_u, kernel_v, bias
         self.w = [views[4 * L + 2 * i] for i in range(nl)]        # (parameter, gradient) pairs

@@ -26,6 +26,7 @@ import torch.distributed as dist
 from . import _lib, ops, shard_plan
 from ._lib import check
 from .keras.layers.base import Dense
+from .training import _DeepFMTower
 
 
 class ShardedEmbedding:
@@ -82,7 +83,7 @@ class ShardedEmbedding:
         return self.weight[:, self.dim] if self.lin_in_row else self.lin
 
 
-class ShardedDeepFMTrainStep:
+class ShardedDeepFMTrainStep(_DeepFMTower):
     def __init__(self, columns, dim: int, dnn_units: Sequence[int], batch_size: int, lr: float = 0.01,
                  seed: int = 0, device=None, group=None, use_graph: bool = True, exchange: str = "p2p",
                  dw_first: bool = False):
@@ -115,24 +116,7 @@ class ShardedDeepFMTrainStep:
         for l in layers:
             l.build((B, in_dim), device=dev)
             in_dim = l.units
-        self.layers = layers
-        # every parameter starts on a 16-byte boundary (the tensor-core path splits operands with float4)
-        r4 = lambda n: (n + 3) // 4 * 4
-        total = 4 + sum(r4(l.kernel.numel()) + r4(l.bias.numel()) for l in layers)
-        self.flat = torch.zeros(total, **f)
-        self.gflat = torch.zeros(total, **f)
-        self.bias, self.g_bias = self.flat[0:1], self.gflat[0:1]
-        self.w, self.b, self.gw, self.gb = [], [], [], []
-        o = 4
-        with torch.no_grad():
-            for l in layers:
-                for src, dst_p, dst_g in ((l.kernel, self.w, self.gw), (l.bias, self.b, self.gb)):
-                    nel = src.numel()
-                    self.flat[o:o + nel].copy_(src.reshape(-1))
-                    src.data = self.flat[o:o + nel].view_as(src)
-                    dst_p.append(src.data)
-                    dst_g.append(self.gflat[o:o + nel].view_as(src))
-                    o += r4(nel)
+        [(self.bias, self.g_bias)] = self._init_tower(layers, lead=[torch.zeros((1,), **f)])     # bias at 0, tower at 4
         # static buffers
         # warm-up ids spread over the tables (all-zero ids would all hit one owner)
         self.ids = torch.stack([torch.randint(0, max(1, r), (B,), device=dev) for r in rows], dim=1).contiguous()
@@ -147,15 +131,6 @@ class ShardedDeepFMTrainStep:
             self.vec_recv = torch.empty((G * self.cap, V), **f)      # rows this rank asked for
             self.grad_send = torch.empty((G * self.cap, V), **f)
             self.grad_recv = torch.empty((G * self.cap, V), **f)
-        self.stack = torch.empty((B, S, D), **f)
-        self.sum_e = torch.empty((B, D), **f)
-        self.fm_logit = torch.empty((B,), **f)
-        self.acts = [torch.empty((B, l.units), **f) for l in layers]
-        self.g_acts = [torch.empty((B, l.units), **f) for l in layers]
-        self.gz_ws = [torch.empty((B, l.units), **f) if l._act != 0 else None for l in layers]
-        self.g_stack = torch.empty((B, S, D), **f)
-        self.loss = torch.zeros((1,), **f)
-        self.prob = torch.empty((B,), **f)
         if exchange == "nccl":
             # "identity tables": the S slots all read the receive buffer (table base = vec_recv, rows = G*cap)
             base = self.vec_recv.data_ptr()
@@ -165,14 +140,8 @@ class ShardedDeepFMTrainStep:
             self.gtp = torch.full((S,), gbase, device=dev, dtype=torch.int64)
             self.glp = torch.full((S,), gbase + D * 4, device=dev, dtype=torch.int64)
             self.trows = torch.full((S,), G * self.cap, device=dev, dtype=torch.int64)
-        kmax = max([S * D] + [l.units for l in layers])
-        _lib.ensure_gemm_workspace(B, kmax, kmax, dev)
-        widths = [S * D] + [l.units for l in layers]
-        cache_bytes = 8 * (B * (widths[0] + 2 * sum(widths[1:])) + sum(a * b for a, b in zip(widths[:-1], widths[1:])))
-        _lib.set_workspace(max(cache_bytes * 5 // 4 + (1 << 20), _lib._workspace.numel() if _lib._workspace is not None else 0), dev)
         self.graph = None
         self.use_graph = use_graph
-        self.graph_error = None
         self.launches_per_step = None
         self._copy_stream = torch.cuda.Stream(device=dev)
         self._side_stream = torch.cuda.Stream(device=dev)
@@ -252,51 +221,7 @@ class ShardedDeepFMTrainStep:
 
         def seg_tower():
             check(lib.dr_gemm_plane_cache(1), "dr_gemm_plane_cache")
-            x, K = self.stack, S * D
-            L = len(self.layers)
-            gz = self.g_acts[-1]
-            head = (L >= 2 and self.layers[-1].units == 1 and self.layers[-1]._act == 0 and self.layers[-2].units <= 256)
-            for i, l in enumerate(self.layers[:L - 1] if head else self.layers):
-                check(lib.dr_dense_fwd(x.data_ptr(), self.w[i].data_ptr(), self.b[i].data_ptr(), B, K, l.units,
-                                       l._act, self.acts[i].data_ptr(), st()), "dr_dense_fwd")
-                x, K = self.acts[i], l.units
-                mark(f"dense_fwd_{i}")
-            if head:      # final Dense(1) + BCE + their backward: one kernel (see DeepFMTrainStep._enqueue)
-                check(lib.dr_dense_head_bce_fwd_bwd(self.acts[L - 2].data_ptr(), self.w[L - 1].data_ptr(),
-                                                    self.b[L - 1].data_ptr(), self.fm_logit.data_ptr(),
-                                                    self.labels.data_ptr(), B, self.layers[L - 2].units,
-                                                    self.layers[L - 2]._act, self.acts[L - 1].data_ptr(),
-                                                    self.prob.data_ptr(), self.loss.data_ptr(), gz.data_ptr(),
-                                                    self.g_acts[L - 2].data_ptr(), self.gw[L - 1].data_ptr(),
-                                                    self.gb[L - 1].data_ptr(), self.gb[L - 2].data_ptr(), st()),
-                      "dr_dense_head_bce_fwd_bwd")
-                mark("head_bce")
-            else:
-                check(lib.dr_bce_logits_fwd_bwd(self.acts[-1].data_ptr(), self.fm_logit.data_ptr(),
-                                                self.labels.data_ptr(), B, self.prob.data_ptr(), self.loss.data_ptr(),
-                                                gz.data_ptr(), st()), "dr_bce")
-                mark("bce")
-            first = L - 2 if head else L - 1
-            for i in range(first, 0, -1):      # chained backward (dr_dense_bwd_chain): see DeepFMTrainStep._enqueue
-                l = self.layers[i]
-                top = i == L - 1
-                have_gb = head and i == L - 2
-                xin, Kin, gx = self.acts[i - 1], self.layers[i - 1].units, self.g_acts[i - 1]
-                check(lib.dr_dense_bwd_chain(xin.data_ptr(), self.w[i].data_ptr(),
-                                             self.acts[i].data_ptr() if top else None, self.g_acts[i].data_ptr(), B, Kin,
-                                             l.units, l._act if top else 0, ops._ptr(self.gz_ws[i]) if top else None,
-                                             gx.data_ptr(), self.gw[i].data_ptr(),
-                                             None if have_gb else self.gb[i].data_ptr(), xin.data_ptr(),
-                                             self.layers[i - 1]._act, st()), "dr_dense_bwd_chain")
-                mark(f"dense_bwd_{i}")
-            l = self.layers[0]      # layer 0: the input gradient first (the embedding update needs it) ...
-            top0 = L == 1
-            gb0 = None if (head and L == 2) else self.gb[0].data_ptr()
-            check(lib.dr_dense_bwd(self.stack.data_ptr(), self.w[0].data_ptr(), self.acts[0].data_ptr() if top0 else None,
-                                   self.g_acts[0].data_ptr(), B, S * D, l.units, l._act if top0 else 0,
-                                   ops._ptr(self.gz_ws[0]) if top0 else None,
-                                   self.g_stack.data_ptr(), None, gb0, st()), "dr_dense_bwd(dx)")
-            mark("dense_bwd_0_dx")
+            self._tower_fwd_bwd(mark)
 
         def seg_update():           # replayed on the SIDE stream: remote vector atomics into the owners' shards
             gz = self.g_acts[-1]
@@ -307,10 +232,7 @@ class ShardedDeepFMTrainStep:
                   "dr_embed_fm_bwd_sharded")
 
         def seg_dw():               # ... meanwhile, on the main stream: layer-0 weight gradient + FM bias gradient
-            l = self.layers[0]
-            gz0 = (self.gz_ws[0] if l._act != 0 else self.g_acts[0]) if len(self.layers) == 1 else self.g_acts[0]
-            check(lib.dr_dense_bwd(self.stack.data_ptr(), self.w[0].data_ptr(), None, gz0.data_ptr(), B, S * D, l.units,
-                                   0, None, None, self.gw[0].data_ptr(), None, st()), "dr_dense_bwd(dw)")
+            self._tower_dw()
             check(lib.dr_gemm_plane_cache(0), "dr_gemm_plane_cache")
             mark("dense_bwd_0_dw")
             torch.sum(self.g_acts[-1].view(-1), dim=0, keepdim=True, out=self.g_bias)      # FM bias gradient (tiny)
@@ -461,49 +383,34 @@ class ShardedDeepFMTrainStep:
         the flat tower)."""
         return [self.emb._buf if self.exchange == "p2p" else self.emb.weight, self.flat]
 
-    def capture(self):
-        """Warm up eagerly, then record the compute segments into CUDA graphs (collectives stay eager NCCL calls:
-        capturing the NCCL all-to-all itself dead-locked on this torch/NCCL build).
+    def _barrier(self):
+        """`capture` restores the shards after a warm-up step that sent remote atomics into every peer's shard: all ranks
+        meet before the restore (every update has landed) and after it (nobody starts a real step before every shard is
+        restored)."""
+        dist.barrier(group=self.group)
 
-        Side-effect free: the warm-up is a real step on the static warm-up ids (with remote atomics into the peers'
-        shards), so every rank snapshots its shard and the tower first and restores them once ALL ranks have finished
-        the warm-up (barrier on both sides of the restore)."""
-        n0 = _lib.launch_count()
-        with torch.no_grad():
-            state = self._persistent_state()
-            saved = [t.clone() for t in state]
-            s = torch.cuda.Stream(device=self.dev)
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                self._enqueue()
-            torch.cuda.current_stream().wait_stream(s)
-            torch.cuda.synchronize()
-            dist.barrier(group=self.group)          # every peer's remote updates of the warm-up step have landed
-            for t, keep in zip(state, saved):
-                t.copy_(keep)
-            del saved
-            torch.cuda.synchronize()
-            dist.barrier(group=self.group)          # nobody starts a real step before every shard is restored
-        self.launches_per_step = _lib.launch_count() - n0
-        self.check_overflow()
-        if self.use_graph:
-            plan = []
-            for fn, kind in self._segments(lambda label: None):
-                if kind in ("graph", "graph_side", "graph_side_fork"):
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        fn()
-                    plan.append((g.replay, kind))
-                else:
-                    plan.append((fn, kind))
-            self.graph = plan
-        return self
+    def _record_graph(self):
+        """Record the compute segments into CUDA graphs; the collectives stay eager NCCL calls (capturing the NCCL
+        all-to-all itself dead-locked on this torch/NCCL build).  Returns the plan `_replay` runs."""
+        plan = []
+        for fn, kind in self._segments(lambda label: None):
+            if kind in ("graph", "graph_side", "graph_side_fork"):
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    fn()
+                plan.append((g.replay, kind))
+            else:
+                plan.append((fn, kind))
+        return plan
+
+    def _replay(self):
+        self._run_plan(self.graph)
 
     def check_overflow(self):
         """exchange='nccl' only: raise if ANY bucket call since the last check ran out of send slots (the flag is
-        sticky on the device; it is cleared here after it has been read).  Called by capture() and by
-        train_step_host() (which synchronises on the loss anyway); callers of the asynchronous step() / run() call it
-        whenever they synchronise."""
+        sticky on the device; it is cleared here after it has been read).  Called by capture(), train_step_host() (which
+        synchronises on the loss anyway) and once at the end of fit_host(); callers of the asynchronous step() / run()
+        call it whenever they synchronise."""
         if self.exchange == "p2p":
             return
         if int(self.overflow.item()) != 0:
@@ -512,104 +419,18 @@ class ShardedDeepFMTrainStep:
                                     "(low-cardinality or skewed slot): lookups were dropped in a step since the last "
                                     "check; rebuild the trainer with a larger shard_plan.capacity slack")
 
-    def run(self):
-        if self.graph is not None:
-            self._run_plan(self.graph)
-        else:
-            self._enqueue()
-
-    def step(self, ids, labels):
-        self.ids.copy_(ids, non_blocking=True)
-        self.labels.copy_(labels.reshape(-1), non_blocking=True)
-        self.run()
-        return self.loss
-
-    def stage_host(self, ids_host, labels_host):
-        if not hasattr(self, "_spare"):
-            self._spare = (torch.empty_like(self.ids), torch.empty_like(self.labels))
-        with torch.cuda.stream(self._copy_stream):
-            self._spare[0].copy_(ids_host, non_blocking=True)
-            self._spare[1].copy_(labels_host.reshape(-1), non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record()
-        self._staged = ev
-
-    def train_step_host(self, ids_host, labels_host, next_ids_host=None, next_labels_host=None) -> float:
-        cur = torch.cuda.current_stream()
-        if self._staged is None:
-            self.stage_host(ids_host, labels_host)
-        cur.wait_event(self._staged)
-        self.ids.copy_(self._spare[0], non_blocking=True)
-        self.labels.copy_(self._spare[1], non_blocking=True)
-        done = torch.cuda.Event()
-        done.record(cur)
-        self._staged = None
-        if next_ids_host is not None:
-            self._copy_stream.wait_event(done)
-            self.stage_host(next_ids_host, next_labels_host)
-        self.run()
-        loss = float(self.loss.item())
-        self.check_overflow()
-        return loss
-
-    def fit_host(self, batches, depth: int = 2):
-        """Pipelined epoch loop over HOST batches (training.fit_host): H2D of the next batch and the D2H read of every
-        step's loss stay off the critical path; the overflow flag of the NCCL exchange is checked once at the end."""
-        from .training import fit_host
-        losses = fit_host(self, batches, depth)
-        self.check_overflow()
-        return losses
-
-    def time_embed_fwd(self, ids_pool, iters: int = 30) -> float:
-        """Mean duration (ms) of this rank's fused gather+FM forward alone (p2p: (G-1)/G of the rows are
-        read from peers over NVLink inside the same kernel).  nccl exchange: times the local
-        identity-table kernel only."""
-        lib, st = self.lib, torch.cuda.current_stream().cuda_stream
+    def _launch_embed_fwd(self, ids, st):
+        """time_embed_fwd's kernel: this rank's fused gather+FM forward (p2p: (G-1)/G of the rows are read from peers
+        over NVLink inside the same kernel).  nccl exchange: the local identity-table kernel only (`ids` unused)."""
         B, S, D, G, V = self.B, self.S, self.D, self.world, self.emb.vdim
-
-        def launch(k):
-            if self.exchange == "p2p":
-                ids = ids_pool[k % len(ids_pool)]
-                check(lib.dr_embed_fm_fwd_sharded(self.emb.peer_ptrs.data_ptr(), G, self.emb.slot_offsets.data_ptr(),
-                                                  self.emb.rows.data_ptr(), ids.data_ptr(), 8, self.bias.data_ptr(),
-                                                  B, S, D, V, self.emb.flags, self.emb.lin_offset,
-                                                  self.stack.data_ptr(), self.sum_e.data_ptr(),
-                                                  self.fm_logit.data_ptr(), st), "dr_embed_fm_fwd_sharded")
-            else:
-                check(lib.dr_embed_fm_fwd(self.tp.data_ptr(), self.lp.data_ptr(), self.trows.data_ptr(),
-                                          self.inv.data_ptr(), 4, self.bias.data_ptr(), B, S, D, V, V, 1,
-                                          self.stack.data_ptr(), self.sum_e.data_ptr(), self.fm_logit.data_ptr(), st),
-                      "dr_embed_fm_fwd")
-
-        for k in range(5):
-            launch(k)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for k in range(iters):
-            launch(k)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
-
-    def profile_kernels(self, ids_pool, labels_pool, iters: int = 10):
-        runs = []
-        for it in range(iters + 2):      # back-to-back, no host sync in between (steady-state clocks / caches)
-            self.ids.copy_(ids_pool[it % len(ids_pool)], non_blocking=True)
-            self.labels.copy_(labels_pool[it % len(labels_pool)].reshape(-1), non_blocking=True)
-            evs = []
-
-            def mark(label, evs=evs):
-                e = torch.cuda.Event(enable_timing=True)
-                e.record()
-                evs.append((label, e))
-
-            self._enqueue(mark)
-            runs.append(evs)
-        torch.cuda.synchronize()
-        sums, count = {}, 0
-        for evs in runs[2:]:
-            count += 1
-            for (l0, e0), (l1, e1) in zip(evs[:-1], evs[1:]):
-                sums[l1] = sums.get(l1, 0.0) + e0.elapsed_time(e1)
-        shares = {k: v / count for k, v in sums.items()}
-        return {"embed_fm_fwd_ms": shares.get("embed_fm_fwd", shares.get("embed_fm_fwd_p2p"))}, shares
+        if self.exchange == "p2p":
+            check(self.lib.dr_embed_fm_fwd_sharded(self.emb.peer_ptrs.data_ptr(), G, self.emb.slot_offsets.data_ptr(),
+                                                   self.emb.rows.data_ptr(), ids.data_ptr(), 8, self.bias.data_ptr(),
+                                                   B, S, D, V, self.emb.flags, self.emb.lin_offset,
+                                                   self.stack.data_ptr(), self.sum_e.data_ptr(),
+                                                   self.fm_logit.data_ptr(), st), "dr_embed_fm_fwd_sharded")
+        else:
+            check(self.lib.dr_embed_fm_fwd(self.tp.data_ptr(), self.lp.data_ptr(), self.trows.data_ptr(),
+                                           self.inv.data_ptr(), 4, self.bias.data_ptr(), B, S, D, V, V, 1,
+                                           self.stack.data_ptr(), self.sum_e.data_ptr(), self.fm_logit.data_ptr(), st),
+                  "dr_embed_fm_fwd")

@@ -33,56 +33,51 @@ from . import _lib, ops
 from ._lib import check
 
 
-def fit_host(trainer, batches, depth: int = 2) -> List[float]:
-    """Pipelined end-to-end loop shared by DeepFMTrainStep and ShardedDeepFMTrainStep (`trainer.fit_host(batches)`).
-
-    `batches`: sequence of (ids_host, labels_host) HOST tensors (pinned for asynchronous copies).  Per step, inside this
-    call: the H2D copy of the batch (copy stream, overlapping the previous step's kernels), the D2D swap into the static
-    buffers the CUDA graph reads, the step, and an asynchronous D2H copy of the step's loss into a pinned ring.  The host
-    reads the loss of step k - depth while step k is being enqueued, i.e. it never idles the GPU waiting for a scalar
-    (train_step_host blocks on `loss.item()` every step); returns every step's loss, in order."""
-    batches = list(batches)
-    if not batches:
-        return []
-    cur = torch.cuda.current_stream()
-    ring = getattr(trainer, "_loss_ring", None)
-    if ring is None or ring.numel() < depth + 1:
-        ring = trainer._loss_ring = torch.empty((depth + 1,), dtype=torch.float32).pin_memory()
-    events: List[Optional[torch.cuda.Event]] = [None] * (depth + 1)
-    losses: List[float] = []
-    trainer._copy_stream.wait_stream(cur)        # whatever still reads the spare buffers has been enqueued on `cur`
-    trainer.stage_host(*batches[0])
-    for k, _ in enumerate(batches):
-        cur.wait_event(trainer._staged)
-        trainer.ids.copy_(trainer._spare[0], non_blocking=True)          # D2D swap into the graph's static buffers
-        trainer.labels.copy_(trainer._spare[1], non_blocking=True)
-        done = torch.cuda.Event()
-        done.record(cur)
-        trainer._staged = None
-        if k + 1 < len(batches):
-            trainer._copy_stream.wait_event(done)                        # the spare buffers are free again
-            trainer.stage_host(*batches[k + 1])
-        trainer.run()
-        slot = k % (depth + 1)
-        if events[slot] is not None:                                     # the loss that lived in this slot: step k-depth-1
-            events[slot].synchronize()
-            losses.append(float(ring[slot]))
-        ring[slot:slot + 1].copy_(trainer.loss.reshape(-1)[:1], non_blocking=True)      # D2H read of this step's result
-        ev = torch.cuda.Event()
-        ev.record(cur)
-        events[slot] = ev
-    n = len(batches)
-    for k in range(max(0, n - (depth + 1)), n):                          # drain, in step order
-        slot = k % (depth + 1)
-        events[slot].synchronize()
-        losses.append(float(ring[slot]))
-    return losses
+def flat_params(params, device):
+    """Move `params` (entries may be None) into ONE zero-filled flat buffer, every parameter starting on a 16-byte boundary
+    (the tensor-core path splits operands with float4), and rebind each `param.data` to its view, so the model keeps
+    working on the weights the trainer updates.  Returns (flat, gflat, [(param view, gradient view) or (None, None)])."""
+    r4 = lambda n: (n + 3) // 4 * 4
+    total = sum(r4(p.numel()) for p in params if p is not None)
+    flat = torch.zeros(total, device=device, dtype=torch.float32)
+    gflat = torch.zeros(total, device=device, dtype=torch.float32)
+    views, o = [], 0
+    with torch.no_grad():
+        for p in params:
+            if p is None:
+                views.append((None, None))
+                continue
+            n = p.numel()
+            flat[o:o + n].copy_(p.reshape(-1))
+            p.data = flat[o:o + n].view_as(p)
+            views.append((p.data, gflat[o:o + n].view_as(p)))
+            o += r4(n)
+    return flat, gflat, views
 
 
 class _WholeStepDriver:
     """What every whole-step trainer shares once it has `_enqueue(mark)` (the step as raw C-ABI calls on the current
     stream), `_persistent_state()`, the static `ids` / `labels` buffers, `loss`, `dev`, `use_graph`, `_copy_stream` and
-    `_staged`: CUDA-graph capture and replay, the host-batch pipeline and the per-kernel-group profile."""
+    `_staged`: CUDA-graph capture and replay, the host-batch pipeline and the per-kernel-group profile.
+
+    A multi-process trainer overrides `_barrier` (all ranks meet), `check_overflow` (raise on a sticky device-side error
+    flag) and `_record_graph` / `_replay` (a step that is not one graph)."""
+
+    def _barrier(self):
+        """Called on both sides of the warm-up restore in `capture`; a no-op for a single process."""
+
+    def check_overflow(self):
+        """Raise if a step since the last check hit a device-side capacity limit; a no-op unless a trainer has one."""
+
+    def _record_graph(self):
+        """Record one step; `run` hands what this returns to `_replay`."""
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self._enqueue()
+        return g
+
+    def _replay(self):
+        self.graph.replay()
 
     def profile_kernels(self, ids_pool, labels_pool, iters: int = 10):
         """Eager (non-graph) passes with a CUDA event on the launching stream between kernel groups.
@@ -108,7 +103,7 @@ class _WholeStepDriver:
             for (l0, e0), (l1, e1) in zip(evs[:-1], evs[1:]):
                 sums[l1] = sums.get(l1, 0.0) + e0.elapsed_time(e1)
         shares = {k: v / count for k, v in sums.items()}
-        return {"embed_fm_fwd_ms": shares["embed_fm_fwd"]}, shares
+        return {"embed_fm_fwd_ms": shares.get("embed_fm_fwd", shares.get("embed_fm_fwd_p2p"))}, shares
 
     def capture(self):
         """Warm up (sets kernel attributes) then record the step into a CUDA graph.
@@ -126,22 +121,22 @@ class _WholeStepDriver:
                 self._enqueue()
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
+            self._barrier()          # every peer's remote updates of the warm-up step have landed
             for t, keep in zip(state, saved):
                 t.copy_(keep)
             del saved
-        torch.cuda.synchronize()
+            torch.cuda.synchronize()
+            self._barrier()          # nobody starts a real step before every peer has restored its state
         self.launches_per_step = _lib.launch_count() - n0
+        self.check_overflow()
         if self.use_graph:
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._enqueue()
-            self.graph = g
+            self.graph = self._record_graph()
         return self
 
     def run(self):
         """One step on whatever is in self.ids / self.labels (device resident)."""
         if self.graph is not None:
-            self.graph.replay()
+            self._replay()
         else:
             self._enqueue()
 
@@ -181,14 +176,174 @@ class _WholeStepDriver:
             self._copy_stream.wait_event(done)
             self.stage_host(next_ids_host, next_labels_host)
         self.run()
-        return float(self.loss.item())          # D2H read of the step's result (synchronises)
+        loss = float(self.loss.item())          # D2H read of the step's result (synchronises)
+        self.check_overflow()
+        return loss
 
     def fit_host(self, batches, depth: int = 2) -> List[float]:
-        """Pipelined epoch loop over HOST batches (see module-level fit_host): the public end-to-end call."""
-        return fit_host(self, batches, depth)
+        """Pipelined epoch loop over HOST batches: the public end-to-end call.
+
+        `batches`: sequence of (ids_host, labels_host) HOST tensors (pinned for asynchronous copies).  Per step, inside
+        this call: the H2D copy of the batch (copy stream, overlapping the previous step's kernels), the D2D swap into the
+        static buffers the CUDA graph reads, the step, and an asynchronous D2H copy of the step's loss into a pinned ring.
+        The host reads the loss of step k - depth while step k is being enqueued, i.e. it never idles the GPU waiting for
+        a scalar (train_step_host blocks on `loss.item()` every step); returns every step's loss, in order.
+        `check_overflow` runs once at the end."""
+        batches = list(batches)
+        if not batches:
+            self.check_overflow()
+            return []
+        cur = torch.cuda.current_stream()
+        ring = getattr(self, "_loss_ring", None)
+        if ring is None or ring.numel() < depth + 1:
+            ring = self._loss_ring = torch.empty((depth + 1,), dtype=torch.float32).pin_memory()
+        events: List[Optional[torch.cuda.Event]] = [None] * (depth + 1)
+        losses: List[float] = []
+        self._copy_stream.wait_stream(cur)          # whatever still reads the spare buffers has been enqueued on `cur`
+        self.stage_host(*batches[0])
+        for k, _ in enumerate(batches):
+            cur.wait_event(self._staged)
+            self.ids.copy_(self._spare[0], non_blocking=True)            # D2D swap into the graph's static buffers
+            self.labels.copy_(self._spare[1], non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(cur)
+            self._staged = None
+            if k + 1 < len(batches):
+                self._copy_stream.wait_event(done)                       # the spare buffers are free again
+                self.stage_host(*batches[k + 1])
+            self.run()
+            slot = k % (depth + 1)
+            if events[slot] is not None:                                 # the loss that lived in this slot: step k-depth-1
+                events[slot].synchronize()
+                losses.append(float(ring[slot]))
+            ring[slot:slot + 1].copy_(self.loss.reshape(-1)[:1], non_blocking=True)     # D2H read of this step's result
+            ev = torch.cuda.Event()
+            ev.record(cur)
+            events[slot] = ev
+        n = len(batches)
+        for k in range(max(0, n - (depth + 1)), n):                      # drain, in step order
+            slot = k % (depth + 1)
+            events[slot].synchronize()
+            losses.append(float(ring[slot]))
+        self.check_overflow()
+        return losses
 
 
-class DeepFMTrainStep(_WholeStepDriver):
+class _DeepFMTower(_WholeStepDriver):
+    """The DeepFM tower as both DeepFM trainers run it: from the stacked embeddings `stack` [B, S*D] and `fm_logit` to
+    the BCE loss, the tower gradients in `gflat` and the input gradient `g_stack` the embedding update reads.  The
+    trainer owns the gather, the embedding update, the optimizers, the streams and `dr_gemm_plane_cache`."""
+
+    def _init_tower(self, layers, lead=()):
+        """Move `lead` and every Dense parameter of `layers` (built) into `flat`, allocate the tower's buffers and size
+        the GEMM workspace for them.  Returns the (parameter, gradient) views of `lead`."""
+        self.layers = layers
+        B, S, D, dev = self.B, self.S, self.D, self.dev
+        lead = list(lead)
+        self.flat, self.gflat, views = flat_params(lead + [p for l in layers for p in (l.kernel, l.bias)], dev)
+        tower = views[len(lead):]
+        self.w, self.gw = [p for p, _ in tower[0::2]], [g for _, g in tower[0::2]]
+        self.b, self.gb = [p for p, _ in tower[1::2]], [g for _, g in tower[1::2]]
+        f = dict(device=dev, dtype=torch.float32)
+        self.stack = torch.empty((B, S, D), **f)
+        self.sum_e = torch.empty((B, D), **f)
+        self.fm_logit = torch.empty((B,), **f)
+        self.acts = [torch.empty((B, l.units), **f) for l in layers]
+        self.g_acts = [torch.empty((B, l.units), **f) for l in layers]       # dL/d(output of layer i)
+        self.gz_ws = [torch.empty((B, l.units), **f) if l._act != 0 else None for l in layers]
+        self.g_stack = torch.empty((B, S, D), **f)
+        self.loss = torch.zeros((1,), **f)
+        self.prob = torch.empty((B,), **f)
+        # the skinny end (final Dense(1) + BCE + their backward) is ONE kernel when the layer below is <= 256 wide
+        L = len(layers)
+        self._fused_head = (L >= 2 and layers[-1].units == 1 and layers[-1]._act == 0 and layers[-2].units <= 256
+                            and self.b[-1] is not None and self.b[-2] is not None)
+        widths = [S * D] + [l.units for l in layers]
+        _lib.ensure_gemm_workspace(B, max(widths), max(widths), dev)
+        # plane cache: x, every activation, every upstream gradient and every kernel, hi + lo
+        cache_bytes = 8 * (B * (widths[0] + 2 * sum(widths[1:])) + sum(a * b for a, b in zip(widths[:-1], widths[1:])))
+        _lib.set_workspace(max(cache_bytes * 5 // 4 + (1 << 20), _lib._workspace.numel() if _lib._workspace is not None else 0), dev)
+        return views[:len(lead)]
+
+    def _tower_fwd_bwd(self, mark, first: int = 0):
+        """Dense forwards from layer `first` (the layers below it have run already), the loss head, the chained backward
+        and the layer-0 input gradient into `g_stack`, on the current stream."""
+        lib, st = self.lib, torch.cuda.current_stream().cuda_stream
+        B, S, D = self.B, self.S, self.D
+        L = len(self.layers)
+        head = self._fused_head
+        gz = self.g_acts[-1]                                   # [B,1]: dL/dlogit
+        x, K = (self.stack, S * D) if first == 0 else (self.acts[first - 1], self.layers[first - 1].units)
+        for i in range(first, L - 1 if head else L):
+            l = self.layers[i]
+            check(lib.dr_dense_fwd(x.data_ptr(), self.w[i].data_ptr(), ops._ptr(self.b[i]), B, K, l.units, l._act,
+                                   self.acts[i].data_ptr(), st), "dr_dense_fwd")
+            mark(f"dense_fwd_{i}")
+            x, K = self.acts[i], l.units
+        if head:
+            check(lib.dr_dense_head_bce_fwd_bwd(self.acts[L - 2].data_ptr(), self.w[L - 1].data_ptr(),
+                                                self.b[L - 1].data_ptr(), self.fm_logit.data_ptr(), self.labels.data_ptr(),
+                                                B, self.layers[L - 2].units, self.layers[L - 2]._act,
+                                                self.acts[L - 1].data_ptr(), self.prob.data_ptr(), self.loss.data_ptr(),
+                                                gz.data_ptr(), self.g_acts[L - 2].data_ptr(), self.gw[L - 1].data_ptr(),
+                                                self.gb[L - 1].data_ptr(), self.gb[L - 2].data_ptr(), st),
+                  "dr_dense_head_bce_fwd_bwd")
+            mark("head_bce")
+        else:
+            check(lib.dr_bce_logits_fwd_bwd(self.acts[-1].data_ptr(), self.fm_logit.data_ptr(), self.labels.data_ptr(), B,
+                                            self.prob.data_ptr(), self.loss.data_ptr(), gz.data_ptr(), st), "dr_bce")
+            mark("bce")
+        # Chained backward: layer i's input gradient leaves its GEMM already multiplied by act'(output of layer i-1)
+        # (dr_dense_bwd_chain), so g_acts[i-1] IS the pre-activation gradient of layer i-1 and no layer below the top
+        # needs its own activation-gradient pass (only the column sums for the bias gradient; the layer right below the
+        # fused head got those from the head kernel too).
+        first_bwd = L - 2 if head else L - 1                  # highest layer that still needs its backward here
+        for i in range(first_bwd, 0, -1):
+            l = self.layers[i]
+            top = (i == L - 1)                                # only without the fused head: gy is dL/d(output), not gz
+            have_gb = head and i == L - 2
+            xin, Kin, gx = self.acts[i - 1], self.layers[i - 1].units, self.g_acts[i - 1]
+            check(lib.dr_dense_bwd_chain(xin.data_ptr(), self.w[i].data_ptr(), self.acts[i].data_ptr() if top else None,
+                                         self.g_acts[i].data_ptr(), B, Kin, l.units, l._act if top else 0,
+                                         ops._ptr(self.gz_ws[i]) if top else None, gx.data_ptr(), self.gw[i].data_ptr(),
+                                         None if have_gb else ops._ptr(self.gb[i]), xin.data_ptr(),
+                                         self.layers[i - 1]._act, st),
+                  "dr_dense_bwd_chain")
+            mark(f"dense_bwd_{i}")
+        # layer 0: the input gradient only (the embedding update needs it); its weight gradient is `_tower_dw`
+        l = self.layers[0]
+        top0 = L == 1
+        gb0 = None if (head and L == 2) else ops._ptr(self.gb[0])
+        check(lib.dr_dense_bwd(self.stack.data_ptr(), self.w[0].data_ptr(), self.acts[0].data_ptr() if top0 else None,
+                               self.g_acts[0].data_ptr(), B, S * D, l.units, l._act if top0 else 0,
+                               ops._ptr(self.gz_ws[0]) if top0 else None,
+                               self.g_stack.data_ptr(), None, gb0, st), "dr_dense_bwd(dx)")
+        mark("dense_bwd_0_dx")
+
+    def _tower_dw(self):
+        """The layer-0 weight gradient, on the current stream (after `_tower_fwd_bwd`)."""
+        l = self.layers[0]
+        gz0 = (self.gz_ws[0] if l._act != 0 else self.g_acts[0]) if len(self.layers) == 1 else self.g_acts[0]
+        check(self.lib.dr_dense_bwd(self.stack.data_ptr(), self.w[0].data_ptr(), None, gz0.data_ptr(), self.B,
+                                    self.S * self.D, l.units, 0, None, None, self.gw[0].data_ptr(), None,
+                                    torch.cuda.current_stream().cuda_stream), "dr_dense_bwd(dw)")
+
+    def time_embed_fwd(self, ids_pool, iters: int = 30) -> float:
+        """Mean duration (ms) of the fused gather+FM forward alone: `iters` back-to-back launches on the
+        launching stream between two CUDA events, cycling through the id pool (tables >> L2)."""
+        st = torch.cuda.current_stream().cuda_stream
+        for k in range(5):
+            self._launch_embed_fwd(ids_pool[k % len(ids_pool)], st)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for k in range(iters):
+            self._launch_embed_fwd(ids_pool[k % len(ids_pool)], st)
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+
+class DeepFMTrainStep(_DeepFMTower):
     def __init__(self, model, batch_size: int, lr: float = 0.01, id_dtype=torch.int64, use_graph: bool = True,
                  optimizer: str = "sgd", beta1: float = 0.9, beta2: float = 0.999, eps: float = 1e-7,
                  embed_fwd: str = "ldg", fwd_chunks: int = 1, dw_first: bool = False):
@@ -223,50 +378,11 @@ class DeepFMTrainStep(_WholeStepDriver):
             if not l.built:
                 l.build((self.B, in_dim), device=dev)
             in_dim = l.units
-        self.layers = layers
-        r4 = lambda n: (n + 3) // 4 * 4      # every parameter starts on a 16-byte boundary
-        sizes = []
-        for l in layers:
-            sizes += [r4(l.kernel.numel()), r4(l.bias.numel()) if l.bias is not None else 0]
-        total = sum(sizes)
-        self.flat = torch.empty(total, device=dev, dtype=torch.float32)
-        self.gflat = torch.zeros(total, device=dev, dtype=torch.float32)
-        self.w: List[torch.Tensor] = []
-        self.b: List[Optional[torch.Tensor]] = []
-        self.gw: List[torch.Tensor] = []
-        self.gb: List[Optional[torch.Tensor]] = []
-        o = 0
-        with torch.no_grad():
-            for l in layers:
-                n = l.kernel.numel()
-                self.flat[o:o + n].copy_(l.kernel.reshape(-1))
-                l.kernel.data = self.flat[o:o + n].view_as(l.kernel)     # parameters alias the flat buffer
-                self.w.append(l.kernel.data)
-                self.gw.append(self.gflat[o:o + n].view_as(l.kernel))
-                o += r4(n)
-                if l.bias is not None:
-                    n = l.bias.numel()
-                    self.flat[o:o + n].copy_(l.bias)
-                    l.bias.data = self.flat[o:o + n]
-                    self.b.append(l.bias.data)
-                    self.gb.append(self.gflat[o:o + n])
-                    o += r4(n)
-                else:
-                    self.b.append(None)
-                    self.gb.append(None)
+        self._init_tower(layers)
         B, S, D = self.B, self.S, self.D
         f = dict(device=dev, dtype=torch.float32)
         self.ids = torch.zeros((B, S), device=dev, dtype=id_dtype)
         self.labels = torch.zeros((B,), **f)
-        self.stack = torch.empty((B, S, D), **f)
-        self.sum_e = torch.empty((B, D), **f)
-        self.fm_logit = torch.empty((B,), **f)
-        self.acts = [torch.empty((B, l.units), **f) for l in layers]
-        self.g_acts = [torch.empty((B, l.units), **f) for l in layers]       # dL/d(output of layer i)
-        self.gz_ws = [torch.empty((B, l.units), **f) if l._act != 0 else None for l in layers]
-        self.g_stack = torch.empty((B, S, D), **f)
-        self.loss = torch.zeros((1,), **f)
-        self.prob = torch.empty((B,), **f)
         self.tp, self.lp, self.rows = coll.pointers(coll.weight, coll.linear)
         if optimizer != "sgd":
             # optimizer state: gradient arena (all-zero between steps), m, v in the tables' own layout
@@ -288,12 +404,6 @@ class DeepFMTrainStep(_WholeStepDriver):
                 ss = self.lib.dr_embed_adam_state_stride(D)
                 self.state = torch.zeros((coll.total_rows, ss), **f)
                 self.g_arena = self.m_arena = self.v_arena = self.g_lin = self.m_lin = self.v_lin = None
-        kmax = max([S * D] + [l.units for l in layers])
-        _lib.ensure_gemm_workspace(B, kmax, kmax, dev)
-        # plane cache: x, every activation, every upstream gradient and every kernel, hi + lo
-        widths = [S * D] + [l.units for l in layers]
-        cache_bytes = 8 * (B * (widths[0] + 2 * sum(widths[1:])) + sum(a * b for a, b in zip(widths[:-1], widths[1:])))
-        _lib.set_workspace(max(cache_bytes * 5 // 4 + (1 << 20), _lib._workspace.numel() if _lib._workspace is not None else 0), dev)
         self.graph = None
         self.use_graph = use_graph
         self._copy_stream = torch.cuda.Stream(device=dev)
@@ -331,12 +441,7 @@ class DeepFMTrainStep(_WholeStepDriver):
         else:
             bounds = [(0, B)]
         l0 = self.layers[0]
-        L = len(self.layers)
-        # the skinny end (final Dense(1) + BCE + their backward) is ONE kernel when the layer below is <= 256 wide
-        head = (L >= 2 and self.layers[-1].units == 1 and self.layers[-1]._act == 0 and self.layers[-2].units <= 256
-                and self.b[-1] is not None and self.b[-2] is not None)
-        fwd_layers = list(enumerate(self.layers[:L - 1] if head else self.layers))
-        chunk_l0 = len(bounds) > 1 and len(fwd_layers) >= 1
+        chunk_l0 = len(bounds) > 1
         esz = self.ids.element_size()
         for (b0, b1) in bounds:
             if self.embed_fwd == "tma":      # opt-in: rows staged through TMA (tile::gather4) into shared memory
@@ -362,68 +467,16 @@ class DeepFMTrainStep(_WholeStepDriver):
                 check(lib.dr_embed_adam_count(self.ids.data_ptr(), self.ids.element_size(), B, S, D, self.rows.data_ptr(),
                                               c._offsets.data_ptr(), self.state.data_ptr(), self._side_stream.cuda_stream),
                       "dr_embed_adam_count")
-        x = self.stack
-        K = S * D
-        gz = self.g_acts[-1]                                   # [B,1]: dL/dlogit
-        for i, l in fwd_layers:
-            if not (chunk_l0 and i == 0):
-                check(lib.dr_dense_fwd(x.data_ptr(), self.w[i].data_ptr(), ops._ptr(self.b[i]), B, K, l.units, l._act,
-                                       self.acts[i].data_ptr(), st), "dr_dense_fwd")
-                mark(f"dense_fwd_{i}")
-            x, K = self.acts[i], l.units
-        if head:
-            check(lib.dr_dense_head_bce_fwd_bwd(self.acts[L - 2].data_ptr(), self.w[L - 1].data_ptr(),
-                                                self.b[L - 1].data_ptr(), self.fm_logit.data_ptr(), self.labels.data_ptr(),
-                                                B, self.layers[L - 2].units, self.layers[L - 2]._act,
-                                                self.acts[L - 1].data_ptr(), self.prob.data_ptr(), self.loss.data_ptr(),
-                                                gz.data_ptr(), self.g_acts[L - 2].data_ptr(), self.gw[L - 1].data_ptr(),
-                                                self.gb[L - 1].data_ptr(), self.gb[L - 2].data_ptr(), st),
-                  "dr_dense_head_bce_fwd_bwd")
-            mark("head_bce")
-        else:
-            check(lib.dr_bce_logits_fwd_bwd(self.acts[-1].data_ptr(), self.fm_logit.data_ptr(), self.labels.data_ptr(), B,
-                                            self.prob.data_ptr(), self.loss.data_ptr(), gz.data_ptr(), st), "dr_bce")
-            mark("bce")
-        # Chained backward: layer i's input gradient leaves its GEMM already multiplied by act'(output of layer i-1)
-        # (dr_dense_bwd_chain), so g_acts[i-1] IS the pre-activation gradient of layer i-1 and no layer below the top
-        # needs its own activation-gradient pass (only the column sums for the bias gradient; the layer right below the
-        # fused head got those from the head kernel too).
-        first = L - 2 if head else L - 1                      # highest layer that still needs its backward here
-        for i in range(first, 0, -1):
-            l = self.layers[i]
-            top = (i == L - 1)                                # only without the fused head: gy is dL/d(output), not gz
-            have_gb = head and i == L - 2
-            xin, Kin, gx = self.acts[i - 1], self.layers[i - 1].units, self.g_acts[i - 1]
-            check(lib.dr_dense_bwd_chain(xin.data_ptr(), self.w[i].data_ptr(), self.acts[i].data_ptr() if top else None,
-                                         self.g_acts[i].data_ptr(), B, Kin, l.units, l._act if top else 0,
-                                         ops._ptr(self.gz_ws[i]) if top else None, gx.data_ptr(), self.gw[i].data_ptr(),
-                                         None if have_gb else ops._ptr(self.gb[i]), xin.data_ptr(),
-                                         self.layers[i - 1]._act, st),
-                  "dr_dense_bwd_chain")
-            mark(f"dense_bwd_{i}")
-        # layer 0: input gradient first, then its weight gradient (tensor cores) runs
-        # CONCURRENTLY with the HBM-bound embedding update on a side stream
-        l = self.layers[0]
-        top0 = L == 1
-        gz0 = (self.gz_ws[0] if l._act != 0 else self.g_acts[0]) if top0 else self.g_acts[0]
-        gb0 = None if (head and L == 2) else ops._ptr(self.gb[0])
-        check(lib.dr_dense_bwd(self.stack.data_ptr(), self.w[0].data_ptr(), self.acts[0].data_ptr() if top0 else None,
-                               self.g_acts[0].data_ptr(), B, S * D, l.units, l._act if top0 else 0,
-                               ops._ptr(self.gz_ws[0]) if top0 else None,
-                               self.g_stack.data_ptr(), None, gb0, st), "dr_dense_bwd(dx)")
-        mark("dense_bwd_0_dx")
+        self._tower_fwd_bwd(mark, first=1 if chunk_l0 else 0)
+        # layer 0's weight gradient (tensor cores) runs CONCURRENTLY with the HBM-bound embedding update on a side stream
+        gz = self.g_acts[-1]
         main = torch.cuda.current_stream()
         side = self._side_stream
         adam = self.optimizer != "sgd"
         fork = torch.cuda.Event()
         fork.record(main)                                  # layer-0 input gradient done: both branches may start
-
-        def launch_dw():
-            check(lib.dr_dense_bwd(self.stack.data_ptr(), self.w[0].data_ptr(), None, gz0.data_ptr(), B, S * D, l.units, 0,
-                                   None, None, self.gw[0].data_ptr(), None, st), "dr_dense_bwd(dw)")
-
         if self.dw_first:                                  # the persistent GEMM takes its one CTA per SM first; the update's
-            launch_dw()                                    # CTAs fill what is left of every SM (knob tc_dw_share)
+            self._tower_dw()                               # CTAs fill what is left of every SM (knob tc_dw_share)
         side.wait_event(fork)
         with torch.cuda.stream(side):
             sst = side.cuda_stream
@@ -489,7 +542,7 @@ class DeepFMTrainStep(_WholeStepDriver):
                                        self.v_bias.data_ptr(), 1, 0.0, ck.beta1, ck.beta2, ck.eps, 1, lt, sst),
                       "dr_adam_step(bias)")
         if not self.dw_first:
-            launch_dw()
+            self._tower_dw()
         main.wait_stream(side)
         mark("dense_bwd_0_dw+embed_fm_bwd")
         if not adam:
@@ -502,28 +555,12 @@ class DeepFMTrainStep(_WholeStepDriver):
         check(lib.dr_gemm_plane_cache(0), "dr_gemm_plane_cache")
         mark("sgd")
 
-    def time_embed_fwd(self, ids_pool, iters: int = 30) -> float:
-        """Mean duration (ms) of the fused gather+FM forward alone: `iters` back-to-back launches on the
-        launching stream between two CUDA events, cycling through the id pool (tables >> L2)."""
-        lib, st, c = self.lib, torch.cuda.current_stream().cuda_stream, self.coll
-        B, S, D = self.B, self.S, self.D
-
-        def launch(k):
-            ids = ids_pool[k % len(ids_pool)]
-            check(lib.dr_embed_fm_fwd(self.tp.data_ptr(), self.lp.data_ptr(), self.rows.data_ptr(), ids.data_ptr(),
-                                      ids.element_size(), c.bias.data_ptr(), B, S, D, c.row_stride, c.lin_stride,
-                                      c.flags, self.stack.data_ptr(), self.sum_e.data_ptr(),
-                                      self.fm_logit.data_ptr(), st), "dr_embed_fm_fwd")
-
-        for k in range(5):
-            launch(k)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for k in range(iters):
-            launch(k)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
+    def _launch_embed_fwd(self, ids, st):
+        c = self.coll
+        check(self.lib.dr_embed_fm_fwd(self.tp.data_ptr(), self.lp.data_ptr(), self.rows.data_ptr(), ids.data_ptr(),
+                                       ids.element_size(), c.bias.data_ptr(), self.B, self.S, self.D, c.row_stride,
+                                       c.lin_stride, c.flags, self.stack.data_ptr(), self.sum_e.data_ptr(),
+                                       self.fm_logit.data_ptr(), st), "dr_embed_fm_fwd")
 
     def _persistent_state(self) -> List[torch.Tensor]:
         """Every tensor a step mutates AND a later step reads: parameters and optimizer state."""
