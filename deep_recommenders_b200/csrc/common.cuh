@@ -16,6 +16,9 @@ namespace dr {
 // split-K heuristic.  Queried once per process (api.cu).
 int num_sms();
 
+// Largest world the row-sharded entries address (peer-base tables of this many pointers live in shared memory).
+constexpr int kMaxShardWorld = 64;
+
 // ---- error plumbing -------------------------------------------------------------------
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);

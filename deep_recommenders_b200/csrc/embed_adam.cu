@@ -380,6 +380,155 @@ static int lpr_of(int D) {
   return lpr;
 }
 
+// ---- the same tf.keras-equal Adam on a row-sharded table (owner(r) = r mod G, local row r div G) ----------------------
+// Every cross-rank access is a plain store (mark) or a vector red.add (the backward into the owners' gradient arenas),
+// and nothing reads it before the ranks meet at a barrier; all Adam arithmetic runs on the owner, in its own memory:
+//   mark    : touch[owner][local] = t for every valid lookup (idempotent stores: races between ranks are harmless)
+//   prepare : the owner collects its rows with touch == t into `list` / `count` and replays their pending steps (stamp,
+//             t-1] (as embed_adam_prepare_kernel), so the forward reads what dense Adam would have left there
+//   apply   : after the backward, step t on every listed row from its gradient row (then zeroed); stamp = t.
+// The gradient arena and the shard share one layout (row stride, first-order weight in the row or trailing at
+// lin_offset); the state blocks are those of dr_embed_adam_state_stride, so dr_embed_adam_flush runs on them unchanged.
+template <typename IdT>
+__global__ void __launch_bounds__(256) shard_adam_mark_kernel(const IdT* __restrict__ ids, int64_t n, int S,
+                                                               const int64_t* __restrict__ slot_offsets,
+                                                               const int64_t* __restrict__ rows, int W,
+                                                               int32_t* const* __restrict__ touch_bases,
+                                                               const int64_t* __restrict__ step_dev) {
+  const int32_t t = (int32_t)*step_dev;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int s = (int)(i % S);
+    const int64_t id = (int64_t)__ldg(ids + i);
+    if ((uint64_t)id >= (uint64_t)__ldg(rows + s)) continue;     // -1 padding, out-of-vocabulary ids
+    const int64_t r = __ldg(slot_offsets + s) + id;
+    touch_bases[r % W][r / W] = t;
+  }
+}
+
+__device__ __forceinline__ float* lin_at(float* base, float* row, int64_t r, int D, int lin_in_row, int64_t lin_off) {
+  return lin_in_row ? row + D : base + lin_off + r;
+}
+
+template <int LPR>
+__global__ void __launch_bounds__(256) shard_adam_prepare_kernel(const int32_t* __restrict__ touch, int64_t n_rows,
+                                                                  int32_t* __restrict__ list, int32_t* __restrict__ count,
+                                                                  float* __restrict__ w, int64_t row_stride,
+                                                                  int64_t lin_off, int lin_in_row,
+                                                                  float* __restrict__ state, int SS, int D,
+                                                                  const int64_t* __restrict__ step_dev, AdamHist hist,
+                                                                  float omb1, float omb2, float eps) {
+  constexpr int G = 32 / LPR;
+  const int lane = threadIdx.x & 31, c = lane % LPR, grp = lane / LPR;
+  const int64_t t_now = *step_dev;
+  const int o_m = D, o_v = 2 * D, o_s = 3 * D;
+  const bool has_lin = lin_in_row || lin_off > 0;
+  // one list slot reservation per CTA pass (not per warp: a single counter serialises its atomics)
+  __shared__ int s_cnt[8], s_pos[8];
+  const int wid = threadIdx.x >> 5;
+  for (int64_t cbase = (int64_t)blockIdx.x * 256; cbase < n_rows; cbase += (int64_t)gridDim.x * 256) {   // CTA-uniform
+    const int64_t base = cbase + wid * 32;
+    const int64_t r = base + lane;
+    const bool hit = r < n_rows && __ldcg(touch + r) == (int32_t)t_now;         // marks of other ranks: not via L1
+    const unsigned mask = __ballot_sync(0xffffffffu, hit);
+    const int nhit = __popc(mask);
+    if (lane == 0) s_cnt[wid] = nhit;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int tot = 0;
+      for (int w = 0; w < 8; ++w) { s_pos[w] = tot; tot += s_cnt[w]; }
+      const int pos0 = tot ? atomicAdd(count, tot) : 0;
+      for (int w = 0; w < 8; ++w) s_pos[w] += pos0;
+    }
+    __syncthreads();
+    if (hit) list[s_pos[wid] + __popc(mask & ((1u << lane) - 1u))] = (int32_t)r;
+    __syncthreads();                                                            // s_pos is rewritten next pass
+    for (int k = 0; k < nhit; k += G) {                                         // G hit rows at a time, one per group
+      const int j = k + grp;
+      int64_t row = -1;
+      if (j < nhit) {
+        unsigned m = mask;
+        for (int q = 0; q < j; ++q) m &= m - 1u;
+        row = base + (__ffs(m) - 1);
+      }
+      float* st = state + (size_t)(row >= 0 ? row : 0) * SS;
+      const int64_t stamp = row >= 0 ? (int64_t)__float_as_int(st[o_s + 4]) : 0;   // every lane reads the stamp ...
+      __syncwarp();                                                               // ... before its leader rewrites it
+      if (row < 0 || stamp <= 0 || stamp >= t_now - 1) continue;
+      float* prow = w + (size_t)row * row_stride;
+      if (c * 4 < D) {
+        float4 mm = *reinterpret_cast<float4*>(st + o_m + c * 4), vv = *reinterpret_cast<float4*>(st + o_v + c * 4);
+        float4 ww = *reinterpret_cast<float4*>(prow + c * 4);
+        float pa[4] = {ww.x, ww.y, ww.z, ww.w}, ma[4] = {mm.x, mm.y, mm.z, mm.w}, va[4] = {vv.x, vv.y, vv.z, vv.w};
+        adam_catch_up<4>(pa, ma, va, stamp, t_now - 1, t_now, hist, omb1, omb2, eps);
+        *reinterpret_cast<float4*>(prow + c * 4) = make_float4(pa[0], pa[1], pa[2], pa[3]);
+        *reinterpret_cast<float4*>(st + o_m + c * 4) = make_float4(ma[0], ma[1], ma[2], ma[3]);
+        *reinterpret_cast<float4*>(st + o_v + c * 4) = make_float4(va[0], va[1], va[2], va[3]);
+      }
+      if (c == 0) {
+        if (has_lin) {
+          float* wp = lin_at(w, prow, row, D, lin_in_row, lin_off);
+          float pa[1] = {*wp}, ma[1] = {st[o_s + 1]}, va[1] = {st[o_s + 2]};
+          adam_catch_up<1>(pa, ma, va, stamp, t_now - 1, t_now, hist, omb1, omb2, eps);
+          *wp = pa[0]; st[o_s + 1] = ma[0]; st[o_s + 2] = va[0];
+        }
+        st[o_s + 4] = __int_as_float((int)(t_now - 1));
+      }
+    }
+  }
+}
+
+template <int LPR>
+__global__ void __launch_bounds__(256) shard_adam_apply_kernel(const int32_t* __restrict__ list,
+                                                                const int32_t* __restrict__ count,
+                                                                float* __restrict__ w, float* __restrict__ g,
+                                                                int64_t row_stride, int64_t lin_off, int lin_in_row,
+                                                                float* __restrict__ state, int SS, int D,
+                                                                const int64_t* __restrict__ step_dev,
+                                                                const float* __restrict__ lr_t_dev, float omb1,
+                                                                float omb2, float eps) {
+  constexpr int G = 32 / LPR;
+  const int lane = threadIdx.x & 31, c = lane % LPR, grp = lane / LPR;
+  const int64_t n = *count;
+  const int t_now = (int)*step_dev;
+  const float lr_t = __ldg(lr_t_dev);
+  const int o_m = D, o_v = 2 * D, o_s = 3 * D;
+  const bool has_lin = lin_in_row || lin_off > 0;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t i = warp * G + grp; i < n; i += nwarps * G) {
+    const int64_t r = __ldg(list + i);
+    float* st = state + (size_t)r * SS;
+    float* prow = w + (size_t)r * row_stride;
+    float* grow = g + (size_t)r * row_stride;
+    if (c * 4 < D) {
+      const float4 gg = __ldcg(reinterpret_cast<const float4*>(grow + c * 4));   // red.add of every rank landed here
+      float4 m = *reinterpret_cast<float4*>(st + o_m + c * 4), v = *reinterpret_cast<float4*>(st + o_v + c * 4);
+      float4 p = *reinterpret_cast<float4*>(prow + c * 4);
+      adam_functor(p.x, gg.x, m.x, v.x, lr_t, omb1, omb2, eps);
+      adam_functor(p.y, gg.y, m.y, v.y, lr_t, omb1, omb2, eps);
+      adam_functor(p.z, gg.z, m.z, v.z, lr_t, omb1, omb2, eps);
+      adam_functor(p.w, gg.w, m.w, v.w, lr_t, omb1, omb2, eps);
+      *reinterpret_cast<float4*>(prow + c * 4) = p;
+      *reinterpret_cast<float4*>(st + o_m + c * 4) = m;
+      *reinterpret_cast<float4*>(st + o_v + c * 4) = v;
+      *reinterpret_cast<float4*>(grow + c * 4) = f4_zero();
+    }
+    if (c == 0) {
+      if (has_lin) {
+        float* wp = lin_at(w, prow, r, D, lin_in_row, lin_off);
+        float* gp = lin_at(g, grow, r, D, lin_in_row, lin_off);
+        float p = *wp, m = st[o_s + 1], v = st[o_s + 2];
+        adam_functor(p, __ldcg(gp), m, v, lr_t, omb1, omb2, eps);
+        *wp = p; st[o_s + 1] = m; st[o_s + 2] = v;
+        *gp = 0.f;
+      }
+      st[o_s + 3] = __int_as_float(0);
+      st[o_s + 4] = __int_as_float(t_now);
+    }
+  }
+}
+
 }  // namespace dr
 
 using namespace dr;
@@ -569,5 +718,109 @@ extern "C" int dr_embed_adam_flush(const int64_t* rows, const int64_t* slot_offs
   }
 #undef DR_FLUSH
   DR_CUDA_LAUNCH_CHECK("dr_embed_adam_flush");
+  return DR_OK;
+}
+
+// ---- row-sharded tf.keras Adam (see shard_adam_mark_kernel) -----------------------------------------------------------
+extern "C" int dr_shard_adam_mark(const void* ids, int id_bytes, int64_t n, int S, const int64_t* slot_offsets,
+                                  const int64_t* rows, int world, int32_t* const* touch_bases, const int64_t* step_dev,
+                                  void* stream) {
+  DR_REQUIRE(n >= 0 && S >= 1 && S <= 4096, DR_EINVAL, "dr_shard_adam_mark: n=%lld S=%d", (long long)n, S);
+  DR_REQUIRE(id_bytes == 8 || id_bytes == 4, DR_EINVAL, "dr_shard_adam_mark: id_bytes=%d (need 4 or 8)", id_bytes);
+  DR_REQUIRE(world >= 1 && world <= kMaxShardWorld, DR_EINVAL, "dr_shard_adam_mark: world=%d outside [1,%d]", world,
+             kMaxShardWorld);
+  DR_REQUIRE(ids && slot_offsets && rows && touch_bases && step_dev, DR_EINVAL, "dr_shard_adam_mark: null pointer");
+  if (n == 0) return DR_OK;
+  int64_t ctas = (n + 255) / 256;
+  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (id_bytes == 8)
+    shard_adam_mark_kernel<int64_t><<<(unsigned)ctas, 256, 0, st>>>((const int64_t*)ids, n, S, slot_offsets, rows, world,
+                                                                     touch_bases, step_dev);
+  else
+    shard_adam_mark_kernel<int32_t><<<(unsigned)ctas, 256, 0, st>>>((const int32_t*)ids, n, S, slot_offsets, rows, world,
+                                                                     touch_bases, step_dev);
+  DR_CUDA_LAUNCH_CHECK("dr_shard_adam_mark");
+  return DR_OK;
+}
+
+static int shard_adam_layout_check(const char* fn, int64_t local_rows, int D, int64_t row_stride, int64_t lin_offset,
+                                   int flags) {
+  DR_REQUIRE(local_rows >= 0 && local_rows < ((int64_t)1 << 31), DR_EINVAL, "%s: local_rows=%lld", fn,
+             (long long)local_rows);
+  DR_REQUIRE(D >= 4 && D <= 128 && D % 4 == 0, DR_EINVAL, "%s: D=%d unsupported", fn, D);
+  const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
+  DR_REQUIRE(row_stride >= D + lin_in_row && row_stride % 4 == 0, DR_EINVAL, "%s: bad row_stride=%lld for D=%d", fn,
+             (long long)row_stride, D);
+  DR_REQUIRE(lin_offset >= 0 && !(lin_in_row && lin_offset > 0) && (lin_offset == 0 || lin_offset >= local_rows * row_stride),
+             DR_EINVAL, "%s: lin_offset=%lld (must trail the rows and be exclusive with DR_EMBED_LIN_IN_ROW)", fn,
+             (long long)lin_offset);
+  return DR_OK;
+}
+
+extern "C" int dr_shard_adam_prepare(int32_t* touch, int64_t local_rows, int32_t* list, int32_t* count, int D,
+                                     int64_t row_stride, int64_t lin_offset, int flags, float* shard, float* state,
+                                     const int64_t* step_dev, const float* lr_hist, int hist_len, float lr, float beta1,
+                                     float beta2, float eps, void* stream) {
+  if (int rc = shard_adam_layout_check("dr_shard_adam_prepare", local_rows, D, row_stride, lin_offset, flags)) return rc;
+  DR_REQUIRE(touch && list && count && shard && state && step_dev, DR_EINVAL, "dr_shard_adam_prepare: null pointer");
+  DR_REQUIRE(hist_len >= 0 && (hist_len == 0 || lr_hist), DR_EINVAL, "dr_shard_adam_prepare: bad lr history");
+  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
+             "dr_shard_adam_prepare: beta1=%g beta2=%g eps=%g out of range", (double)beta1, (double)beta2, (double)eps);
+  DR_REQUIRE(aligned16(shard) && aligned16(state), DR_EALIGN, "dr_shard_adam_prepare: shard / state not 16-B aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  DR_CUDA_CALL(cudaMemsetAsync(count, 0, sizeof(int32_t), st));
+  if (local_rows == 0) return DR_OK;
+  const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
+  const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
+  int64_t ctas = (local_rows + 255) / 256;
+  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
+#define DR_SPREP(L)                                                                                                    \
+  shard_adam_prepare_kernel<L><<<(unsigned)ctas, 256, 0, st>>>(touch, local_rows, list, count, shard, row_stride,      \
+                                                               lin_offset, lin_in_row, state, adam_state_stride(D), D, \
+                                                               step_dev, h, 1.f - beta1, 1.f - beta2, eps)
+  switch (lpr_of(D)) {
+    case 1: DR_SPREP(1); break;
+    case 2: DR_SPREP(2); break;
+    case 4: DR_SPREP(4); break;
+    case 8: DR_SPREP(8); break;
+    case 16: DR_SPREP(16); break;
+    default: DR_SPREP(32); break;
+  }
+#undef DR_SPREP
+  DR_CUDA_LAUNCH_CHECK("dr_shard_adam_prepare");
+  return DR_OK;
+}
+
+extern "C" int dr_shard_adam_apply(const int32_t* list, const int32_t* count, int64_t local_rows, int D,
+                                   int64_t row_stride, int64_t lin_offset, int flags, float* shard, float* grad,
+                                   float* state, const int64_t* step_dev, const float* lr_t_dev, float beta1, float beta2,
+                                   float eps, void* stream) {
+  if (int rc = shard_adam_layout_check("dr_shard_adam_apply", local_rows, D, row_stride, lin_offset, flags)) return rc;
+  DR_REQUIRE(list && count && shard && grad && state && step_dev && lr_t_dev, DR_EINVAL, "dr_shard_adam_apply: null pointer");
+  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
+             "dr_shard_adam_apply: beta1=%g beta2=%g eps=%g out of range", (double)beta1, (double)beta2, (double)eps);
+  DR_REQUIRE(aligned16(shard) && aligned16(grad) && aligned16(state), DR_EALIGN,
+             "dr_shard_adam_apply: shard / grad / state not 16-B aligned");
+  if (local_rows == 0) return DR_OK;
+  const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
+  const int lpr = lpr_of(D);
+  int64_t ctas = (local_rows * lpr + 255) / 256;
+  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
+  cudaStream_t st = (cudaStream_t)stream;
+#define DR_SAPPLY(L)                                                                                                   \
+  shard_adam_apply_kernel<L><<<(unsigned)ctas, 256, 0, st>>>(list, count, shard, grad, row_stride, lin_offset,         \
+                                                             lin_in_row, state, adam_state_stride(D), D, step_dev,     \
+                                                             lr_t_dev, 1.f - beta1, 1.f - beta2, eps)
+  switch (lpr) {
+    case 1: DR_SAPPLY(1); break;
+    case 2: DR_SAPPLY(2); break;
+    case 4: DR_SAPPLY(4); break;
+    case 8: DR_SAPPLY(8); break;
+    case 16: DR_SAPPLY(16); break;
+    default: DR_SAPPLY(32); break;
+  }
+#undef DR_SAPPLY
+  DR_CUDA_LAUNCH_CHECK("dr_shard_adam_apply");
   return DR_OK;
 }

@@ -89,8 +89,6 @@ struct EmbedBwdParams {
                 // points never write a knob: sharded addressing simply passes mode = 0)
 };
 
-constexpr int kMaxShardWorld = 64;
-
 // shared memory carve-up: [S] table ptr | [S] lin ptr | [S] rows | per-warp id slices
 __host__ __device__ inline size_t embed_smem_bytes(int S, int warps, int G, int id_bytes) {
   size_t hdr = (size_t)S * (sizeof(void*) * 2 + sizeof(int64_t) * 2) + kMaxShardWorld * sizeof(void*);

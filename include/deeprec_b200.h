@@ -608,6 +608,35 @@ int dr_embed_adam_flush(const int64_t* rows, const int64_t* slot_offsets, int S,
                         float* const* lin_ptrs, float* state, const int64_t* step_dev, const float* lr_hist,
                         int hist_len, float lr, float beta1, float beta2, float eps, void* stream);
 
+/* The same tf.keras-equal Adam (examples/train_deepfm_on_movielens_keras.py:44 tf.keras.optimizers.Adam(),
+ * examples/train_fm_on_movielens_estimator.py:51 tf.train.AdamOptimizer(0.01)) on ROW-SHARDED tables (owner(r) = r mod
+ * world, local row r div world), the optimizer of ShardedDeepFMTrainStep(optimizer="adam_rows_tf").  Every cross-rank
+ * access is a plain store (mark) or a vector red.add (the backward into the owners' gradient arenas) that nothing reads
+ * before the ranks meet at a barrier; all Adam arithmetic runs on the owner, in its own memory.  Per rank: a gradient
+ * arena in the shard's own layout (row_stride, first-order weight in the row with DR_EMBED_LIN_IN_ROW or trailing at
+ * lin_offset floats from the base), an int32 touch array [local_rows], an int32 row list [local_rows] + device count, and
+ * state blocks [local_rows, dr_embed_adam_state_stride(D)] (dr_embed_adam_flush runs on them with S = 1).  One step t
+ * (step_dev after dr_adam_advance_hist):
+ *   dr_shard_adam_mark    touch_bases[owner][local] = t for every valid lookup (global ids through slot_offsets / rows
+ *                         over `world` peer touch arrays; the NCCL exchange passes its received local ids with world 1,
+ *                         S = 1, rows = {local_rows}, slot_offsets = {0}; -1 padding is skipped).  Barrier.
+ *   dr_shard_adam_prepare the owner lists its rows with touch == t (list, count: device-resident, no host sync) and
+ *                         replays their pending steps (stamp, t-1], as dr_embed_adam_prepare.  Barrier, forward, backward
+ *                         into the gradient arenas (scale 1 / world), barrier.
+ *   dr_shard_adam_apply   step t on every listed row from its gradient row, which it zeroes; stamp = t, count = 0.
+ * world outside [1, 64], D outside {4, 8, ..., 128} or a null pointer return DR_EINVAL before any launch. */
+int dr_shard_adam_mark(const void* ids, int id_bytes, int64_t n, int S, const int64_t* slot_offsets,
+                       const int64_t* rows, int world, int32_t* const* touch_bases, const int64_t* step_dev,
+                       void* stream);
+int dr_shard_adam_prepare(int32_t* touch, int64_t local_rows, int32_t* list, int32_t* count, int D,
+                          int64_t row_stride, int64_t lin_offset, int flags, float* shard, float* state,
+                          const int64_t* step_dev, const float* lr_hist, int hist_len, float lr, float beta1,
+                          float beta2, float eps, void* stream);
+int dr_shard_adam_apply(const int32_t* list, const int32_t* count, int64_t local_rows, int D, int64_t row_stride,
+                        int64_t lin_offset, int flags, float* shard, float* grad, float* state,
+                        const int64_t* step_dev, const float* lr_t_dev, float beta1, float beta2, float eps,
+                        void* stream);
+
 /* ---- 8(f) #2  id pipeline: raw feature value -> int64 row id, bit-exact with TensorFlow's columns.
  * categorical_column_with_hash_bucket = FarmHash Fingerprint64(bytes of str(value)) mod num_buckets
  * (tf.strings.to_hash_bucket_fast).  Device entries take device pointers; strings travel as one byte
