@@ -94,6 +94,9 @@ _SIGS = {
                                 _i, _f, _f, _f, _f, _p],
     "dr_embed_adam_prepare": [_p, _i, _i64, _i, _i, _p, _p, _i64, _i64, _i, _p, _p, _p, _p, _p, _i, _f, _f, _f, _f, _p],
     "dr_embed_adam_flush": [_p, _p, _i, _i, _i64, _i64, _i64, _i, _p, _p, _p, _p, _p, _i, _f, _f, _f, _f, _p],
+    "dr_embed_adam_catch_up": [_p, _i, _i64, _i, _i, _p, _p, _i64, _i64, _i, _p, _p, _p, _p, _p, _i, _f, _f, _f, _f, _p],
+    "dr_embed_adam_rows_tf": [_p, _i, _i64, _i64, _i, _p, _p, _p, _p, _i64, _i64, _p, _i64, _i64, _i, _i64, _i64, _i,
+                              _p, _p, _p, _p, _p, _p, _i, _f, _f, _f, _f, _p],
     "dr_shard_adam_mark": [_p, _i, _i64, _i, _p, _p, _i, _p, _p, _p],
     "dr_shard_adam_prepare": [_p, _i64, _p, _p, _i, _i64, _i64, _i, _p, _p, _p, _p, _i, _f, _f, _f, _f, _p],
     "dr_shard_adam_apply": [_p, _p, _i64, _i, _i64, _i64, _i, _p, _p, _p, _p, _p, _f, _f, _f, _p],

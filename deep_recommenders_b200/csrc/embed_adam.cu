@@ -364,6 +364,189 @@ __global__ void __launch_bounds__(256) embed_adam_flush_kernel(float* const* __r
   }
 }
 
+// ---- the same tf.keras-equal Adam for the layer API (optimizers.RowSparseAdam) ----------------------------------------
+// There a forward may run without a backward (evaluation), so the forward-side pass must leave no count behind:
+//   catch_up : before a forward, bring every row the lookups read up to the current step t_now (the flush, restricted to
+//              the batch's rows).  The lane group whose CAS moves the row's stamp to t_now replays (stamp, t_now].
+//   rows_tf  : after the clock has advanced to t, step t from per-lookup gradient rows given with strides (FNN's input
+//              row, a [B, S, D] stack gradient, a bag's row gradient), counted beforehand by dr_embed_adam_count; the
+//              count / accumulate / last-applies scheme of embed_fm_bwd_adam_kernel on the same state blocks.
+template <int LPR, typename IdT>
+__global__ void __launch_bounds__(256) embed_adam_catch_up_kernel(const IdT* __restrict__ ids, int64_t n_lookups, int S,
+                                                                   int D, const int64_t* __restrict__ rows,
+                                                                   const int64_t* __restrict__ slot_offsets,
+                                                                   float* const* __restrict__ table_ptrs,
+                                                                   float* const* __restrict__ lin_ptrs, int64_t row_stride,
+                                                                   int64_t lin_stride, int lin_in_row,
+                                                                   float* __restrict__ state, int SS,
+                                                                   const int64_t* __restrict__ step_dev, AdamHist hist,
+                                                                   float omb1, float omb2, float eps) {
+  constexpr int G = 32 / LPR;
+  const int lane = threadIdx.x & 31, c = lane % LPR, grp = lane / LPR;
+  const int64_t t_now = *step_dev;
+  const int o_m = D, o_v = 2 * D, o_s = 3 * D;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t base = warp * G; base < n_lookups; base += nwarps * G) {
+    const int64_t L = base + grp;
+    int64_t id = -1;
+    int s = 0;
+    if (L < n_lookups) {
+      s = (int)(L % S);
+      id = (int64_t)__ldg(ids + L);
+      if ((uint64_t)id >= (uint64_t)__ldg(rows + s)) id = -1;
+    }
+    float* st = id >= 0 ? state + (size_t)(__ldg(slot_offsets + s) + id) * SS : nullptr;
+    int won = 0, stamp_i = 0;
+    if (id >= 0 && c == 0) {
+      stamp_i = __float_as_int(ld_cg1(st + o_s + 4));
+      if (stamp_i > 0 && stamp_i < t_now)      // never updated (m = v = 0) or already current: nothing to replay
+        won = atomicCAS(reinterpret_cast<int*>(st + o_s + 4), stamp_i, (int)t_now) == stamp_i;
+    }
+    won = __shfl_sync(0xffffffffu, won, grp * LPR);
+    stamp_i = __shfl_sync(0xffffffffu, stamp_i, grp * LPR);
+    if (!won) continue;
+    const int64_t stamp = stamp_i;
+    float* prow = table_ptrs[s] + (size_t)id * row_stride;
+    if (c * 4 < D) {
+      float4 m = ld_cg4(st + o_m + c * 4), v = ld_cg4(st + o_v + c * 4);
+      float4 w = *reinterpret_cast<const float4*>(prow + c * 4);
+      float pa[4] = {w.x, w.y, w.z, w.w}, ma[4] = {m.x, m.y, m.z, m.w}, va[4] = {v.x, v.y, v.z, v.w};
+      adam_catch_up<4>(pa, ma, va, stamp, t_now, t_now, hist, omb1, omb2, eps);
+      *reinterpret_cast<float4*>(prow + c * 4) = make_float4(pa[0], pa[1], pa[2], pa[3]);
+      stg4(st + o_m + c * 4, make_float4(ma[0], ma[1], ma[2], ma[3]));
+      stg4(st + o_v + c * 4, make_float4(va[0], va[1], va[2], va[3]));
+    }
+    if (c == 0 && (lin_in_row || lin_ptrs)) {
+      float* wp = lin_in_row ? prow + D : lin_ptrs[s] + (size_t)id * lin_stride;
+      float pa[1] = {*wp}, ma[1] = {ld_cg1(st + o_s + 1)}, va[1] = {ld_cg1(st + o_s + 2)};
+      adam_catch_up<1>(pa, ma, va, stamp, t_now, t_now, hist, omb1, omb2, eps);
+      *wp = pa[0]; st[o_s + 1] = ma[0]; st[o_s + 2] = va[0];
+    }
+  }
+}
+
+struct AdamRowsParams {
+  const void* ids;
+  const int64_t* row_splits;     // bags: lookup L is a member of bag b, row_splits[b] <= L < row_splits[b + 1] (S == 1)
+  int64_t n, B;
+  int S, D;
+  const int64_t* rows;
+  const int64_t* slot_offsets;
+  const float* g_emb;            // gradient row of lookup (b, s) at g_emb + b * g_ld + s * g_slot
+  int64_t g_ld, g_slot;
+  const float* g_lin;            // nullable: first-order gradient of lookup (b, s) at g_lin + b * gl_ld + s * gl_slot
+  int64_t gl_ld, gl_slot;
+  float* const* table_ptrs;
+  float* const* lin_ptrs;
+  int64_t row_stride, lin_stride;
+  int lin_in_row;
+  float* state;
+  int SS;
+  const int64_t* step_dev;
+  const float* lr_t_dev;
+  AdamHist hist;
+  float omb1, omb2, eps;
+};
+
+template <int LPR, typename IdT, bool BAGS>
+__global__ void __launch_bounds__(256) embed_adam_rows_tf_kernel(const AdamRowsParams p) {
+  constexpr int G = 32 / LPR;
+  const int lane = threadIdx.x & 31, c = lane % LPR, grp = lane / LPR;
+  const int D = p.D, SS = p.SS, o_m = D, o_v = 2 * D, o_s = 3 * D;
+  const bool chunk_ok = c * 4 < D;
+  const bool has_w = p.g_lin != nullptr;
+  const IdT* __restrict__ ids = reinterpret_cast<const IdT*>(p.ids);
+  const int64_t t_now = *p.step_dev;
+  const float lr_t = __ldg(p.lr_t_dev);
+  const float omb1 = p.omb1, omb2 = p.omb2, eps = p.eps;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t base = warp * G; base < p.n; base += nwarps * G) {     // warp-uniform trip count: the shuffles below
+    const int64_t L = base + grp;
+    int64_t id = -1, b = 0;
+    int s = 0;
+    float den = 1.f;
+    if (L < p.n) {
+      id = (int64_t)__ldg(ids + L);
+      if (BAGS) {                                       // the bag of member L: the last b with row_splits[b] <= L
+        int64_t lo = 0, hi = p.B;
+        while (hi - lo > 1) {
+          const int64_t mid = (lo + hi) >> 1;
+          if (__ldg(p.row_splits + mid) <= L) lo = mid; else hi = mid;
+        }
+        b = lo;
+      } else {
+        s = (int)(L % p.S);
+        b = L / p.S;
+      }
+      const int64_t nrows = __ldg(p.rows + s);
+      if ((uint64_t)id >= (uint64_t)nrows) {
+        id = -1;
+      } else if (BAGS) {                                // mean combiner: the bag's valid members share its gradient
+        int cnt = 0;
+        for (int64_t j = __ldg(p.row_splits + b), e = __ldg(p.row_splits + b + 1); j < e; ++j) {
+          const int64_t q = (int64_t)__ldg(ids + j);
+          cnt += (q >= 0 && q < nrows) ? 1 : 0;
+        }
+        den = (float)cnt;
+      }
+    }
+    float* st = nullptr;
+    if (id >= 0) {
+      st = p.state + (size_t)(__ldg(p.slot_offsets + s) + id) * SS;
+      if (chunk_ok) {
+        float4 g = ldg4(p.g_emb + (size_t)b * p.g_ld + (size_t)s * p.g_slot + c * 4);
+        if (BAGS) g = make_float4(g.x / den, g.y / den, g.z / den, g.w / den);
+        red_add_v4(st + c * 4, g);
+      }
+      if (c == 0 && has_w) red_add_f32(st + o_s, __ldg(p.g_lin + (size_t)b * p.gl_ld + (size_t)s * p.gl_slot));
+    }
+    __threadfence();     // this lane's contributions are performed before the group leader announces them
+    __syncwarp();
+    int old = 0;
+    if (id >= 0 && c == 0) old = atomicSub(reinterpret_cast<int*>(st + o_s + 3), 1);
+    old = __shfl_sync(0xffffffffu, old, grp * LPR);
+    int stamp_i = 0;
+    if (id >= 0 && c == 0 && old == 1) stamp_i = __float_as_int(ld_cg1(st + o_s + 4));
+    stamp_i = __shfl_sync(0xffffffffu, stamp_i, grp * LPR);
+    if (id < 0 || old != 1) continue;                  // not the last contributor of this row in this step
+    __threadfence();
+    const int64_t stamp = stamp_i;
+    float* prow = p.table_ptrs[s] + (size_t)id * p.row_stride;
+    if (chunk_ok) {
+      const float4 g = ld_cg4(st + c * 4);
+      float4 m = ld_cg4(st + o_m + c * 4), v = ld_cg4(st + o_v + c * 4);
+      float4 w = *reinterpret_cast<const float4*>(prow + c * 4);
+      float pa[4] = {w.x, w.y, w.z, w.w}, ma[4] = {m.x, m.y, m.z, m.w}, va[4] = {v.x, v.y, v.z, v.w};
+      adam_catch_up<4>(pa, ma, va, stamp, t_now - 1, t_now, p.hist, omb1, omb2, eps);
+      w = make_float4(pa[0], pa[1], pa[2], pa[3]); m = make_float4(ma[0], ma[1], ma[2], ma[3]);
+      v = make_float4(va[0], va[1], va[2], va[3]);
+      adam_functor(w.x, g.x, m.x, v.x, lr_t, omb1, omb2, eps);
+      adam_functor(w.y, g.y, m.y, v.y, lr_t, omb1, omb2, eps);
+      adam_functor(w.z, g.z, m.z, v.z, lr_t, omb1, omb2, eps);
+      adam_functor(w.w, g.w, m.w, v.w, lr_t, omb1, omb2, eps);
+      *reinterpret_cast<float4*>(prow + c * 4) = w;
+      stg4(st + o_m + c * 4, m);
+      stg4(st + o_v + c * 4, v);
+      stg4(st + c * 4, f4_zero());
+    }
+    if (c == 0) {
+      if (has_w) {
+        float* wp = p.lin_in_row ? prow + D : p.lin_ptrs[s] + (size_t)id * p.lin_stride;
+        float pa[1] = {*wp}, ma[1] = {ld_cg1(st + o_s + 1)}, va[1] = {ld_cg1(st + o_s + 2)};
+        adam_catch_up<1>(pa, ma, va, stamp, t_now - 1, t_now, p.hist, omb1, omb2, eps);
+        adam_functor(pa[0], ld_cg1(st + o_s), ma[0], va[0], lr_t, omb1, omb2, eps);
+        *wp = pa[0];
+        st[o_s + 1] = ma[0];
+        st[o_s + 2] = va[0];
+        st[o_s] = 0.f;
+      }
+      st[o_s + 4] = __int_as_float((int)t_now);
+    }
+  }
+}
+
 __global__ void adam_advance_hist_kernel(int64_t* step, float lr, float b1, float b2, float* lr_t, float* lr_hist,
                                          int hist_len) {
   const int64_t t = *step + 1;
@@ -718,6 +901,121 @@ extern "C" int dr_embed_adam_flush(const int64_t* rows, const int64_t* slot_offs
   }
 #undef DR_FLUSH
   DR_CUDA_LAUNCH_CHECK("dr_embed_adam_flush");
+  return DR_OK;
+}
+
+// ---- tf.keras Adam of the layer API (see embed_adam_catch_up_kernel) --------------------------------------------------
+static int adam_rows_layout_check(const char* fn, int D, int64_t& row_stride, int64_t& lin_stride, int flags,
+                                  float* const* lin_ptrs, int& lin_in_row) {
+  DR_REQUIRE(D >= 4 && D <= 128 && D % 4 == 0, DR_EINVAL, "%s: D=%d unsupported", fn, D);
+  DR_REQUIRE(flags == (flags & DR_EMBED_LIN_IN_ROW), DR_EINVAL, "%s: flags=%d (only DR_EMBED_LIN_IN_ROW)", fn, flags);
+  if (row_stride == 0) row_stride = D;
+  if (lin_stride == 0) lin_stride = 1;
+  lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
+  DR_REQUIRE(row_stride >= D + (lin_in_row ? 4 : 0) && row_stride % 4 == 0 && lin_stride >= 1, DR_EINVAL,
+             "%s: bad strides row=%lld lin=%lld for D=%d", fn, (long long)row_stride, (long long)lin_stride, D);
+  DR_REQUIRE(!(lin_in_row && lin_ptrs), DR_EINVAL, "%s: lin_ptrs given with DR_EMBED_LIN_IN_ROW", fn);
+  return DR_OK;
+}
+
+extern "C" int dr_embed_adam_catch_up(const void* ids, int id_bytes, int64_t n, int S, int D, const int64_t* rows,
+                                      const int64_t* slot_offsets, int64_t row_stride, int64_t lin_stride, int flags,
+                                      float* const* table_ptrs, float* const* lin_ptrs, float* state,
+                                      const int64_t* step_dev, const float* lr_hist, int hist_len, float lr,
+                                      float beta1, float beta2, float eps, void* stream) {
+  const char* fn = "dr_embed_adam_catch_up";
+  DR_REQUIRE(n >= 0 && S >= 1 && S <= 4096 && n % S == 0, DR_EINVAL, "%s: n=%lld S=%d", fn, (long long)n, S);
+  DR_REQUIRE(id_bytes == 8 || id_bytes == 4, DR_EINVAL, "%s: id_bytes=%d (need 4 or 8)", fn, id_bytes);
+  int lin_in_row = 0;
+  if (int rc = adam_rows_layout_check(fn, D, row_stride, lin_stride, flags, lin_ptrs, lin_in_row)) return rc;
+  DR_REQUIRE(hist_len >= 0 && (hist_len == 0 || lr_hist), DR_EINVAL, "%s: bad lr history", fn);
+  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
+             "%s: beta1=%g beta2=%g eps=%g out of range", fn, (double)beta1, (double)beta2, (double)eps);
+  if (n == 0) return DR_OK;
+  DR_REQUIRE(ids && rows && slot_offsets && table_ptrs && state && step_dev, DR_EINVAL, "%s: null pointer", fn);
+  DR_REQUIRE(aligned16(state), DR_EALIGN, "%s: state not 16-B aligned", fn);
+  const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
+  const int lpr = lpr_of(D);
+  int64_t ctas = (n * lpr + 255) / 256;
+  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
+  cudaStream_t st = (cudaStream_t)stream;
+#define DR_CATCH2(L, IdT)                                                                                              \
+  embed_adam_catch_up_kernel<L, IdT><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, n, S, D, rows, slot_offsets,      \
+                                                                   table_ptrs, lin_ptrs, row_stride, lin_stride,       \
+                                                                   lin_in_row, state, adam_state_stride(D), step_dev, h, \
+                                                                   1.f - beta1, 1.f - beta2, eps)
+#define DR_CATCH(L) do { if (id_bytes == 8) DR_CATCH2(L, int64_t); else DR_CATCH2(L, int32_t); } while (0)
+  switch (lpr) {
+    case 1: DR_CATCH(1); break;
+    case 2: DR_CATCH(2); break;
+    case 4: DR_CATCH(4); break;
+    case 8: DR_CATCH(8); break;
+    case 16: DR_CATCH(16); break;
+    default: DR_CATCH(32); break;
+  }
+#undef DR_CATCH
+#undef DR_CATCH2
+  DR_CUDA_LAUNCH_CHECK(fn);
+  return DR_OK;
+}
+
+extern "C" int dr_embed_adam_rows_tf(const void* ids, int id_bytes, int64_t n, int64_t B, int S,
+                                     const int64_t* row_splits, const int64_t* rows, const int64_t* slot_offsets,
+                                     const float* g_emb, int64_t g_ld, int64_t g_slot, const float* g_lin,
+                                     int64_t gl_ld, int64_t gl_slot, int D, int64_t row_stride, int64_t lin_stride,
+                                     int flags, float* const* table_ptrs, float* const* lin_ptrs, float* state,
+                                     const int64_t* step_dev, const float* lr_t_dev, const float* lr_hist, int hist_len,
+                                     float lr, float beta1, float beta2, float eps, void* stream) {
+  const char* fn = "dr_embed_adam_rows_tf";
+  DR_REQUIRE(n >= 0 && B >= 0 && S >= 1 && S <= 4096, DR_EINVAL, "%s: n=%lld B=%lld S=%d", fn, (long long)n,
+             (long long)B, S);
+  DR_REQUIRE(row_splits ? S == 1 : n == B * S, DR_EINVAL, "%s: %s", fn,
+             row_splits ? "bags (row_splits) need S = 1" : "n != B * S");
+  DR_REQUIRE(id_bytes == 8 || id_bytes == 4, DR_EINVAL, "%s: id_bytes=%d (need 4 or 8)", fn, id_bytes);
+  int lin_in_row = 0;
+  if (int rc = adam_rows_layout_check(fn, D, row_stride, lin_stride, flags, lin_ptrs, lin_in_row)) return rc;
+  DR_REQUIRE(!g_lin == !(lin_in_row || lin_ptrs), DR_EINVAL,
+             "%s: g_lin and the first-order weights (lin_ptrs or DR_EMBED_LIN_IN_ROW) come together", fn);
+  // a stride of 0 broadcasts one row (a zero gradient for a term the forward did not use)
+  DR_REQUIRE(g_ld >= 0 && g_slot >= 0 && g_ld % 4 == 0 && g_slot % 4 == 0 && (B <= 1 || g_ld == 0 || g_ld >= D) &&
+                 (S == 1 || g_slot == 0 || g_slot >= D) && (!g_lin || (gl_ld >= 0 && gl_slot >= 0)),
+             DR_EINVAL, "%s: bad gradient strides g_ld=%lld g_slot=%lld gl_ld=%lld gl_slot=%lld for D=%d", fn,
+             (long long)g_ld, (long long)g_slot, (long long)gl_ld, (long long)gl_slot, D);
+  DR_REQUIRE(hist_len >= 0 && (hist_len == 0 || lr_hist), DR_EINVAL, "%s: bad lr history", fn);
+  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
+             "%s: beta1=%g beta2=%g eps=%g out of range", fn, (double)beta1, (double)beta2, (double)eps);
+  if (n == 0) return DR_OK;
+  DR_REQUIRE(ids && rows && slot_offsets && g_emb && table_ptrs && state && step_dev && lr_t_dev && (!row_splits || B >= 1),
+             DR_EINVAL, "%s: null pointer", fn);
+  DR_REQUIRE(aligned16(g_emb) && aligned16(state), DR_EALIGN, "%s: g_emb / state not 16-B aligned", fn);
+  AdamRowsParams p{};
+  p.ids = ids; p.row_splits = row_splits; p.n = n; p.B = B; p.S = S; p.D = D; p.rows = rows;
+  p.slot_offsets = slot_offsets; p.g_emb = g_emb; p.g_ld = g_ld; p.g_slot = g_slot; p.g_lin = g_lin; p.gl_ld = gl_ld;
+  p.gl_slot = gl_slot; p.table_ptrs = table_ptrs; p.lin_ptrs = lin_ptrs; p.row_stride = row_stride;
+  p.lin_stride = lin_stride; p.lin_in_row = lin_in_row; p.state = state; p.SS = adam_state_stride(D);
+  p.step_dev = step_dev; p.lr_t_dev = lr_t_dev; p.hist = AdamHist{lr_hist, hist_len, lr, beta1, beta2};
+  p.omb1 = 1.f - beta1; p.omb2 = 1.f - beta2; p.eps = eps;
+  const int lpr = lpr_of(D);
+  int64_t ctas = (n * lpr + 255) / 256;
+  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
+  cudaStream_t st = (cudaStream_t)stream;
+#define DR_ROWS3(L, IdT)                                                                                \
+  do {                                                                                                  \
+    if (row_splits) embed_adam_rows_tf_kernel<L, IdT, true><<<(unsigned)ctas, 256, 0, st>>>(p);         \
+    else embed_adam_rows_tf_kernel<L, IdT, false><<<(unsigned)ctas, 256, 0, st>>>(p);                   \
+  } while (0)
+#define DR_ROWS(L) do { if (id_bytes == 8) DR_ROWS3(L, int64_t); else DR_ROWS3(L, int32_t); } while (0)
+  switch (lpr) {
+    case 1: DR_ROWS(1); break;
+    case 2: DR_ROWS(2); break;
+    case 4: DR_ROWS(4); break;
+    case 8: DR_ROWS(8); break;
+    case 16: DR_ROWS(16); break;
+    default: DR_ROWS(32); break;
+  }
+#undef DR_ROWS
+#undef DR_ROWS3
+  DR_CUDA_LAUNCH_CHECK(fn);
   return DR_OK;
 }
 

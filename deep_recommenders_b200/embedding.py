@@ -30,6 +30,11 @@ from torch import nn
 from . import ops
 
 
+def _flush_row_optimizer(module, prefix, keep_vars):
+    if module.row_optimizer is not None:
+        module.row_optimizer.flush()
+
+
 class EmbeddingCollection(nn.Module):
     def __init__(self, rows: Sequence[int], dim: int, with_linear: bool = True, device=None,
                  init_stddev: Optional[float] = None, seed: Optional[int] = None,
@@ -75,6 +80,10 @@ class EmbeddingCollection(nn.Module):
         self.register_buffer("_offsets", torch.tensor(offs[:-1], dtype=torch.int64, device=dev), persistent=False)
         self.register_buffer("_rows", torch.tensor(self.rows_list, dtype=torch.int64, device=dev), persistent=False)
         self._ptr_cache = {}
+        # optimizers.RowSparseAdam, once one trains the tables: the forward ops replay the rows' pending steps first,
+        # and the arena is flushed before state_dict() reads it
+        self.row_optimizer = None
+        self.register_state_dict_pre_hook(_flush_row_optimizer)
 
     # device pointer arrays for the kernel (computed on device: no host sync)
     def pointers(self, weight: torch.Tensor, linear: Optional[torch.Tensor], cache: bool = True):

@@ -48,6 +48,14 @@ class FM(object):
     def parameters(self):
         return self.collection.parameters()
 
+    def embedding_collection(self):
+        """The EmbeddingCollection of the tables and first-order weights (what an optimizers.RowSparseAdam trains)."""
+        return self.collection
+
+    def dense_variables(self):
+        """The trainable variables outside the table arena: the bias of the first-order term."""
+        return [self.collection.bias]
+
     def export(self, path):
         """Write the trained tables to `path` as one torch.save file of CPU tensors, keyed by feature name like the two
         dicts the reference's FNN reads from an FM SavedModel (fnn.py:32-48) -- what ranking.FNN warm-starts from:
@@ -57,6 +65,8 @@ class FM(object):
         Loadable with torch.load(path, weights_only=True).  The tensors are copies: the file does not share storage
         with the collection's arena."""
         coll = self.collection
+        if coll.row_optimizer is not None:     # the rows' pending Adam steps first: the file holds what dense Adam would
+            coll.row_optimizer.flush()
 
         def cpu(t):
             return t.detach().to("cpu", copy=True).contiguous()

@@ -30,6 +30,22 @@ class DeepFM(object):
         yield from self._fm.parameters()
         yield from self._dnn.parameters()
 
+    def embedding_collection(self):
+        """The EmbeddingCollection of the FM part's tables and first-order weights (shared with the tower's input)."""
+        return self._fm.embedding_collection()
+
+    def dense_variables(self):
+        """The trainable variables outside the table arena: the FM bias and the tower's kernels and biases.  A tower
+        that no call has built yet is built here, as the first call would build it (same shapes, same seeded
+        initialisers), so that an optimizer made before the first step holds every variable."""
+        coll = self.embedding_collection()
+        width = coll.num_slots * coll.dim
+        for layer in self._dnn.layers:
+            if not layer.built:
+                layer.build((None, width), device=coll.weight.device)
+            width = layer.units
+        return self._fm.dense_variables() + list(self._dnn.parameters())
+
     def __call__(self, *args, **kwargs):
         return self.call(*args, **kwargs)
 

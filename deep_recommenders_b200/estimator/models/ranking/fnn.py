@@ -127,6 +127,14 @@ class FNN(object):
             yield self.embeddings.linear
         yield from self._dnn.parameters()
 
+    def embedding_collection(self):
+        """The EmbeddingCollection of the embeddings and first-order weights warm-started from the FM."""
+        return self.embeddings
+
+    def dense_variables(self):
+        """The trainable variables outside the table arena: the tower's kernels and biases (the bias is a constant)."""
+        return list(self._dnn.parameters())
+
     def __call__(self, *args, **kwargs):
         return self.call(*args, **kwargs)
 

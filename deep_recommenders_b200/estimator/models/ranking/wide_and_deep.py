@@ -62,6 +62,14 @@ class WDL(object):
         the tower is included here so that the deep optimizer trains it (DESIGN.md section 7)."""
         return [self.embeddings.weight] + list(self._dnn.parameters())
 
+    def embedding_collection(self):
+        """The EmbeddingCollection of the deep part's tables (no first-order weights)."""
+        return self.embeddings
+
+    def dense_variables(self):
+        """The deep variables outside the table arena: the tower's kernels and biases."""
+        return list(self._dnn.parameters())
+
     def parameters(self):
         yield from self.wide_variables()
         yield from self.deep_variables()

@@ -67,6 +67,8 @@ class EmbedFM(torch.autograd.Function):
         ids = _ids(ids)
         B, S = ids.shape
         D = meta.dim
+        if _row_opt(meta) is not None:
+            meta.row_optimizer.catch_up(ids)
         stack = torch.empty((B, S, D), device=weight.device, dtype=torch.float32)
         sum_e = torch.empty((B, D), device=weight.device, dtype=torch.float32) if want_logit else None
         logit = torch.empty((B,), device=weight.device, dtype=torch.float32) if want_logit else None
@@ -102,6 +104,8 @@ class EmbedFM(torch.autograd.Function):
         g_logit = _f32(g_logit, "g_logit") if (want_logit and g_logit is not None) else None
         if g_stack is None and g_logit is None:
             return None, None, None, None, None, None, None
+        if _row_opt(meta) is not None:
+            return EmbedFM._backward_rows(ctx, ids, stack, sum_e, bias, g_stack, g_logit)
         fused = meta.sparse_lr is not None
         if fused:
             gw, gl, gb = weight, linear, bias
@@ -126,6 +130,42 @@ class EmbedFM(torch.autograd.Function):
         if fused:
             return None, None, None, None, None, None, None
         return None, gw, gl, gb, None, None, None
+
+    @staticmethod
+    def _backward_rows(ctx, ids, stack, sum_e, bias, g_stack, g_logit):
+        """A RowSparseAdam trains the tables: hand it what its step() needs and return the bias gradient only."""
+        lib = _lib.load()
+        meta = ctx.meta
+        opt = meta.row_optimizer
+        B, S = ids.shape
+        D = meta.dim
+        if g_logit is not None and not ctx.no_fm:
+            opt.record_fm(ids, stack, sum_e, g_logit, g_stack)
+        else:     # no FM term: the stack gradient is the row gradient, g_logit the first-order one
+            g, ld, sl = (g_stack, S * D, D) if g_stack is not None else (stack.new_zeros((D,)), 0, 0)
+            gl, gl_ld = None, 0
+            if meta.with_linear:
+                gl, gl_ld = (g_logit, 1) if (g_logit is not None and ctx.has_lin) else (stack.new_zeros((1,)), 0)
+            opt.record_rows(ids, g, 0, ld, sl, gl, 0, gl_ld, 0)
+        gb = None
+        if ctx.has_bias and g_logit is not None:
+            gb = torch.empty_like(bias)
+            check(lib.dr_act_bwd_colsum(None, g_logit.data_ptr(), B, 1, 0, None, gb.data_ptr(), _stream()),
+                  "dr_act_bwd_colsum")
+        return None, None, None, gb, None, None, None
+
+
+def _row_opt(meta):
+    """The RowSparseAdam attached to an EmbeddingCollection (optimizers.py), or None."""
+    return getattr(meta, "row_optimizer", None)
+
+
+def _no_lookup(ids: torch.Tensor, slots) -> torch.Tensor:
+    """A copy of ids with the given columns set to -1 (no lookup)."""
+    ids = ids.clone()
+    if slots:
+        ids[:, list(slots)] = -1
+    return ids
 
 
 class Gather(torch.autograd.Function):
@@ -1313,6 +1353,8 @@ class EmbedFMMixed(torch.autograd.Function):
     @staticmethod
     def forward(ctx, ids, weight, linear, bias, meta, bags):
         lib = _lib.load()
+        if _row_opt(meta) is not None:
+            meta.row_optimizer.catch_up(ids, bags)
         if not meta.with_linear:
             return EmbedFMMixed._forward_no_linear(ctx, ids, weight, meta, bags)
         if bias is None:
@@ -1373,7 +1415,49 @@ class EmbedFMMixed(torch.autograd.Function):
         return None, (None if fused_sgd else gw), None, None, None, None
 
     @staticmethod
+    def _backward_rows(ctx, g_stack, g_logit):
+        """A RowSparseAdam trains the tables: hand it the per-lookup gradient rows (the bag slots' as their bags' rows)
+        and return the bias gradient only.  Without the FM term they are g_stack itself; with it, one dr_embed_fm_bwd
+        forms them in [B, S, D] / [B, S] scratch "tables" that lookup (b, s) reads as row b."""
+        lib = _lib.load()
+        meta = ctx.meta
+        ids, stack, sum_e, _, _, bias, _ = ctx.saved_tensors
+        B, S = ids.shape
+        D = meta.dim
+        dev = stack.device
+        g_stack = None if g_stack is None else _f32(g_stack, "g_stack")
+        g_logit = None if g_logit is None else _f32(g_logit, "g_logit")
+        if g_stack is None and (g_logit is None or not meta.with_linear):
+            return None, None, None, None, None, None
+        gb, gl, gl_ld, gl_sl = None, None, 0, 0
+        if not meta.with_linear:
+            g, ld, sl = g_stack, S * D, D
+        else:
+            if g_logit is None:
+                g_logit = torch.zeros((B,), device=dev, dtype=torch.float32)
+            g = torch.zeros((B, S, D), device=dev, dtype=torch.float32)
+            gl = torch.zeros((B, S), device=dev, dtype=torch.float32)
+            gb = torch.zeros_like(bias)
+            ld, sl, gl_ld, gl_sl = S * D, D, S, 1
+            cols = torch.arange(S, device=dev, dtype=torch.int64)
+            tp, lp = g.data_ptr() + cols * (4 * D), gl.data_ptr() + cols * 4
+            rows_b = torch.full((S,), B, device=dev, dtype=torch.int64)
+            ar = torch.arange(B, device=dev, dtype=ids.dtype).unsqueeze(1).expand(B, S).contiguous()
+            with torch.no_grad():
+                check(lib.dr_embed_fm_bwd(ar.data_ptr(), ar.element_size(), rows_b.data_ptr(), stack.data_ptr(),
+                                          sum_e.data_ptr(), g_logit.data_ptr(), _ptr(g_stack), B, S, D, ld, S, 0,
+                                          tp.data_ptr(), lp.data_ptr(), gb.data_ptr(), 1.0, _stream()),
+                      "dr_embed_fm_bwd")
+        opt = meta.row_optimizer
+        opt.record_rows(_no_lookup(ids, [s for s, _, _ in ctx.saved_bags]), g, 0, ld, sl, gl, 0, gl_ld, gl_sl)
+        for s, bid, bsp in ctx.saved_bags:
+            opt.record_bag(s, bid, bsp, g, s * sl, ld, gl, s * gl_sl, gl_ld)
+        return None, None, None, gb, None, None
+
+    @staticmethod
     def backward(ctx, g_stack, g_logit):
+        if _row_opt(ctx.meta) is not None:
+            return EmbedFMMixed._backward_rows(ctx, g_stack, g_logit)
         if not ctx.meta.with_linear:
             return EmbedFMMixed._backward_no_linear(ctx, g_stack)
         lib = _lib.load()
@@ -1436,6 +1520,8 @@ class FnnInputFn(torch.autograd.Function):
         bias = _f32(bias, "bias")
         if bias.numel() != 1:
             raise ValueError(f"FnnInputFn: bias must have one element, got {tuple(bias.shape)}")
+        if _row_opt(meta) is not None:
+            meta.row_optimizer.catch_up(ids, bags)
         if bags:
             ids, tp, lp, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, linear, meta, bags)
         else:
@@ -1463,7 +1549,13 @@ class FnnInputFn(torch.autograd.Function):
         g_x = _f32(g_x, "g_x")
         B, S = ids.shape
         D = meta.dim
-        _, ld = fnn_layout(S, D)
+        P, ld = fnn_layout(S, D)
+        opt = _row_opt(meta)
+        if opt is not None:     # a RowSparseAdam trains the tables: g_x holds every lookup's gradient row
+            opt.record_rows(_no_lookup(ids, [s for s, _, _ in ctx.saved_bags]), g_x, P, ld, D, g_x, 1, ld, 1)
+            for s, bid, bsp in ctx.saved_bags:
+                opt.record_bag(s, bid, bsp, g_x, P + s * D, ld, g_x, 1 + s, ld)
+            return None, None, None, None, None, None
         fused_sgd = meta.sparse_lr is not None
         if fused_sgd:
             gw, gl, scale = weight, linear, -float(meta.sparse_lr)

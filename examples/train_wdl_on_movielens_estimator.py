@@ -8,7 +8,11 @@ The reference's two `minimize` calls read the same forward pass and update disjo
 one backward and both updates is the same step.  Data: the TFRecord reader when a MovieLens directory is given, else
 seeded synthetic MovieLens-1M-shaped batches.  Exits non-zero if the training loss did not fall.
 
+--embedding-optimizer rows_tf trains the deep part's tables with optimizers.RowSparseAdam instead of dense Adam over the
+arena: the same TF1 Adam, at row-sparse cost, on the clock of the dense optimizer that keeps the tower (default: dense).
+
     python examples/train_wdl_on_movielens_estimator.py [--train-steps N] [--eval-steps N] [--data DIR]
+                                                        [--embedding-optimizer {dense,rows_tf}]
 Needs a CUDA device (the model runs in libdeeprec_b200.so; there is no CPU fallback).
 """
 import argparse
@@ -21,6 +25,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from deep_recommenders_b200 import feature_column as fc  # noqa: E402     (tf.feature_column)
 from deep_recommenders_b200 import ops  # noqa: E402                      (tf.train.FtrlOptimizer / AdamOptimizer)
+from deep_recommenders_b200.optimizers import HISTORY, RowSparseAdam  # noqa: E402
 from deep_recommenders_b200.keras import engine as K  # noqa: E402        (tf.metrics.auc)
 from deep_recommenders.estimator.models.ranking import WDL  # noqa: E402
 
@@ -81,9 +86,9 @@ class DeepAdam:
     """tf.train.AdamOptimizer(0.01) on the deep variables: TensorFlow's ApplyAdam (ops.adam_step_), dense over each
     variable, with the bias-corrected rate kept on the device."""
 
-    def __init__(self, params, lr=0.01, beta1=0.9, beta2=0.999, eps=1e-8):
+    def __init__(self, params, lr=0.01, beta1=0.9, beta2=0.999, eps=1e-8, history=0):
         self.params = [(p, torch.zeros_like(p), torch.zeros_like(p)) for p in params]
-        self.clock = ops.AdamClock(lr, beta1, beta2, eps, device=self.params[0][0].device)
+        self.clock = ops.AdamClock(lr, beta1, beta2, eps, device=self.params[0][0].device, history=history)
 
     def step(self):
         self.clock.advance()
@@ -94,13 +99,15 @@ class DeepAdam:
             ops.adam_step_(p.data, p.grad, m, v, 0.0, c.beta1, c.beta2, c.eps, zero_grad=True, lr_t_dev=c.lr_t)
 
 
-def main():
+def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--train-steps", type=int, default=400)
     ap.add_argument("--eval-steps", type=int, default=20)
     ap.add_argument("--batch-size", type=int, default=1024)
     ap.add_argument("--data", default=None, help="MovieLens TFRecord directory (datasets.MovielensRanking); default synthetic")
-    args = ap.parse_args()
+    ap.add_argument("--embedding-optimizer", choices=("dense", "rows_tf"), default="dense",
+                    help="Adam of the deep tables: dense over the arena, or optimizers.RowSparseAdam (same numbers)")
+    args = ap.parse_args(argv)
     indicator_columns, embedding_columns = build_columns()
     crossed_product_columns = cross_product_transformation()
     if args.data:
@@ -112,7 +119,12 @@ def main():
 
     model = WDL(indicator_columns + crossed_product_columns, embedding_columns, [64, 16], seed=42, device="cuda")
     wide_optimizer = ops.FtrlOptimizer(0.01, l1_regularization_strength=0.5)
-    deep_optimizer = DeepAdam(model.deep_variables(), 0.01)
+    rows_optimizer = None
+    if args.embedding_optimizer == "dense":
+        deep_optimizer = DeepAdam(model.deep_variables(), 0.01)
+    else:
+        deep_optimizer = DeepAdam(model.dense_variables(), 0.01, history=HISTORY)
+        rows_optimizer = RowSparseAdam(model.embedding_collection(), 0.01, clock=deep_optimizer.clock)
     dev = torch.device("cuda")
 
     losses = []
@@ -126,6 +138,8 @@ def main():
         loss.backward()
         wide_optimizer.apply(model.linear)
         deep_optimizer.step()
+        if rows_optimizer is not None:
+            rows_optimizer.step()
         losses.append(loss.detach())
         if (step + 1) % 100 == 0:
             print(f"step {step + 1}: loss {float(torch.stack(losses[-100:]).mean()):.4f}")
@@ -145,6 +159,7 @@ def main():
     print(f"eval auc: {auc.result():.4f}")
     if not last < first:
         raise SystemExit("the training loss did not fall")
+    return first, last, float(auc.result())
 
 
 if __name__ == "__main__":

@@ -608,6 +608,38 @@ int dr_embed_adam_flush(const int64_t* rows, const int64_t* slot_offsets, int S,
                         float* const* lin_ptrs, float* state, const int64_t* step_dev, const float* lr_hist,
                         int hist_len, float lr, float beta1, float beta2, float eps, void* stream);
 
+/* The same TensorFlow-equal Adam for the layer API (optimizers.RowSparseAdam), where a forward may run without a
+ * backward and the gradient of a lookup comes in several layouts.  Same state blocks (dr_embed_adam_state_stride), same
+ * clock (dr_adam_advance_hist), same replay and kCatchUpMax cap as above.  Lookups are ids [n] with slot i % S.
+ *   dr_embed_adam_catch_up  before a forward (training or evaluation, with step_dev = the last completed step t):
+ *                           replays the pending steps (stamp, t] of every row the lookups read.  It counts nothing,
+ *                           so a forward that no backward follows leaves no state behind.
+ *   dr_embed_adam_rows_tf   after dr_adam_advance_hist moved step_dev to t and dr_embed_adam_count counted the same
+ *                           lookups: step t on every row they touch.  The gradient row of lookup (b, s) is read at
+ *                           g_emb + b * g_ld + s * g_slot (16-B aligned; multiples of 4 floats, each 0 or at least
+ *                           D: a stride of 0 broadcasts one row), its first-order
+ *                           gradient at g_lin + b * gl_ld + s * gl_slot.  g_lin is NULL exactly when the table has no
+ *                           first-order weights (lin_ptrs NULL and no DR_EMBED_LIN_IN_ROW); then no first-order slot is
+ *                           touched.  row_splits (nullable, [B + 1], row_splits[0] = 0, row_splits[B] = n) makes the
+ *                           lookups the members of B bags of one slot (S = 1, mean combiner): each valid member takes its
+ *                           bag's gradient row / the bag's valid count and its first-order gradient at scale 1.  Without
+ *                           it, n = B * S.  Duplicate lookups of a row are summed before the update; ids < 0 or >= rows
+ *                           take none.
+ * Bad sizes, strides or flags, D outside {4, 8, ..., 128} or a null pointer return DR_EINVAL before any launch;
+ * a misaligned g_emb / state DR_EALIGN. */
+int dr_embed_adam_catch_up(const void* ids, int id_bytes, int64_t n, int S, int D, const int64_t* rows,
+                           const int64_t* slot_offsets, int64_t row_stride, int64_t lin_stride, int flags,
+                           float* const* table_ptrs, float* const* lin_ptrs, float* state, const int64_t* step_dev,
+                           const float* lr_hist, int hist_len, float lr, float beta1, float beta2, float eps,
+                           void* stream);
+int dr_embed_adam_rows_tf(const void* ids, int id_bytes, int64_t n, int64_t B, int S, const int64_t* row_splits,
+                          const int64_t* rows, const int64_t* slot_offsets, const float* g_emb, int64_t g_ld,
+                          int64_t g_slot, const float* g_lin, int64_t gl_ld, int64_t gl_slot, int D,
+                          int64_t row_stride, int64_t lin_stride, int flags, float* const* table_ptrs,
+                          float* const* lin_ptrs, float* state, const int64_t* step_dev, const float* lr_t_dev,
+                          const float* lr_hist, int hist_len, float lr, float beta1, float beta2, float eps,
+                          void* stream);
+
 /* The same tf.keras-equal Adam (examples/train_deepfm_on_movielens_keras.py:44 tf.keras.optimizers.Adam(),
  * examples/train_fm_on_movielens_estimator.py:51 tf.train.AdamOptimizer(0.01)) on ROW-SHARDED tables (owner(r) = r mod
  * world, local row r div world), the optimizer of ShardedDeepFMTrainStep(optimizer="adam_rows_tf").  Every cross-rank
