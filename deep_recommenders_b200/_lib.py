@@ -33,6 +33,7 @@ _SIGS = {
     "dr_set_workspace": [_p, C.c_uint64],
     "dr_gemm_plane_cache": [_i],
     "dr_debug_gemm": [_p, _p, _p, _i64, _i64, _i64, _i, _i, _p],
+    "dr_debug_gemm_epi": [_p, _p, _p, _i64, _i64, _i64, _i, _i, _i64, _i, _i, _p, _p, _i, _p],
     "dr_embed_fm_fwd": [_p, _p, _p, _p, _i, _p, _i64, _i, _i, _i64, _i64, _i, _p, _p, _p, _p],
     "dr_embed_fm_fwd_tma": [_p, _i64, _p, _p, _p, _i, _p, _i64, _i, _i, _i64, _p, _p, _p, _p],
     "dr_embed_fm_bwd": [_p, _i, _p, _p, _p, _p, _p, _i64, _i, _i, _i64, _i64, _i, _p, _p, _p, _f, _p],

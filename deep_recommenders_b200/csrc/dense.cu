@@ -541,3 +541,14 @@ extern "C" int dr_debug_gemm(const float* A, const float* B, float* C, int64_t M
   GemmArgs a = mk(A, B, C, M, N, K, transA ? M : K, transB ? K : N, N, EPI_STORE);
   return gemm_launch(a, transA != 0, transB != 0, (cudaStream_t)stream);
 }
+
+extern "C" int dr_debug_gemm_epi(const float* A, const float* B, float* C, int64_t M, int64_t N, int64_t K, int transA,
+                                 int transB, int64_t ldc, int epi, int act, const float* bias, const float* aux0,
+                                 int splitk, void* stream) {
+  DR_REQUIRE(ldc >= N && (epi == EPI_STORE || epi == EPI_BIAS_ACT || epi == EPI_ATOMIC || epi == EPI_ACTGRAD) &&
+                 splitk >= 1 && (splitk == 1 || epi == EPI_ATOMIC),
+             DR_EINVAL, "dr_debug_gemm_epi: bad ldc / epi / splitk");
+  GemmArgs a = mk(A, B, C, M, N, K, transA ? M : K, transB ? K : N, ldc, epi);
+  a.act = act; a.bias = bias; a.aux0 = aux0; a.splitk = splitk;
+  return gemm_launch(a, transA != 0, transB != 0, (cudaStream_t)stream);
+}

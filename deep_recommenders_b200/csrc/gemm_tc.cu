@@ -8,8 +8,11 @@
 //
 // Structure (one 128 x BN output tile per work item, persistent grid, 416 threads, sm_90a only):
 //   warps 0-7   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async.m64n{BN}k8.tf32 (accumulator in
-//               registers) x 4 k-steps x 3 products per k-block, then the fused epilogue (gemm.cuh Epi modes) straight
-//               from the accumulator registers (float2 stores / split-K reductions).  Variant 2: each thread loads its
+//               registers) x 4 k-steps x 3 products per k-block, then the fused epilogue (gemm.cuh Epi modes).  The
+//               modes whose only output is C write the warpgroup's 64 x BN results into a shared-memory staging tile
+//               that one thread stores with TMA (a TMA reduce-add for split-K), so the warpgroup goes on to the next
+//               tile's MMAs while the tile drains; the others, and C that TMA cannot address, store float2 / issue
+//               split-K reductions straight from the accumulator registers.  Variant 2: each thread loads its
 //               A-fragment elements from the raw A tile, splits them in registers and passes them to wgmma as a
 //               register fragment; B comes from the plane ring.  Variant 1: both operands from the plane ring.
 //   warps 8-11  splitters (variant 2): turn every staged raw fp32 B tile into its hi and lo planes in the layout wgmma
@@ -64,6 +67,7 @@ constexpr int TC_SPLITTERS = 128;
 constexpr int TC_THREADS = TC_CONSUMERS + TC_SPLITTERS + 32;
 constexpr int TC_WP_THREADS = TC_CONSUMERS + 32;   // weight-plane kernel: consumers + TMA warp
 constexpr int TC_PLANE_STAGES = 2;
+constexpr int TC_RAW_STAGES = 3;                   // raw ring depth of the splitter kernels (2 when shared)
 constexpr int TC_MAX_RAW_STAGES = 4;
 constexpr int TC_WP_STAGES = 4;                    // ring depth of the weight-plane kernel
 
@@ -95,6 +99,21 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
+}
+// Shared -> global TMA store of one box, or its element-wise add into global memory; one bulk group per call site.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* smem_src, int c0, int c1, bool add) {
+  if (add)
+    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(tm), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
+  else
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(tm), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -325,6 +344,19 @@ __device__ __forceinline__ void st_pair(float* p, const float2 v, const bool two
   }
 }
 
+// Staging tile of one consumer warpgroup: its 64 x BN results as BN / 32 boxes of 64 rows x 32 floats, each box in the
+// TMA SWIZZLE_128B layout (16-B chunk c of row r at r * 128 + ((c ^ (r & 7)) << 4)), 8 KB apart; the base is 1024-B
+// aligned.  `stg_frag_addr`: address of the thread's float2 at d[4 j + 2 h], from `stg` = the tile's row 16 w of warp w
+// of the warpgroup.  A warp's store of one (h, j) covers 8 rows (lane / 4, so r & 7 = lane / 4) x 8 columns: lane pairs (lane % 4 = 0, 1 and 2, 3) fill chunks 2 (j % 4) and
+// 2 (j % 4) + 1 of their row, XORed with r & 7.  Rows r and r ^ 1 land on the same chunk pair and the other three pairs
+// of rows on the three other pairs, so every bank takes exactly two of the 256 bytes: two wavefronts, the least for a
+// 256-B store.
+__device__ __forceinline__ uint32_t stg_frag_addr(const uint32_t stg, const int lane, const int h, const int j) {
+  const uint32_t r = (uint32_t)(lane >> 2) + 8u * (uint32_t)h;
+  const uint32_t chunk = (uint32_t)(2 * (j & 3) + ((lane >> 1) & 1)) ^ (uint32_t)(lane >> 2);
+  return stg + (uint32_t)(j >> 2) * 8192u + r * 128u + (chunk << 4) + (uint32_t)(lane & 1) * 8u;
+}
+
 // Fused epilogue of one warpgroup's 64 x BN accumulator in one epilogue mode EPI (and activation ACT), both fixed at
 // compile time, so the whole fragment is straight-line code.  Fragment layout of wgmma's D: warp w of the warpgroup owns
 // rows 16 w .. 16 w + 15; d[4 j + {0, 1}] are columns 8 j + 2 (lane % 4) + {0, 1} of row lane / 4, d[4 j + {2, 3}] the
@@ -333,14 +365,19 @@ __device__ __forceinline__ void st_pair(float* p, const float2 v, const bool two
 // loaded before any arithmetic on it, so their latencies overlap; G is small enough that the loads fit beside the
 // accumulators without spilling.  Each element's arithmetic is that of the FFMA kernel's epi_scalar (gemm.cu), operation
 // for operation, so both kernels round alike.
-template <int BN, int EPI, int ACT, bool VEC>
+// STAGED: the results go to the warpgroup's staging tile at shared address `stg` instead of global memory (EPI_ATOMIC:
+// the bare accumulators, which a TMA reduce-add then adds into C); EPI_ACTGRAD reads aux0 from the same place, where the
+// producer has loaded it, and overwrites it in place.  The arithmetic is the same.
+template <int BN, int EPI, int ACT, bool VEC, bool STAGED = false>
 __device__ __forceinline__ void tc_epilogue_mode(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw,
-                                                 const int64_t n0, const int lane) {
+                                                 const int64_t n0, const int lane, const uint32_t stg = 0) {
   constexpr int G = (EPI == EPI_CROSS || EPI == EPI_CROSS_DX || EPI == EPI_SCORES) ? 2 : 4;
   constexpr bool BIAS = EPI == EPI_BIAS_ACT || EPI == EPI_CROSS || EPI == EPI_SCORES;
   constexpr bool AUX0 = EPI == EPI_ACTGRAD || EPI == EPI_CROSS || EPI == EPI_CROSS_DX;
   constexpr bool AUX1 = EPI == EPI_CROSS || EPI == EPI_CROSS_DX;
   static_assert((BN / 8) % G == 0, "column groups must tile the fragment");
+  static_assert(!STAGED || EPI == EPI_STORE || EPI == EPI_BIAS_ACT || EPI == EPI_ACTGRAD || EPI == EPI_ATOMIC,
+                "staged modes write C only");
   const int64_t nl = n0 + 2 * (lane & 3);
   int64_t m[2], row[2];
   bool row_ok[2];
@@ -378,8 +415,12 @@ __device__ __forceinline__ void tc_epilogue_mode(const GemmArgs& a, const float 
       }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if constexpr (AUX0) x0[h][g] = row_ok[h] && col_ok ? ld_pair<VEC>(a.aux0 + row[h] + 8 * (j0 + g), two)
-                                                           : make_float2(0.f, 0.f);
+        if constexpr (AUX0 && STAGED) {   // EPI_ACTGRAD: the producer has loaded aux0's tile into the staging tile
+          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x0[h][g].x), "=f"(x0[h][g].y)
+                       : "r"(stg_frag_addr(stg, lane, h, j0 + g)) : "memory");
+        } else if constexpr (AUX0) {
+          x0[h][g] = row_ok[h] && col_ok ? ld_pair<VEC>(a.aux0 + row[h] + 8 * (j0 + g), two) : make_float2(0.f, 0.f);
+        }
         if constexpr (AUX1) x1[h][g] = row_ok[h] && col_ok ? ld_pair<VEC>(a.aux1 + row[h] + 8 * (j0 + g), two)
                                                            : make_float2(0.f, 0.f);
       }
@@ -402,9 +443,11 @@ __device__ __forceinline__ void tc_epilogue_mode(const GemmArgs& a, const float 
         float* c = a.C + off;
         float2 r = make_float2(v0, v1);
         if constexpr (EPI == EPI_ATOMIC) {
-          red_add_f32(c, v0);
-          if (two) red_add_f32(c + 1, v1);
-          continue;
+          if constexpr (!STAGED) {
+            red_add_f32(c, v0);
+            if (two) red_add_f32(c + 1, v1);
+            continue;
+          }
         } else if constexpr (EPI == EPI_BIAS_ACT) {
           r = make_float2(act_apply(v0 + bv[g].x, ACT), act_apply(v1 + bv[g].y, ACT));
         } else if constexpr (EPI == EPI_ACTGRAD) {
@@ -432,27 +475,34 @@ __device__ __forceinline__ void tc_epilogue_mode(const GemmArgs& a, const float 
           if (rmask[h] && q != n && cid[g][0] == rid[h]) r.x = r.x + (-FLT_MAX / 100.0f);
           if (rmask[h] && q != n + 1 && cid[g][1] == rid[h]) r.y = r.y + (-FLT_MAX / 100.0f);
         }
-        st_pair<VEC>(c, r, two);
+        if constexpr (STAGED) {
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stg_frag_addr(stg, lane, h, j)), "f"(r.x), "f"(r.y)
+                       : "memory");
+        } else {
+          st_pair<VEC>(c, r, two);
+        }
       }
     }
   }
 }
 
-template <int BN, int EPI, int ACT>
+template <int BN, int EPI, int ACT, bool STAGED = false>
 __device__ __forceinline__ void tc_epilogue_vec(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw,
-                                                const int64_t n0, const int lane, const bool vec_ok) {
-  if (vec_ok) tc_epilogue_mode<BN, EPI, ACT, true>(a, d, mw, n0, lane);
-  else tc_epilogue_mode<BN, EPI, ACT, false>(a, d, mw, n0, lane);
+                                                const int64_t n0, const int lane, const bool vec_ok,
+                                                const uint32_t stg = 0) {
+  if (vec_ok) tc_epilogue_mode<BN, EPI, ACT, true, STAGED>(a, d, mw, n0, lane, stg);
+  else tc_epilogue_mode<BN, EPI, ACT, false, STAGED>(a, d, mw, n0, lane, stg);
 }
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool STAGED = false>
 __device__ __forceinline__ void tc_epilogue_act(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw,
-                                                const int64_t n0, const int lane, const bool vec_ok) {
+                                                const int64_t n0, const int lane, const bool vec_ok,
+                                                const uint32_t stg = 0) {
   switch (a.act) {
-    case DR_ACT_RELU: tc_epilogue_vec<BN, EPI, DR_ACT_RELU>(a, d, mw, n0, lane, vec_ok); return;
-    case DR_ACT_SIGMOID: tc_epilogue_vec<BN, EPI, DR_ACT_SIGMOID>(a, d, mw, n0, lane, vec_ok); return;
-    case DR_ACT_TANH: tc_epilogue_vec<BN, EPI, DR_ACT_TANH>(a, d, mw, n0, lane, vec_ok); return;
-    default: tc_epilogue_vec<BN, EPI, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
+    case DR_ACT_RELU: tc_epilogue_vec<BN, EPI, DR_ACT_RELU, STAGED>(a, d, mw, n0, lane, vec_ok, stg); return;
+    case DR_ACT_SIGMOID: tc_epilogue_vec<BN, EPI, DR_ACT_SIGMOID, STAGED>(a, d, mw, n0, lane, vec_ok, stg); return;
+    case DR_ACT_TANH: tc_epilogue_vec<BN, EPI, DR_ACT_TANH, STAGED>(a, d, mw, n0, lane, vec_ok, stg); return;
+    default: tc_epilogue_vec<BN, EPI, DR_ACT_NONE, STAGED>(a, d, mw, n0, lane, vec_ok, stg); return;
   }
 }
 
@@ -470,6 +520,19 @@ __device__ __forceinline__ void tc_epilogue(const GemmArgs& a, const float (&d)[
     case EPI_CROSS_DX: tc_epilogue_vec<BN, EPI_CROSS_DX, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
     case EPI_SCORES: tc_epilogue_vec<BN, EPI_SCORES, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
     default: tc_epilogue_vec<BN, EPI_STORE, DR_ACT_NONE>(a, d, mw, n0, lane, vec_ok); return;
+  }
+}
+
+// The modes whose only output is C (tc_staged_ok) write the warpgroup's staging tile at `stg`.
+template <int BN>
+__device__ __forceinline__ void tc_epilogue_staged(const GemmArgs& a, const float (&d)[BN / 2], const int64_t mw,
+                                                   const int64_t n0, const int lane, const bool vec_ok,
+                                                   const uint32_t stg) {
+  switch (a.epi) {
+    case EPI_BIAS_ACT: tc_epilogue_act<BN, EPI_BIAS_ACT, true>(a, d, mw, n0, lane, vec_ok, stg); return;
+    case EPI_ATOMIC: tc_epilogue_mode<BN, EPI_ATOMIC, DR_ACT_NONE, false, true>(a, d, mw, n0, lane, stg); return;
+    case EPI_ACTGRAD: tc_epilogue_act<BN, EPI_ACTGRAD, true>(a, d, mw, n0, lane, vec_ok, stg); return;
+    default: tc_epilogue_mode<BN, EPI_STORE, DR_ACT_NONE, false, true>(a, d, mw, n0, lane, stg); return;
   }
 }
 
@@ -496,16 +559,24 @@ __device__ __forceinline__ void tc_epilogue_acc(const GemmArgs& a, const float (
 
 // Shared-memory stages of one tile width.  The plane ring holds [Ah | Al | Bh | Bl] in variant 1 and [Bh | Bl] in
 // variant 2, whose consumers split A in registers; the raw ring (variant 2 only) holds [A raw | B raw], or
-// [A raw | Bh | Bl] in the weight-plane kernel, which has no plane ring.
+// [A raw | Bh | Bl] in the weight-plane kernel, which has no plane ring.  A launch with the staged epilogue adds the
+// 128 x BN staging tile after the rings.  MAX_RAW: the deepest raw ring launched; STAGED_RAW: the deepest that leaves
+// room for the staging tile (3 for the weight-plane kernel at BN = 128, whose 4-deep ring takes 192 KB).
+constexpr size_t TC_SMEM_LIMIT = 232448;   // 227 KB of shared memory per CTA
+constexpr size_t TC_STATIC_SMEM = 2048;     // the barriers: ptxas pads them to 1 KB granules ahead of the ring
 template <int BN, bool PRESPLIT, bool WPLANES = false>
 struct TcSmem {
   static constexpr int A_TILE = TC_BM * TC_BK * 4;   // 16 KB
   static constexpr int B_TILE = BN * TC_BK * 4;
+  static constexpr int STG = TC_BM * BN * 4;
   static constexpr int PLANE_STAGE = WPLANES ? 0 : (PRESPLIT ? 2 * A_TILE : 0) + 2 * B_TILE;
   static constexpr int RAW_STAGE = PRESPLIT ? 0 : A_TILE + (WPLANES ? 2 : 1) * B_TILE;
-  static constexpr size_t bytes(int raw_stages) {   // + 1024: the ring base is rounded up to 1024 B
-    return (size_t)TC_PLANE_STAGES * PLANE_STAGE + (size_t)raw_stages * RAW_STAGE + 1024;
+  static constexpr int MAX_RAW = PRESPLIT ? 0 : (WPLANES ? TC_WP_STAGES : TC_RAW_STAGES);
+  static constexpr size_t bytes(int raw_stages, bool staged) {   // + 1024: the ring base is rounded up to 1024 B
+    return (size_t)TC_PLANE_STAGES * PLANE_STAGE + (size_t)raw_stages * RAW_STAGE + (staged ? STG : 0) + 1024;
   }
+  // + TC_STATIC_SMEM: the static shared memory beside the dynamic ring
+  static constexpr int STAGED_RAW = bytes(MAX_RAW, true) + TC_STATIC_SMEM <= TC_SMEM_LIMIT ? MAX_RAW : MAX_RAW - 1;
 };
 
 // A consumer thread's A-fragment elements in the raw A stage.  `a_frag_base`: byte offset of element 0 of k-step 0 (row
@@ -543,9 +614,10 @@ struct TcWidth { static constexpr int value = N; };
 // (tmBh / tmBl); the threads are the consumers and the TMA warp only.
 template <int BN, bool A_MN, bool B_MN, bool PRESPLIT, bool ACC, bool WPLANES = false>
 __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUtensorMap& tmAl, const CUtensorMap& tmBh,
-                                             const CUtensorMap& tmBl, const GemmArgs& a, const int raw_stages,
-                                             const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
-                                             const int64_t total_items) {
+                                             const CUtensorMap& tmBl, const CUtensorMap& tmC, const CUtensorMap& tmAux,
+                                             const GemmArgs& a,
+                                             const int raw_stages, const int staged, const int64_t m_tiles,
+                                             const int64_t n_tiles, const int64_t per, const int64_t total_items) {
   static_assert(!WPLANES || (!PRESPLIT && !A_MN && !B_MN && !ACC), "weight planes: K-major A split in registers");
   using S = TcSmem<BN, PRESPLIT, WPLANES>;
   constexpr int A_TILE = S::A_TILE, B_TILE = S::B_TILE, PLANE_STAGE = S::PLANE_STAGE, RAW_STAGE = S::RAW_STAGE;
@@ -553,8 +625,13 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* planes = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* raws = planes + TC_PLANE_STAGES * PLANE_STAGE;
+  uint8_t* stage_tile = raws + (size_t)raw_stages * RAW_STAGE;   // staged epilogue: 64 x BN per consumer warpgroup
   __shared__ __align__(8) uint64_t raw_full[TC_MAX_RAW_STAGES], raw_empty[TC_MAX_RAW_STAGES],
       pl_full[TC_PLANE_STAGES], pl_empty[TC_PLANE_STAGES];
+  // staged EPI_ACTGRAD, per consumer warpgroup: aux0's tile has landed in the staging tile / the TMA store of the
+  // previous tile has read it
+  __shared__ __align__(8) uint64_t aux_full[2], stg_free[2];
+  const bool aux_tma = staged && a.epi == EPI_ACTGRAD;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t kblocks = (a.K + TC_BK - 1) / TC_BK;
@@ -569,6 +646,10 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
       mbar_init(&pl_full[s], PRESPLIT ? 1 : TC_SPLITTERS);
       mbar_init(&pl_empty[s], TC_CONSUMERS);         // every consumer thread arrives
     }
+    for (int w = 0; w < 2; ++w) {
+      mbar_init(&aux_full[w], 1);                    // the producer's expect_tx arrival
+      mbar_init(&stg_free[w], 1);                    // the warpgroup's leader, once its store has read the tile
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
@@ -580,9 +661,24 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAh) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBh) : "memory");
       if (WPLANES) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBl) : "memory");
-      uint32_t it = 0;
+      uint32_t it = 0, aux_it[2] = {0, 0};
       for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
         const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
+        // staged EPI_ACTGRAD: aux0's 64 x BN block of each warpgroup with rows in range, behind the tile's last k-block
+        // (by then the consumers are past the previous tile's epilogue), once the warpgroup's previous store has read
+        // the staging tile
+        auto load_aux = [&]() {
+          const int boxes = (int)min((int64_t)(BN / 32), (a.N - t.n0 + 31) / 32);
+          for (int w = 0; w < 2; ++w) {
+            if (t.m0 + 64 * w >= a.M) continue;
+            mbar_wait(&stg_free[w], (aux_it[w] & 1u) ^ 1u);
+            ++aux_it[w];
+            mbar_expect_tx(&aux_full[w], (uint32_t)boxes * (64u * 128u));
+            for (int q = 0; q < boxes; ++q)
+              tma_load_2d(stage_tile + (size_t)w * (64 * BN * 4) + q * (64 * 128), &tmAux, &aux_full[w],
+                          (int)(t.n0 + 32 * q), (int)(t.m0 + 64 * w));
+          }
+        };
         for (int i = 0; i < t.nkb; ++i, ++it) {
           const int k = (t.kb0 + i) * TC_BK;
           if (PRESPLIT) {      // K-major planes from the workspace straight into the plane ring
@@ -605,6 +701,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
             else tma_load_2d(st + A_TILE, &tmBh, &raw_full[s], (int)t.n0, k);
             if (WPLANES) tma_load_2d(st + A_TILE + B_TILE, &tmBl, &raw_full[s], k, (int)t.n0);
           }
+          if (aux_tma && i + 1 == t.nkb) load_aux();
         }
       }
     }
@@ -635,7 +732,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
                         (((reinterpret_cast<uintptr_t>(a.C) | reinterpret_cast<uintptr_t>(a.bias) |
                            reinterpret_cast<uintptr_t>(a.aux0) | reinterpret_cast<uintptr_t>(a.aux1) |
                            reinterpret_cast<uintptr_t>(a.out2)) & 7u) == 0);
-    uint32_t it = 0;
+    uint32_t it = 0, aux_it = 0;
     for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
       const TcItem t = tc_decode(item, n_tiles, m_tiles, kblocks, per, BN);
       if (t.m0 + wg * 64 >= a.M) {
@@ -735,9 +832,36 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
       wgmma_wait<0>();
       if (WPLANES) mbar_arrive(&raw_empty[(it - 1) % (uint32_t)raw_stages]);
       else mbar_arrive(&pl_empty[(it - 1) % TC_PLANE_STAGES]);
-      if constexpr (ACC) tc_epilogue_acc<BN>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane);
-      else tc_epilogue<BN>(a, d, t.m0 + wg * 64 + (warp & 3) * 16, t.n0, lane, vec_ok);
+      const int64_t mw = t.m0 + wg * 64 + (warp & 3) * 16;
+      if constexpr (ACC) {
+        tc_epilogue_acc<BN>(a, d, mw, t.n0, lane);
+      } else if (staged) {
+        // Staged epilogue: the warpgroup writes its 64 x BN results into its staging tile and one thread hands the
+        // tile to TMA (a store, or a reduce-add for split-K), which drains it while the warpgroup runs the next tile's
+        // MMAs.  The tile is rewritten only after the previous tile's TMA has finished reading it.
+        const bool leader = (threadIdx.x & 127) == 0;
+        uint8_t* stg = stage_tile + (size_t)wg * (64 * BN * 4);
+        if (leader) bulk_wait_read0();
+        named_barrier_sync(1 + wg, 128);
+        if (aux_tma) mbar_wait(&aux_full[wg], (aux_it++) & 1u);
+        tc_epilogue_staged<BN>(a, d, mw, t.n0, lane, vec_ok, smem_u32(stg) + (uint32_t)(warp & 3) * (16u * 128u));
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to TMA
+        named_barrier_sync(1 + wg, 128);
+        if (leader) {
+          // TMA clips the rows past M and the columns past N; a box wholly past N is not issued
+          for (int q = 0; q < BN / 32 && t.n0 + 32 * q < a.N; ++q)
+            tma_store_2d(&tmC, stg + q * (64 * 128), (int)(t.n0 + 32 * q), (int)(t.m0 + 64 * wg), a.epi == EPI_ATOMIC);
+          bulk_commit();
+          if (aux_tma) {   // the producer loads the next tile's aux0 block here
+            bulk_wait_read0();
+            mbar_arrive(&stg_free[wg]);
+          }
+        }
+      } else {
+        tc_epilogue<BN>(a, d, mw, t.n0, lane, vec_ok);
+      }
     }
+    if (staged && (threadIdx.x & 127) == 0) bulk_wait0();
   }
 }
 
@@ -747,20 +871,24 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmAh, const CUte
 template <int BN, bool A_MN, bool B_MN, bool PRESPLIT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-               const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const GemmArgs a,
-               const int raw_stages, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
+               const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
+               const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAux, const GemmArgs a,
+               const int raw_stages, const int staged, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
                const int64_t total_items) {
-  gemm_tc_body<BN, A_MN, B_MN, PRESPLIT, false>(tmAh, tmAl, tmBh, tmBl, a, raw_stages, m_tiles, n_tiles, per, total_items);
+  gemm_tc_body<BN, A_MN, B_MN, PRESPLIT, false>(tmAh, tmAl, tmBh, tmBl, tmC, tmAux, a, raw_stages, staged, m_tiles, n_tiles, per,
+                                                total_items);
 }
 
 // EPI_CROSS_DX_ACC: the only GEMM that accumulates into C is the Cross input gradient h @ W^T, both operands K-major.
 template <int BN, bool PRESPLIT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_acc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-                   const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const GemmArgs a,
-                   const int raw_stages, const int64_t m_tiles, const int64_t n_tiles, const int64_t per,
-                   const int64_t total_items) {
-  gemm_tc_body<BN, false, false, PRESPLIT, true>(tmAh, tmAl, tmBh, tmBl, a, raw_stages, m_tiles, n_tiles, per, total_items);
+                   const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
+                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAux,
+                   const GemmArgs a, const int raw_stages, const int staged, const int64_t m_tiles,
+                   const int64_t n_tiles, const int64_t per, const int64_t total_items) {
+  gemm_tc_body<BN, false, false, PRESPLIT, true>(tmAh, tmAl, tmBh, tmBl, tmC, tmAux, a, raw_stages, 0, m_tiles, n_tiles, per,
+                                                 total_items);
 }
 
 // Weight planes: K-major raw A (tmAh) split in registers, B's K-major hi / lo planes (tmBh / tmBl) from the workspace.
@@ -769,10 +897,11 @@ template <int BN>
 __global__ void __launch_bounds__(TC_WP_THREADS, 1)
 gemm_tc_wplanes_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                        const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-                       const GemmArgs a, const int raw_stages, const int64_t m_tiles, const int64_t n_tiles,
-                       const int64_t per, const int64_t total_items) {
-  gemm_tc_body<BN, false, false, false, false, true>(tmAh, tmAl, tmBh, tmBl, a, raw_stages, m_tiles, n_tiles, per,
-                                                     total_items);
+                       const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAux,
+                       const GemmArgs a, const int raw_stages, const int staged, const int64_t m_tiles,
+                       const int64_t n_tiles, const int64_t per, const int64_t total_items) {
+  gemm_tc_body<BN, false, false, false, false, true>(tmAh, tmAl, tmBh, tmBl, tmC, tmAux, a, raw_stages, staged, m_tiles,
+                                                     n_tiles, per, total_items);
 }
 
 // ---- host side ---------------------------------------------------------------------------------------
@@ -861,17 +990,36 @@ bool gemm_tc_eligible(const GemmArgs& a, bool ta, bool tb) {
 int g_tune_tc_stages = 0;    // 0 = three raw stages; 2 = two (32 KB less shared memory at the widest tile)
 int g_tune_tc_pair = 1;      // accepted and read back for callers that set it; H100 has no two-CTA MMA, so it selects nothing
 
+// The staged epilogue serves the modes whose only output is C, when TMA can address C (16-B aligned base, ldc % 4 == 0).
+// EPI_ACTGRAD's aux0 (pitch ldc, as C) is loaded by TMA into the staging tile, so it must be 16-B aligned too.
+static bool tc_staged_ok(const GemmArgs& a) {
+  return (a.epi == EPI_STORE || a.epi == EPI_BIAS_ACT || a.epi == EPI_ACTGRAD || a.epi == EPI_ATOMIC) &&
+         aligned16(a.C) && (a.ldc & 3) == 0 && (a.epi != EPI_ACTGRAD || aligned16(a.aux0));
+}
+
+// `tms`: the operand maps [Ah, Al, Bh, Bl] and room for C's and aux0's.  `raw_stages`: the ring depth of the register epilogue.
+// A splitter kernel with the two-stage ring (it runs beside another kernel) keeps the register epilogue and its smaller
+// shared-memory footprint; the weight-plane kernel gives up a ring stage for the staging tile where both do not fit.
 template <int BN, bool A_MN, bool B_MN, bool PRESPLIT, bool WPLANES = false>
-static int launch_tc(const CUtensorMap* tms, const GemmArgs& a, int raw_stages, cudaStream_t st) {
+static int launch_tc(CUtensorMap* tms, const GemmArgs& a, int raw_stages, cudaStream_t st) {
   using S = TcSmem<BN, PRESPLIT, WPLANES>;
-  const size_t smem = S::bytes(raw_stages);
-  static_assert(S::bytes(TC_MAX_RAW_STAGES) + 256 <= 232448,
-                "plane ring + raw ring exceed the 227 KB of shared memory per CTA");
+  static_assert(S::bytes(S::MAX_RAW, false) + TC_STATIC_SMEM <= TC_SMEM_LIMIT &&
+                    S::bytes(S::STAGED_RAW, true) + TC_STATIC_SMEM <= TC_SMEM_LIMIT,
+                "the rings and the staging tile exceed the 227 KB of shared memory per CTA");
   auto k = gemm_tc_kernel<BN, A_MN, B_MN, PRESPLIT>;
   if constexpr (WPLANES) k = gemm_tc_wplanes_kernel<BN>;
   if constexpr (!A_MN && !B_MN && BN <= 64 && !WPLANES) {
     if (a.epi == EPI_CROSS_DX_ACC) k = gemm_tc_acc_kernel<BN, PRESPLIT>;
   }
+  const bool staged = tc_staged_ok(a) && raw_stages != 2;
+  if (staged) {
+    raw_stages = raw_stages < S::STAGED_RAW ? raw_stages : S::STAGED_RAW;
+    // boxes of 64 rows x 32 floats (one warpgroup's rows, one 128-B swizzle row), in the staging tile's layout
+    if (int rc = make_map(&tms[4], a.C, a.N, a.M, a.ldc, 32, 64, true)) return rc;
+    if (a.epi == EPI_ACTGRAD)
+      if (int rc = make_map(&tms[5], a.aux0, a.N, a.M, a.ldc, 32, 64, true)) return rc;
+  }
+  const size_t smem = S::bytes(raw_stages, staged);
   DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t m_tiles = (a.M + TC_BM - 1) / TC_BM, n_tiles = (a.N + BN - 1) / BN;
   const int64_t kblocks = (a.K + TC_BK - 1) / TC_BK;
@@ -879,8 +1027,9 @@ static int launch_tc(const CUtensorMap* tms, const GemmArgs& a, int raw_stages, 
   const int64_t splits = (kblocks + per - 1) / per;          // every split owns >= 1 k-block
   const int64_t total = m_tiles * n_tiles * splits;
   const int64_t ctas = total < (int64_t)num_sms() ? total : (int64_t)num_sms();
-  k<<<(unsigned)ctas, WPLANES ? TC_WP_THREADS : TC_THREADS, smem, st>>>(tms[0], tms[1], tms[2], tms[3], a, raw_stages,
-                                                                         m_tiles, n_tiles, per, total);
+  k<<<(unsigned)ctas, WPLANES ? TC_WP_THREADS : TC_THREADS, smem, st>>>(tms[0], tms[1], tms[2], tms[3], tms[4], tms[5], a,
+                                                                         raw_stages, staged ? 1 : 0, m_tiles, n_tiles,
+                                                                         per, total);
   DR_CUDA_LAUNCH_CHECK("gemm_tc");
   return DR_OK;
 }
@@ -921,7 +1070,7 @@ int gemm_tc_launch(const GemmArgs& a0, bool ta, bool tb, cudaStream_t st) {
   // the accumulating epilogue holds three addresses per element: beside the 64 accumulators of a 128-wide tile it does not
   // fit the 128-register cap without spilling, so it runs 128 x 64 tiles at most
   if (a.epi == EPI_CROSS_DX_ACC && bn == 128) bn = 64;
-  CUtensorMap tms[4];
+  CUtensorMap tms[6] = {};
   size_t ae, be;
   plane_elems(a, ta, tb, &ae, &be);
   auto planes = [&](const float* src, size_t elems, bool transposed, int64_t rows, int64_t ld, float** hi, float** lo,
@@ -965,7 +1114,7 @@ int gemm_tc_launch(const GemmArgs& a0, bool ta, bool tb, cudaStream_t st) {
   if (g_tune_gemm_variant == 2) {
     // Variant 2: tensor maps straight on the source operands (staged as stored), split in shared memory.
     const bool A_MN = ta, B_MN = !tb;
-    const int raw_stages = (g_tune_tc_stages == 2 || a.stages == 2 || a.share) ? 2 : 3;
+    const int raw_stages = (g_tune_tc_stages == 2 || a.stages == 2 || a.share) ? 2 : TC_RAW_STAGES;
     if (!A_MN) {
       if (int rc = make_map(&tms[0], a.A, a.K, a.M, a.lda, TC_BK, TC_BM, true)) return rc;
     } else {

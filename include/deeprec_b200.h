@@ -849,6 +849,13 @@ int dr_tune_get(const char* key, int* value);
 int dr_debug_gemm(const float* A, const float* B, float* C, int64_t M, int64_t N, int64_t K,
                   int transA, int transB, void* stream);
 
+/* Developer hook: the same GEMM with a fused epilogue and C's row pitch ldc (>= N):
+ *   epi 0: C = acc;  1: C = act(acc + bias[n]);  2: C += acc (split-K over `splitk` parts, C pre-set by the caller);
+ *   3: C = acc * act'(aux0[m, n]) (aux0 has pitch ldc). */
+int dr_debug_gemm_epi(const float* A, const float* B, float* C, int64_t M, int64_t N, int64_t K,
+                      int transA, int transB, int64_t ldc, int epi, int act, const float* bias,
+                      const float* aux0, int splitk, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
