@@ -18,70 +18,9 @@
 // of EVERY row each step and moves every row by its decayed momentum (dr_adam_step over the arena is that exact form, at
 // 7 arena sweeps per step); this is the documented deviation of the row-sparse form.  On the rows a step touches the
 // update is TensorFlow's functor exactly.
-#include "common.cuh"
+#include "adam.cuh"
 
 namespace dr {
-
-__device__ __forceinline__ void adam_functor(float& p, float g, float& m, float& v, float lr_t, float omb1, float omb2,
-                                             float eps) {
-  // training_ops ApplyAdam: m += (g - m)(1 - b1); v += (g*g - v)(1 - b2); var -= lr_t * m / (sqrt(v) + eps)
-  m += (g - m) * omb1;
-  v += (g * g - v) * omb2;
-  p -= (m * lr_t) / (sqrtf(v) + eps);
-}
-
-__host__ __device__ inline int adam_state_stride(int D) { return (3 * D + 5 + 31) / 32 * 32; }   // + count + step stamp
-
-__device__ __forceinline__ float4 ld_cg4(const float* p) {
-  float4 r;
-  asm volatile("ld.global.cg.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p) : "memory");
-  return r;
-}
-__device__ __forceinline__ float ld_cg1(const float* p) {
-  float r;
-  asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(r) : "l"(p) : "memory");
-  return r;
-}
-
-// ---- exact tf.keras Adam for rows that were NOT touched for a while (EXACT mode) ---------------------------------------
-// TensorFlow's Adam is dense: in a step that does not touch a row, m <- m - m(1-b1), v <- v - v(1-b2) and the row still
-// moves by -lr_j m / (sqrt(v) + eps).  The row-sparse form replays those skipped steps when the row is next touched (or
-// flushed): per-row stamp = last step whose update the row has seen; lr_j comes from the history dr_adam_advance_hist
-// keeps (ring of `hist_len` bias-corrected rates), or is recomputed when the step fell out of the ring.  Steps beyond
-// kCatchUpMax after the stamp cannot move the row any more (m has decayed by 0.9^2048, far below fp32's range relative to
-// v): they only decay v, in closed form.
-constexpr int kCatchUpMax = 2048;
-struct AdamHist {
-  const float* lr_hist;
-  int hist_len;
-  float lr, b1, b2;
-};
-__device__ __forceinline__ float adam_lr_at(const AdamHist& h, int64_t j, int64_t t_now) {
-  if (h.lr_hist && t_now - j < h.hist_len) return __ldg(h.lr_hist + (j % h.hist_len));
-  return h.lr * sqrtf(1.f - powf(h.b2, (float)j)) / (1.f - powf(h.b1, (float)j));
-}
-// N elements of one lane: replay steps (stamp, upto] with zero gradient
-template <int N>
-__device__ __forceinline__ void adam_catch_up(float (&p)[N], float (&m)[N], float (&v)[N], int64_t stamp, int64_t upto,
-                                              int64_t t_now, const AdamHist& h, float omb1, float omb2, float eps) {
-  if (stamp <= 0 || upto <= stamp) return;                    // never updated (m = v = 0): nothing to replay
-  const int64_t gap = upto - stamp;
-  const int n = (int)(gap < kCatchUpMax ? gap : kCatchUpMax);
-  for (int k = 1; k <= n; ++k) {
-    const float lr_j = adam_lr_at(h, stamp + k, t_now);
-#pragma unroll
-    for (int e = 0; e < N; ++e) {
-      m[e] = fmaf(-m[e], omb1, m[e]);
-      v[e] = fmaf(-v[e], omb2, v[e]);
-      p[e] -= __fdividef(m[e] * lr_j, sqrtf(v[e]) + eps);
-    }
-  }
-  if (gap > n) {
-    const float dm = powf(1.f - omb1, (float)(gap - n)), dv = powf(1.f - omb2, (float)(gap - n));
-#pragma unroll
-    for (int e = 0; e < N; ++e) { m[e] *= dm; v[e] *= dv; }
-  }
-}
 
 template <typename IdT>
 __global__ void __launch_bounds__(256) embed_adam_count_kernel(const IdT* __restrict__ ids, int64_t n, int S,
@@ -96,7 +35,6 @@ __global__ void __launch_bounds__(256) embed_adam_count_kernel(const IdT* __rest
       atomicAdd(reinterpret_cast<int*>(state + (size_t)(__ldg(slot_offsets + s) + id) * SS + cnt_off), 1);
   }
 }
-
 
 // EXACT, before the forward: count the batch's lookups per row (as embed_adam_count_kernel) AND bring every row the batch
 // touches up to date with step t-1, so that the forward reads what tf.keras Adam's dense update would have left there.
@@ -138,21 +76,13 @@ __global__ void __launch_bounds__(256) embed_adam_prepare_kernel(const IdT* __re
     const int64_t stamp = stamp_i;
     if (first && stamp > 0 && stamp < t_now - 1) {
       float* prow = table_ptrs[s] + (size_t)id * row_stride;
-      if (c * 4 < D) {
-        float4 m = ld_cg4(st + o_m + c * 4), v = ld_cg4(st + o_v + c * 4);
-        float4 w = *reinterpret_cast<const float4*>(prow + c * 4);
-        float pa[4] = {w.x, w.y, w.z, w.w}, ma[4] = {m.x, m.y, m.z, m.w}, va[4] = {v.x, v.y, v.z, v.w};
-        adam_catch_up<4>(pa, ma, va, stamp, t_now - 1, t_now, hist, omb1, omb2, eps);
-        *reinterpret_cast<float4*>(prow + c * 4) = make_float4(pa[0], pa[1], pa[2], pa[3]);
-        stg4(st + o_m + c * 4, make_float4(ma[0], ma[1], ma[2], ma[3]));
-        stg4(st + o_v + c * 4, make_float4(va[0], va[1], va[2], va[3]));
-      }
+      if (c * 4 < D)
+        adam_replay_chunk<LdCg>(st, o_m, o_v, prow, c * 4, stamp, t_now - 1, t_now, hist, omb1,
+                                omb2, eps);
       if (c == 0) {
         if (lin_in_row || lin_ptrs) {
           float* wp = lin_in_row ? prow + D : lin_ptrs[s] + (size_t)id * lin_stride;
-          float pa[1] = {*wp}, ma[1] = {ld_cg1(st + o_s + 1)}, va[1] = {ld_cg1(st + o_s + 2)};
-          adam_catch_up<1>(pa, ma, va, stamp, t_now - 1, t_now, hist, omb1, omb2, eps);
-          *wp = pa[0]; st[o_s + 1] = ma[0]; st[o_s + 2] = va[0];
+          adam_replay_weight<LdCg>(wp, st, o_s, stamp, t_now - 1, t_now, hist, omb1, omb2, eps);
         }
         st[o_s + 4] = __int_as_float((int)(t_now - 1));
       }
@@ -271,12 +201,8 @@ __global__ void __launch_bounds__(256) embed_fm_bwd_adam_kernel(const AdamBwdPar
           const float4 g = ld_cg4(st + c * 4);
           float4 m = ld_cg4(st + o_m + c * 4), v = ld_cg4(st + o_v + c * 4);
           float4 w = *reinterpret_cast<const float4*>(prow + c * 4);
-          if (EXACT) {     // replay the steps this row sat out, then take this step's update
-            float pa[4] = {w.x, w.y, w.z, w.w}, ma[4] = {m.x, m.y, m.z, m.w}, va[4] = {v.x, v.y, v.z, v.w};
-            adam_catch_up<4>(pa, ma, va, stamp, t_now - 1, t_now, p.hist, omb1, omb2, eps);
-            w = make_float4(pa[0], pa[1], pa[2], pa[3]); m = make_float4(ma[0], ma[1], ma[2], ma[3]);
-            v = make_float4(va[0], va[1], va[2], va[3]);
-          }
+          if (EXACT)     // replay the steps this row sat out, then take this step's update
+            adam_catch_up4(w, m, v, stamp, t_now - 1, t_now, p.hist, omb1, omb2, eps);
           adam_functor(w.x, g.x, m.x, v.x, lr_t, omb1, omb2, eps);
           adam_functor(w.y, g.y, m.y, v.y, lr_t, omb1, omb2, eps);
           adam_functor(w.z, g.z, m.z, v.z, lr_t, omb1, omb2, eps);
@@ -290,11 +216,7 @@ __global__ void __launch_bounds__(256) embed_fm_bwd_adam_kernel(const AdamBwdPar
           float* wp = p.lin_in_row ? prow + D : s_lin[s] + (size_t)id * p.lin_stride;
           float w = *wp, m = ld_cg1(st + o_s + 1), v = ld_cg1(st + o_s + 2);
           const float g = ld_cg1(st + o_s);
-          if (EXACT) {
-            float pa[1] = {w}, ma[1] = {m}, va[1] = {v};
-            adam_catch_up<1>(pa, ma, va, stamp, t_now - 1, t_now, p.hist, omb1, omb2, eps);
-            w = pa[0]; m = ma[0]; v = va[0];
-          }
+          if (EXACT) adam_catch_up1(w, m, v, stamp, t_now - 1, t_now, p.hist, omb1, omb2, eps);
           adam_functor(w, g, m, v, lr_t, omb1, omb2, eps);
           *wp = w;
           st[o_s + 1] = m;
@@ -345,20 +267,12 @@ __global__ void __launch_bounds__(256) embed_adam_flush_kernel(float* const* __r
     while (s + 1 < S && __ldg(slot_offsets + s + 1) <= r) ++s;
     const int64_t id = r - __ldg(slot_offsets + s);
     float* prow = table_ptrs[s] + (size_t)id * row_stride;
-    if (c * 4 < D) {
-      float4 m = *reinterpret_cast<float4*>(st + o_m + c * 4), v = *reinterpret_cast<float4*>(st + o_v + c * 4);
-      float4 w = *reinterpret_cast<float4*>(prow + c * 4);
-      float pa[4] = {w.x, w.y, w.z, w.w}, ma[4] = {m.x, m.y, m.z, m.w}, va[4] = {v.x, v.y, v.z, v.w};
-      adam_catch_up<4>(pa, ma, va, stamp, t_now, t_now, hist, omb1, omb2, eps);
-      *reinterpret_cast<float4*>(prow + c * 4) = make_float4(pa[0], pa[1], pa[2], pa[3]);
-      *reinterpret_cast<float4*>(st + o_m + c * 4) = make_float4(ma[0], ma[1], ma[2], ma[3]);
-      *reinterpret_cast<float4*>(st + o_v + c * 4) = make_float4(va[0], va[1], va[2], va[3]);
-    }
+    if (c * 4 < D)
+      adam_replay_chunk<LdPlain>(st, o_m, o_v, prow, c * 4, stamp, t_now, t_now, hist, omb1,
+                                 omb2, eps);
     if (c == 0 && (lin_in_row || lin_ptrs)) {
       float* wp = lin_in_row ? prow + D : lin_ptrs[s] + (size_t)id * lin_stride;
-      float pa[1] = {*wp}, ma[1] = {st[o_s + 1]}, va[1] = {st[o_s + 2]};
-      adam_catch_up<1>(pa, ma, va, stamp, t_now, t_now, hist, omb1, omb2, eps);
-      *wp = pa[0]; st[o_s + 1] = ma[0]; st[o_s + 2] = va[0];
+      adam_replay_weight<LdPlain>(wp, st, o_s, stamp, t_now, t_now, hist, omb1, omb2, eps);
     }
     if (c == 0) st[o_s + 4] = __int_as_float((int)t_now);
   }
@@ -408,20 +322,12 @@ __global__ void __launch_bounds__(256) embed_adam_catch_up_kernel(const IdT* __r
     if (!won) continue;
     const int64_t stamp = stamp_i;
     float* prow = table_ptrs[s] + (size_t)id * row_stride;
-    if (c * 4 < D) {
-      float4 m = ld_cg4(st + o_m + c * 4), v = ld_cg4(st + o_v + c * 4);
-      float4 w = *reinterpret_cast<const float4*>(prow + c * 4);
-      float pa[4] = {w.x, w.y, w.z, w.w}, ma[4] = {m.x, m.y, m.z, m.w}, va[4] = {v.x, v.y, v.z, v.w};
-      adam_catch_up<4>(pa, ma, va, stamp, t_now, t_now, hist, omb1, omb2, eps);
-      *reinterpret_cast<float4*>(prow + c * 4) = make_float4(pa[0], pa[1], pa[2], pa[3]);
-      stg4(st + o_m + c * 4, make_float4(ma[0], ma[1], ma[2], ma[3]));
-      stg4(st + o_v + c * 4, make_float4(va[0], va[1], va[2], va[3]));
-    }
+    if (c * 4 < D)
+      adam_replay_chunk<LdCg>(st, o_m, o_v, prow, c * 4, stamp, t_now, t_now, hist, omb1, omb2,
+                              eps);
     if (c == 0 && (lin_in_row || lin_ptrs)) {
       float* wp = lin_in_row ? prow + D : lin_ptrs[s] + (size_t)id * lin_stride;
-      float pa[1] = {*wp}, ma[1] = {ld_cg1(st + o_s + 1)}, va[1] = {ld_cg1(st + o_s + 2)};
-      adam_catch_up<1>(pa, ma, va, stamp, t_now, t_now, hist, omb1, omb2, eps);
-      *wp = pa[0]; st[o_s + 1] = ma[0]; st[o_s + 2] = va[0];
+      adam_replay_weight<LdCg>(wp, st, o_s, stamp, t_now, t_now, hist, omb1, omb2, eps);
     }
   }
 }
@@ -514,33 +420,14 @@ __global__ void __launch_bounds__(256) embed_adam_rows_tf_kernel(const AdamRowsP
     __threadfence();
     const int64_t stamp = stamp_i;
     float* prow = p.table_ptrs[s] + (size_t)id * p.row_stride;
-    if (chunk_ok) {
-      const float4 g = ld_cg4(st + c * 4);
-      float4 m = ld_cg4(st + o_m + c * 4), v = ld_cg4(st + o_v + c * 4);
-      float4 w = *reinterpret_cast<const float4*>(prow + c * 4);
-      float pa[4] = {w.x, w.y, w.z, w.w}, ma[4] = {m.x, m.y, m.z, m.w}, va[4] = {v.x, v.y, v.z, v.w};
-      adam_catch_up<4>(pa, ma, va, stamp, t_now - 1, t_now, p.hist, omb1, omb2, eps);
-      w = make_float4(pa[0], pa[1], pa[2], pa[3]); m = make_float4(ma[0], ma[1], ma[2], ma[3]);
-      v = make_float4(va[0], va[1], va[2], va[3]);
-      adam_functor(w.x, g.x, m.x, v.x, lr_t, omb1, omb2, eps);
-      adam_functor(w.y, g.y, m.y, v.y, lr_t, omb1, omb2, eps);
-      adam_functor(w.z, g.z, m.z, v.z, lr_t, omb1, omb2, eps);
-      adam_functor(w.w, g.w, m.w, v.w, lr_t, omb1, omb2, eps);
-      *reinterpret_cast<float4*>(prow + c * 4) = w;
-      stg4(st + o_m + c * 4, m);
-      stg4(st + o_v + c * 4, v);
-      stg4(st + c * 4, f4_zero());
-    }
+    if (chunk_ok)
+      adam_replay_step_chunk(st + c * 4, st + o_m + c * 4, st + o_v + c * 4, prow + c * 4, stamp, t_now - 1, t_now,
+                                   p.hist, lr_t, omb1, omb2, eps);
     if (c == 0) {
       if (has_w) {
         float* wp = p.lin_in_row ? prow + D : p.lin_ptrs[s] + (size_t)id * p.lin_stride;
-        float pa[1] = {*wp}, ma[1] = {ld_cg1(st + o_s + 1)}, va[1] = {ld_cg1(st + o_s + 2)};
-        adam_catch_up<1>(pa, ma, va, stamp, t_now - 1, t_now, p.hist, omb1, omb2, eps);
-        adam_functor(pa[0], ld_cg1(st + o_s), ma[0], va[0], lr_t, omb1, omb2, eps);
-        *wp = pa[0];
-        st[o_s + 1] = ma[0];
-        st[o_s + 2] = va[0];
-        st[o_s] = 0.f;
+        adam_replay_step_weight(wp, st, o_s, stamp, t_now - 1, t_now, p.hist, lr_t,
+                                      omb1, omb2, eps);
       }
       st[o_s + 4] = __int_as_float((int)t_now);
     }
@@ -555,12 +442,6 @@ __global__ void adam_advance_hist_kernel(int64_t* step, float lr, float b1, floa
   const float v = (float)((double)lr * sqrt(1.0 - p2) / (1.0 - p1));
   *lr_t = v;
   if (lr_hist && hist_len > 0) lr_hist[t % hist_len] = v;
-}
-
-static int lpr_of(int D) {
-  int chunks = D / 4, lpr = 1;
-  while (lpr < chunks) lpr <<= 1;
-  return lpr;
 }
 
 // ---- the same tf.keras-equal Adam on a row-sharded table (owner(r) = r mod G, local row r div G) ----------------------
@@ -639,22 +520,13 @@ __global__ void __launch_bounds__(256) shard_adam_prepare_kernel(const int32_t* 
       __syncwarp();                                                               // ... before its leader rewrites it
       if (row < 0 || stamp <= 0 || stamp >= t_now - 1) continue;
       float* prow = w + (size_t)row * row_stride;
-      if (c * 4 < D) {
-        float4 mm = *reinterpret_cast<float4*>(st + o_m + c * 4), vv = *reinterpret_cast<float4*>(st + o_v + c * 4);
-        float4 ww = *reinterpret_cast<float4*>(prow + c * 4);
-        float pa[4] = {ww.x, ww.y, ww.z, ww.w}, ma[4] = {mm.x, mm.y, mm.z, mm.w}, va[4] = {vv.x, vv.y, vv.z, vv.w};
-        adam_catch_up<4>(pa, ma, va, stamp, t_now - 1, t_now, hist, omb1, omb2, eps);
-        *reinterpret_cast<float4*>(prow + c * 4) = make_float4(pa[0], pa[1], pa[2], pa[3]);
-        *reinterpret_cast<float4*>(st + o_m + c * 4) = make_float4(ma[0], ma[1], ma[2], ma[3]);
-        *reinterpret_cast<float4*>(st + o_v + c * 4) = make_float4(va[0], va[1], va[2], va[3]);
-      }
+      if (c * 4 < D)
+        adam_replay_chunk<LdPlain>(st, o_m, o_v, prow, c * 4, stamp, t_now - 1, t_now, hist,
+                                   omb1, omb2, eps);
       if (c == 0) {
-        if (has_lin) {
-          float* wp = lin_at(w, prow, row, D, lin_in_row, lin_off);
-          float pa[1] = {*wp}, ma[1] = {st[o_s + 1]}, va[1] = {st[o_s + 2]};
-          adam_catch_up<1>(pa, ma, va, stamp, t_now - 1, t_now, hist, omb1, omb2, eps);
-          *wp = pa[0]; st[o_s + 1] = ma[0]; st[o_s + 2] = va[0];
-        }
+        if (has_lin)
+          adam_replay_weight<LdPlain>(lin_at(w, prow, row, D, lin_in_row, lin_off), st, o_s, stamp,
+                                      t_now - 1, t_now, hist, omb1, omb2, eps);
         st[o_s + 4] = __int_as_float((int)(t_now - 1));
       }
     }
@@ -688,10 +560,7 @@ __global__ void __launch_bounds__(256) shard_adam_apply_kernel(const int32_t* __
       const float4 gg = __ldcg(reinterpret_cast<const float4*>(grow + c * 4));   // red.add of every rank landed here
       float4 m = *reinterpret_cast<float4*>(st + o_m + c * 4), v = *reinterpret_cast<float4*>(st + o_v + c * 4);
       float4 p = *reinterpret_cast<float4*>(prow + c * 4);
-      adam_functor(p.x, gg.x, m.x, v.x, lr_t, omb1, omb2, eps);
-      adam_functor(p.y, gg.y, m.y, v.y, lr_t, omb1, omb2, eps);
-      adam_functor(p.z, gg.z, m.z, v.z, lr_t, omb1, omb2, eps);
-      adam_functor(p.w, gg.w, m.w, v.w, lr_t, omb1, omb2, eps);
+      adam_functor4(p, gg, m, v, lr_t, omb1, omb2, eps);
       *reinterpret_cast<float4*>(prow + c * 4) = p;
       *reinterpret_cast<float4*>(st + o_m + c * 4) = m;
       *reinterpret_cast<float4*>(st + o_v + c * 4) = v;
@@ -729,14 +598,12 @@ extern "C" int dr_embed_adam_count(const void* ids, int id_bytes, int64_t B, int
   if (B == 0) return DR_OK;
   DR_REQUIRE(ids && rows && slot_offsets && state, DR_EINVAL, "dr_embed_adam_count: null pointer");
   const int64_t n = B * S;
-  int64_t ctas = (n + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
-  const int SS = adam_state_stride(D);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (id_bytes == 8)
-    embed_adam_count_kernel<int64_t><<<(unsigned)ctas, 256, 0, st>>>((const int64_t*)ids, n, S, rows, slot_offsets, state, SS, 3 * D + 3);
-  else
-    embed_adam_count_kernel<int32_t><<<(unsigned)ctas, 256, 0, st>>>((const int32_t*)ids, n, S, rows, slot_offsets, state, SS, 3 * D + 3);
+  const int64_t ctas = capped_grid(n, 256, 16);
+  with_id_type(id_bytes, [&](auto id) {
+    using IdT = decltype(id);
+    embed_adam_count_kernel<IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
+        (const IdT*)ids, n, S, rows, slot_offsets, state, adam_state_stride(D), 3 * D + 3);
+  });
   DR_CUDA_LAUNCH_CHECK("dr_embed_adam_count");
   return DR_OK;
 }
@@ -763,8 +630,7 @@ static int embed_fm_bwd_adam_impl(const char* fn, const void* ids, int id_bytes,
   const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
   DR_REQUIRE(row_stride >= D + (lin_in_row ? 4 : 0) && row_stride % 4 == 0 && lin_stride >= 1, DR_EINVAL,
              "%s: bad strides row=%lld lin=%lld", fn, (long long)row_stride, (long long)lin_stride);
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
-             "%s: beta1=%g beta2=%g eps=%g out of range", fn, (double)beta1, (double)beta2, (double)eps);
+  if (int rc = check_adam_hparams(fn, beta1, beta2, eps)) return rc;
   const bool exact = step_dev != nullptr;
   AdamBwdParams p{};
   p.ids = ids; p.rows = rows; p.slot_offsets = slot_offsets; p.stack = stack; p.sum_e = sum_e; p.g_logit = g_logit;
@@ -775,25 +641,13 @@ static int embed_fm_bwd_adam_impl(const char* fn, const void* ids, int id_bytes,
   p.step_dev = step_dev; p.hist = AdamHist{lr_hist, hist_len, lr, beta1, beta2};
   const int threads = 256, warps = threads / 32;
   const size_t smem = (size_t)S * (sizeof(void*) * 2 + sizeof(int64_t) * 2);
-  int64_t ctas = (B + warps - 1) / warps;
-  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
+  const int64_t ctas = capped_grid(B, warps, 8);
   cudaStream_t st = (cudaStream_t)stream;
-#define DR_ADAM2(L, IdT)                                                                                        \
-  do {                                                                                                          \
-    if (exact) embed_fm_bwd_adam_kernel<L, IdT, true><<<(unsigned)ctas, threads, smem, st>>>(p);                \
-    else embed_fm_bwd_adam_kernel<L, IdT, false><<<(unsigned)ctas, threads, smem, st>>>(p);                     \
-  } while (0)
-#define DR_ADAM(L) do { if (id_bytes == 8) DR_ADAM2(L, int64_t); else DR_ADAM2(L, int32_t); } while (0)
-  switch (lpr_of(D)) {
-    case 1: DR_ADAM(1); break;
-    case 2: DR_ADAM(2); break;
-    case 4: DR_ADAM(4); break;
-    case 8: DR_ADAM(8); break;
-    case 16: DR_ADAM(16); break;
-    default: DR_ADAM(32); break;
-  }
-#undef DR_ADAM
-#undef DR_ADAM2
+  with_lpr_id(lanes_per_row(D / 4), id_bytes, [&](auto L, auto id) {
+    using IdT = decltype(id);
+    if (exact) embed_fm_bwd_adam_kernel<L, IdT, true><<<(unsigned)ctas, threads, smem, st>>>(p);
+    else embed_fm_bwd_adam_kernel<L, IdT, false><<<(unsigned)ctas, threads, smem, st>>>(p);
+  });
   DR_CUDA_LAUNCH_CHECK(fn);
   return DR_OK;
 }
@@ -824,8 +678,8 @@ extern "C" int dr_embed_fm_bwd_adam_tf(const void* ids, int id_bytes, const int6
 extern "C" int dr_adam_advance_hist(int64_t* step_dev, float lr, float beta1, float beta2, float* lr_t_dev,
                                     float* lr_hist, int hist_len, void* stream) {
   DR_REQUIRE(step_dev && lr_t_dev, DR_EINVAL, "dr_adam_advance_hist: null pointer");
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && hist_len >= 0, DR_EINVAL,
-             "dr_adam_advance_hist: beta1=%g beta2=%g hist_len=%d out of range", (double)beta1, (double)beta2, hist_len);
+  if (int rc = check_adam_hparams("dr_adam_advance_hist", beta1, beta2, 0.f)) return rc;
+  DR_REQUIRE(hist_len >= 0, DR_EINVAL, "dr_adam_advance_hist: hist_len=%d out of range", hist_len);
   adam_advance_hist_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_dev, lr, beta1, beta2, lr_t_dev, lr_hist, hist_len);
   DR_CUDA_LAUNCH_CHECK("dr_adam_advance_hist");
   return DR_OK;
@@ -846,27 +700,15 @@ extern "C" int dr_embed_adam_prepare(const void* ids, int id_bytes, int64_t B, i
   if (lin_stride == 0) lin_stride = 1;
   const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
   const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
-  const int lpr = lpr_of(D);
+  const int lpr = lanes_per_row(D / 4);
   const int64_t n = B * S;
-  int64_t ctas = (n * lpr + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
-  cudaStream_t st = (cudaStream_t)stream;
-#define DR_PREP2(L, IdT)                                                                                               \
-  embed_adam_prepare_kernel<L, IdT><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, n, S, D, rows, slot_offsets, table_ptrs, \
-                                                                  lin_in_row ? nullptr : lin_ptrs, row_stride, lin_stride, \
-                                                                  lin_in_row, state, adam_state_stride(D), step_dev, h,  \
-                                                                  1.f - beta1, 1.f - beta2, eps)
-#define DR_PREP(L) do { if (id_bytes == 8) DR_PREP2(L, int64_t); else DR_PREP2(L, int32_t); } while (0)
-  switch (lpr) {
-    case 1: DR_PREP(1); break;
-    case 2: DR_PREP(2); break;
-    case 4: DR_PREP(4); break;
-    case 8: DR_PREP(8); break;
-    case 16: DR_PREP(16); break;
-    default: DR_PREP(32); break;
-  }
-#undef DR_PREP
-#undef DR_PREP2
+  const int64_t ctas = capped_grid(n * lpr, 256, 16);
+  with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
+    using IdT = decltype(id);
+    embed_adam_prepare_kernel<L, IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
+        (const IdT*)ids, n, S, D, rows, slot_offsets, table_ptrs, lin_in_row ? nullptr : lin_ptrs, row_stride, lin_stride,
+        lin_in_row, state, adam_state_stride(D), step_dev, h, 1.f - beta1, 1.f - beta2, eps);
+  });
   DR_CUDA_LAUNCH_CHECK("dr_embed_adam_prepare");
   return DR_OK;
 }
@@ -883,23 +725,13 @@ extern "C" int dr_embed_adam_flush(const int64_t* rows, const int64_t* slot_offs
   if (lin_stride == 0) lin_stride = 1;
   const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
   const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
-  const int lpr = lpr_of(D);
-  int64_t ctas = (total_rows * lpr + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
-  cudaStream_t st = (cudaStream_t)stream;
-#define DR_FLUSH(L)                                                                                                 \
-  embed_adam_flush_kernel<L><<<(unsigned)ctas, 256, 0, st>>>(table_ptrs, lin_in_row ? nullptr : lin_ptrs, rows, slot_offsets, S, \
-                                                           D, row_stride, lin_stride, lin_in_row, state, adam_state_stride(D), \
-                                                           total_rows, step_dev, h, 1.f - beta1, 1.f - beta2, eps)
-  switch (lpr) {
-    case 1: DR_FLUSH(1); break;
-    case 2: DR_FLUSH(2); break;
-    case 4: DR_FLUSH(4); break;
-    case 8: DR_FLUSH(8); break;
-    case 16: DR_FLUSH(16); break;
-    default: DR_FLUSH(32); break;
-  }
-#undef DR_FLUSH
+  const int lpr = lanes_per_row(D / 4);
+  const int64_t ctas = capped_grid(total_rows * lpr, 256, 16);
+  with_lpr(lpr, [&](auto L) {
+    embed_adam_flush_kernel<L><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
+        table_ptrs, lin_in_row ? nullptr : lin_ptrs, rows, slot_offsets, S, D, row_stride, lin_stride, lin_in_row, state,
+        adam_state_stride(D), total_rows, step_dev, h, 1.f - beta1, 1.f - beta2, eps);
+  });
   DR_CUDA_LAUNCH_CHECK("dr_embed_adam_flush");
   return DR_OK;
 }
@@ -929,32 +761,19 @@ extern "C" int dr_embed_adam_catch_up(const void* ids, int id_bytes, int64_t n, 
   int lin_in_row = 0;
   if (int rc = adam_rows_layout_check(fn, D, row_stride, lin_stride, flags, lin_ptrs, lin_in_row)) return rc;
   DR_REQUIRE(hist_len >= 0 && (hist_len == 0 || lr_hist), DR_EINVAL, "%s: bad lr history", fn);
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
-             "%s: beta1=%g beta2=%g eps=%g out of range", fn, (double)beta1, (double)beta2, (double)eps);
+  if (int rc = check_adam_hparams(fn, beta1, beta2, eps)) return rc;
   if (n == 0) return DR_OK;
   DR_REQUIRE(ids && rows && slot_offsets && table_ptrs && state && step_dev, DR_EINVAL, "%s: null pointer", fn);
   DR_REQUIRE(aligned16(state), DR_EALIGN, "%s: state not 16-B aligned", fn);
   const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
-  const int lpr = lpr_of(D);
-  int64_t ctas = (n * lpr + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
-  cudaStream_t st = (cudaStream_t)stream;
-#define DR_CATCH2(L, IdT)                                                                                              \
-  embed_adam_catch_up_kernel<L, IdT><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, n, S, D, rows, slot_offsets,      \
-                                                                   table_ptrs, lin_ptrs, row_stride, lin_stride,       \
-                                                                   lin_in_row, state, adam_state_stride(D), step_dev, h, \
-                                                                   1.f - beta1, 1.f - beta2, eps)
-#define DR_CATCH(L) do { if (id_bytes == 8) DR_CATCH2(L, int64_t); else DR_CATCH2(L, int32_t); } while (0)
-  switch (lpr) {
-    case 1: DR_CATCH(1); break;
-    case 2: DR_CATCH(2); break;
-    case 4: DR_CATCH(4); break;
-    case 8: DR_CATCH(8); break;
-    case 16: DR_CATCH(16); break;
-    default: DR_CATCH(32); break;
-  }
-#undef DR_CATCH
-#undef DR_CATCH2
+  const int lpr = lanes_per_row(D / 4);
+  const int64_t ctas = capped_grid(n * lpr, 256, 16);
+  with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
+    using IdT = decltype(id);
+    embed_adam_catch_up_kernel<L, IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
+        (const IdT*)ids, n, S, D, rows, slot_offsets, table_ptrs, lin_ptrs, row_stride, lin_stride, lin_in_row, state,
+        adam_state_stride(D), step_dev, h, 1.f - beta1, 1.f - beta2, eps);
+  });
   DR_CUDA_LAUNCH_CHECK(fn);
   return DR_OK;
 }
@@ -982,8 +801,7 @@ extern "C" int dr_embed_adam_rows_tf(const void* ids, int id_bytes, int64_t n, i
              DR_EINVAL, "%s: bad gradient strides g_ld=%lld g_slot=%lld gl_ld=%lld gl_slot=%lld for D=%d", fn,
              (long long)g_ld, (long long)g_slot, (long long)gl_ld, (long long)gl_slot, D);
   DR_REQUIRE(hist_len >= 0 && (hist_len == 0 || lr_hist), DR_EINVAL, "%s: bad lr history", fn);
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
-             "%s: beta1=%g beta2=%g eps=%g out of range", fn, (double)beta1, (double)beta2, (double)eps);
+  if (int rc = check_adam_hparams(fn, beta1, beta2, eps)) return rc;
   if (n == 0) return DR_OK;
   DR_REQUIRE(ids && rows && slot_offsets && g_emb && table_ptrs && state && step_dev && lr_t_dev && (!row_splits || B >= 1),
              DR_EINVAL, "%s: null pointer", fn);
@@ -995,26 +813,14 @@ extern "C" int dr_embed_adam_rows_tf(const void* ids, int id_bytes, int64_t n, i
   p.lin_stride = lin_stride; p.lin_in_row = lin_in_row; p.state = state; p.SS = adam_state_stride(D);
   p.step_dev = step_dev; p.lr_t_dev = lr_t_dev; p.hist = AdamHist{lr_hist, hist_len, lr, beta1, beta2};
   p.omb1 = 1.f - beta1; p.omb2 = 1.f - beta2; p.eps = eps;
-  const int lpr = lpr_of(D);
-  int64_t ctas = (n * lpr + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
+  const int lpr = lanes_per_row(D / 4);
+  const int64_t ctas = capped_grid(n * lpr, 256, 16);
   cudaStream_t st = (cudaStream_t)stream;
-#define DR_ROWS3(L, IdT)                                                                                \
-  do {                                                                                                  \
-    if (row_splits) embed_adam_rows_tf_kernel<L, IdT, true><<<(unsigned)ctas, 256, 0, st>>>(p);         \
-    else embed_adam_rows_tf_kernel<L, IdT, false><<<(unsigned)ctas, 256, 0, st>>>(p);                   \
-  } while (0)
-#define DR_ROWS(L) do { if (id_bytes == 8) DR_ROWS3(L, int64_t); else DR_ROWS3(L, int32_t); } while (0)
-  switch (lpr) {
-    case 1: DR_ROWS(1); break;
-    case 2: DR_ROWS(2); break;
-    case 4: DR_ROWS(4); break;
-    case 8: DR_ROWS(8); break;
-    case 16: DR_ROWS(16); break;
-    default: DR_ROWS(32); break;
-  }
-#undef DR_ROWS
-#undef DR_ROWS3
+  with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
+    using IdT = decltype(id);
+    if (row_splits) embed_adam_rows_tf_kernel<L, IdT, true><<<(unsigned)ctas, 256, 0, st>>>(p);
+    else embed_adam_rows_tf_kernel<L, IdT, false><<<(unsigned)ctas, 256, 0, st>>>(p);
+  });
   DR_CUDA_LAUNCH_CHECK(fn);
   return DR_OK;
 }
@@ -1029,15 +835,12 @@ extern "C" int dr_shard_adam_mark(const void* ids, int id_bytes, int64_t n, int 
              kMaxShardWorld);
   DR_REQUIRE(ids && slot_offsets && rows && touch_bases && step_dev, DR_EINVAL, "dr_shard_adam_mark: null pointer");
   if (n == 0) return DR_OK;
-  int64_t ctas = (n + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (id_bytes == 8)
-    shard_adam_mark_kernel<int64_t><<<(unsigned)ctas, 256, 0, st>>>((const int64_t*)ids, n, S, slot_offsets, rows, world,
-                                                                     touch_bases, step_dev);
-  else
-    shard_adam_mark_kernel<int32_t><<<(unsigned)ctas, 256, 0, st>>>((const int32_t*)ids, n, S, slot_offsets, rows, world,
-                                                                     touch_bases, step_dev);
+  const int64_t ctas = capped_grid(n, 256, 16);
+  with_id_type(id_bytes, [&](auto id) {
+    using IdT = decltype(id);
+    shard_adam_mark_kernel<IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>((const IdT*)ids, n, S, slot_offsets,
+                                                                                 rows, world, touch_bases, step_dev);
+  });
   DR_CUDA_LAUNCH_CHECK("dr_shard_adam_mark");
   return DR_OK;
 }
@@ -1060,33 +863,24 @@ extern "C" int dr_shard_adam_prepare(int32_t* touch, int64_t local_rows, int32_t
                                      int64_t row_stride, int64_t lin_offset, int flags, float* shard, float* state,
                                      const int64_t* step_dev, const float* lr_hist, int hist_len, float lr, float beta1,
                                      float beta2, float eps, void* stream) {
-  if (int rc = shard_adam_layout_check("dr_shard_adam_prepare", local_rows, D, row_stride, lin_offset, flags)) return rc;
-  DR_REQUIRE(touch && list && count && shard && state && step_dev, DR_EINVAL, "dr_shard_adam_prepare: null pointer");
-  DR_REQUIRE(hist_len >= 0 && (hist_len == 0 || lr_hist), DR_EINVAL, "dr_shard_adam_prepare: bad lr history");
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
-             "dr_shard_adam_prepare: beta1=%g beta2=%g eps=%g out of range", (double)beta1, (double)beta2, (double)eps);
-  DR_REQUIRE(aligned16(shard) && aligned16(state), DR_EALIGN, "dr_shard_adam_prepare: shard / state not 16-B aligned");
+  const char* fn = "dr_shard_adam_prepare";
+  if (int rc = shard_adam_layout_check(fn, local_rows, D, row_stride, lin_offset, flags)) return rc;
+  DR_REQUIRE(touch && list && count && shard && state && step_dev, DR_EINVAL, "%s: null pointer", fn);
+  DR_REQUIRE(hist_len >= 0 && (hist_len == 0 || lr_hist), DR_EINVAL, "%s: bad lr history", fn);
+  if (int rc = check_adam_hparams(fn, beta1, beta2, eps)) return rc;
+  DR_REQUIRE(aligned16(shard) && aligned16(state), DR_EALIGN, "%s: shard / state not 16-B aligned", fn);
   cudaStream_t st = (cudaStream_t)stream;
   DR_CUDA_CALL(cudaMemsetAsync(count, 0, sizeof(int32_t), st));
   if (local_rows == 0) return DR_OK;
   const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
   const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
-  int64_t ctas = (local_rows + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
-#define DR_SPREP(L)                                                                                                    \
-  shard_adam_prepare_kernel<L><<<(unsigned)ctas, 256, 0, st>>>(touch, local_rows, list, count, shard, row_stride,      \
-                                                               lin_offset, lin_in_row, state, adam_state_stride(D), D, \
-                                                               step_dev, h, 1.f - beta1, 1.f - beta2, eps)
-  switch (lpr_of(D)) {
-    case 1: DR_SPREP(1); break;
-    case 2: DR_SPREP(2); break;
-    case 4: DR_SPREP(4); break;
-    case 8: DR_SPREP(8); break;
-    case 16: DR_SPREP(16); break;
-    default: DR_SPREP(32); break;
-  }
-#undef DR_SPREP
-  DR_CUDA_LAUNCH_CHECK("dr_shard_adam_prepare");
+  const int64_t ctas = capped_grid(local_rows, 256, 16);
+  with_lpr(lanes_per_row(D / 4), [&](auto L) {
+    shard_adam_prepare_kernel<L><<<(unsigned)ctas, 256, 0, st>>>(touch, local_rows, list, count, shard, row_stride,
+                                                                 lin_offset, lin_in_row, state, adam_state_stride(D), D,
+                                                                 step_dev, h, 1.f - beta1, 1.f - beta2, eps);
+  });
+  DR_CUDA_LAUNCH_CHECK(fn);
   return DR_OK;
 }
 
@@ -1094,31 +888,21 @@ extern "C" int dr_shard_adam_apply(const int32_t* list, const int32_t* count, in
                                    int64_t row_stride, int64_t lin_offset, int flags, float* shard, float* grad,
                                    float* state, const int64_t* step_dev, const float* lr_t_dev, float beta1, float beta2,
                                    float eps, void* stream) {
-  if (int rc = shard_adam_layout_check("dr_shard_adam_apply", local_rows, D, row_stride, lin_offset, flags)) return rc;
-  DR_REQUIRE(list && count && shard && grad && state && step_dev && lr_t_dev, DR_EINVAL, "dr_shard_adam_apply: null pointer");
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
-             "dr_shard_adam_apply: beta1=%g beta2=%g eps=%g out of range", (double)beta1, (double)beta2, (double)eps);
+  const char* fn = "dr_shard_adam_apply";
+  if (int rc = shard_adam_layout_check(fn, local_rows, D, row_stride, lin_offset, flags)) return rc;
+  DR_REQUIRE(list && count && shard && grad && state && step_dev && lr_t_dev, DR_EINVAL, "%s: null pointer", fn);
+  if (int rc = check_adam_hparams(fn, beta1, beta2, eps)) return rc;
   DR_REQUIRE(aligned16(shard) && aligned16(grad) && aligned16(state), DR_EALIGN,
-             "dr_shard_adam_apply: shard / grad / state not 16-B aligned");
+             "%s: shard / grad / state not 16-B aligned", fn);
   if (local_rows == 0) return DR_OK;
   const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
-  const int lpr = lpr_of(D);
-  int64_t ctas = (local_rows * lpr + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 16) ctas = (int64_t)num_sms() * 16;
-  cudaStream_t st = (cudaStream_t)stream;
-#define DR_SAPPLY(L)                                                                                                   \
-  shard_adam_apply_kernel<L><<<(unsigned)ctas, 256, 0, st>>>(list, count, shard, grad, row_stride, lin_offset,         \
-                                                             lin_in_row, state, adam_state_stride(D), D, step_dev,     \
-                                                             lr_t_dev, 1.f - beta1, 1.f - beta2, eps)
-  switch (lpr) {
-    case 1: DR_SAPPLY(1); break;
-    case 2: DR_SAPPLY(2); break;
-    case 4: DR_SAPPLY(4); break;
-    case 8: DR_SAPPLY(8); break;
-    case 16: DR_SAPPLY(16); break;
-    default: DR_SAPPLY(32); break;
-  }
-#undef DR_SAPPLY
-  DR_CUDA_LAUNCH_CHECK("dr_shard_adam_apply");
+  const int lpr = lanes_per_row(D / 4);
+  const int64_t ctas = capped_grid(local_rows * lpr, 256, 16);
+  with_lpr(lpr, [&](auto L) {
+    shard_adam_apply_kernel<L><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
+        list, count, shard, grad, row_stride, lin_offset, lin_in_row, state, adam_state_stride(D), D, step_dev, lr_t_dev,
+        1.f - beta1, 1.f - beta2, eps);
+  });
+  DR_CUDA_LAUNCH_CHECK(fn);
   return DR_OK;
 }

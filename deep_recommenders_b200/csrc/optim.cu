@@ -6,17 +6,9 @@
 // scatter_add of the touched rows).  dr_adam_step is that dense update in one pass over the parameter arena;
 // the row-sparse gradients are accumulated beforehand by dr_embed_fm_bwd / dr_scatter_add with scale = 1.
 // HBM-bound: 4 reads + 3 (or 4, zero_grad) writes of n floats per step.
-#include "common.cuh"
+#include "adam.cuh"
 
 namespace dr {
-
-__device__ __forceinline__ void adam_elem(float& p, float g, float& m, float& v, float lr_t, float omb1, float omb2,
-                                          float eps) {
-  // TF's ApplyAdam functor: m += (g - m)(1 - b1); v += (g*g - v)(1 - b2); var -= lr_t * m / (sqrt(v) + eps)
-  m += (g - m) * omb1;
-  v += (g * g - v) * omb2;
-  p -= (m * lr_t) / (sqrtf(v) + eps);
-}
 
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, float* __restrict__ g,
                                                     float* __restrict__ m, float* __restrict__ v, int64_t n,
@@ -31,10 +23,7 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, float*
     const float4 gg = reinterpret_cast<const float4*>(g)[i];
     float4 mm = reinterpret_cast<float4*>(m)[i];
     float4 vv = reinterpret_cast<float4*>(v)[i];
-    adam_elem(pp.x, gg.x, mm.x, vv.x, lr_t, omb1, omb2, eps);
-    adam_elem(pp.y, gg.y, mm.y, vv.y, lr_t, omb1, omb2, eps);
-    adam_elem(pp.z, gg.z, mm.z, vv.z, lr_t, omb1, omb2, eps);
-    adam_elem(pp.w, gg.w, mm.w, vv.w, lr_t, omb1, omb2, eps);
+    adam_functor4(pp, gg, mm, vv, lr_t, omb1, omb2, eps);
     reinterpret_cast<float4*>(p)[i] = pp;
     reinterpret_cast<float4*>(m)[i] = mm;
     reinterpret_cast<float4*>(v)[i] = vv;
@@ -42,7 +31,7 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, float*
   }
   for (int64_t i = n4 * 4 + tid; i < n; i += stride) {
     float pp = p[i], mm = m[i], vv = v[i];
-    adam_elem(pp, g[i], mm, vv, lr_t, omb1, omb2, eps);
+    adam_functor(pp, g[i], mm, vv, lr_t, omb1, omb2, eps);
     p[i] = pp; m[i] = mm; v[i] = vv;
     if (zero_grad) g[i] = 0.f;
   }
@@ -57,11 +46,9 @@ extern "C" int dr_adam_step(float* p, float* g, float* m, float* v, int64_t n, f
   DR_REQUIRE(n >= 0, DR_EINVAL, "dr_adam_step: n=%lld < 0", (long long)n);
   if (n == 0) return DR_OK;
   DR_REQUIRE(p && g && m && v, DR_EINVAL, "dr_adam_step: null pointer");
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
-             "dr_adam_step: beta1=%g beta2=%g eps=%g out of range", (double)beta1, (double)beta2, (double)eps);
+  if (int rc = check_adam_hparams("dr_adam_step", beta1, beta2, eps)) return rc;
   const int vec_ok = aligned16(p) && aligned16(g) && aligned16(m) && aligned16(v);
-  int64_t ctas = (n / 4 + 255) / 256;
-  if (ctas > num_sms() * 8) ctas = num_sms() * 8;
+  int64_t ctas = capped_grid(n / 4, 256, 8);
   if (ctas < 1) ctas = 1;
   adam_kernel<<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, lr_t, 1.f - beta1, 1.f - beta2, eps,
                                                                  zero_grad, vec_ok, lr_t_dev);
@@ -123,17 +110,17 @@ __global__ void __launch_bounds__(256) lazy_adam_rows_kernel(const IdT* __restri
       const size_t o = (size_t)row * row_stride + c * 4;
       float4 pp = ldg4(p + o), mm = ldg4(m + o), vv = ldg4(v + o);
       const float4 gg = ldg4(g + o);
-      adam_elem(pp.x, gg.x, mm.x, vv.x, lr_t, omb1, omb2, eps);
+      adam_functor(pp.x, gg.x, mm.x, vv.x, lr_t, omb1, omb2, eps);
       if (!lin_lane) {   // the [w | pad] chunk only carries one parameter
-        adam_elem(pp.y, gg.y, mm.y, vv.y, lr_t, omb1, omb2, eps);
-        adam_elem(pp.z, gg.z, mm.z, vv.z, lr_t, omb1, omb2, eps);
-        adam_elem(pp.w, gg.w, mm.w, vv.w, lr_t, omb1, omb2, eps);
+        adam_functor(pp.y, gg.y, mm.y, vv.y, lr_t, omb1, omb2, eps);
+        adam_functor(pp.z, gg.z, mm.z, vv.z, lr_t, omb1, omb2, eps);
+        adam_functor(pp.w, gg.w, mm.w, vv.w, lr_t, omb1, omb2, eps);
       }
       stg4(p + o, pp); stg4(m + o, mm); stg4(v + o, vv); stg4(g + o, f4_zero());
     }
     if (won && lin_p && c == 0) {   // split layout: first-order weights live in their own arrays
       float pp = lin_p[row], mm = lin_m[row], vv = lin_v[row];
-      adam_elem(pp, lin_g[row], mm, vv, lr_t, omb1, omb2, eps);
+      adam_functor(pp, lin_g[row], mm, vv, lr_t, omb1, omb2, eps);
       lin_p[row] = pp; lin_m[row] = mm; lin_v[row] = vv; lin_g[row] = 0.f;
     }
   }
@@ -142,8 +129,7 @@ __global__ void __launch_bounds__(256) lazy_adam_rows_kernel(const IdT* __restri
 
 extern "C" int dr_adam_advance(int64_t* step_dev, float lr, float beta1, float beta2, float* lr_t_dev, void* stream) {
   DR_REQUIRE(step_dev && lr_t_dev, DR_EINVAL, "dr_adam_advance: null pointer");
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f, DR_EINVAL,
-             "dr_adam_advance: beta1=%g beta2=%g out of range", (double)beta1, (double)beta2);
+  if (int rc = check_adam_hparams("dr_adam_advance", beta1, beta2, 0.f)) return rc;
   adam_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_dev, lr, beta1, beta2, lr_t_dev);
   DR_CUDA_LAUNCH_CHECK("dr_adam_advance");
   return DR_OK;
@@ -167,30 +153,16 @@ extern "C" int dr_lazy_adam_rows(const void* ids, int id_bytes, int64_t B, int S
   DR_REQUIRE(!(lin_p && lin_in_row), DR_EINVAL, "dr_lazy_adam_rows: first-order arrays AND DR_EMBED_LIN_IN_ROW");
   DR_REQUIRE(aligned16(p) && aligned16(g) && aligned16(m) && aligned16(v), DR_EALIGN,
              "dr_lazy_adam_rows: an arena base is not 16-B aligned");
-  DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
-             "dr_lazy_adam_rows: beta1=%g beta2=%g eps=%g out of range", (double)beta1, (double)beta2, (double)eps);
-  int chunks = D / 4 + lin_in_row, lpr = 1;
-  while (lpr < chunks) lpr <<= 1;
+  if (int rc = check_adam_hparams("dr_lazy_adam_rows", beta1, beta2, eps)) return rc;
+  const int lpr = lanes_per_row(D / 4 + lin_in_row);     // the [w | pad] chunk takes a lane of its own
   const int64_t n = B * S;
-  const int64_t groups_per_cta = 256 / lpr;
-  int64_t ctas = (n + groups_per_cta - 1) / groups_per_cta;
-  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
-  cudaStream_t st = (cudaStream_t)stream;
-#define DR_LAZY(L, IdT)                                                                                              \
-  lazy_adam_rows_kernel<L, IdT><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, n, S, rows, slot_offsets, p, g, m, v, \
-                                                                row_stride, D, lin_in_row, lin_p, lin_g, lin_m, lin_v, \
-                                                                stamp, step_dev, lr_t_dev, 1.f - beta1, 1.f - beta2, eps)
-#define DR_LAZY_ID(L) do { if (id_bytes == 8) DR_LAZY(L, int64_t); else DR_LAZY(L, int32_t); } while (0)
-  switch (lpr) {
-    case 1: DR_LAZY_ID(1); break;
-    case 2: DR_LAZY_ID(2); break;
-    case 4: DR_LAZY_ID(4); break;
-    case 8: DR_LAZY_ID(8); break;
-    case 16: DR_LAZY_ID(16); break;
-    default: DR_LAZY_ID(32); break;
-  }
-#undef DR_LAZY_ID
-#undef DR_LAZY
+  const int64_t ctas = capped_grid(n, 256 / lpr, 8);
+  with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
+    using IdT = decltype(id);
+    lazy_adam_rows_kernel<L, IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
+        (const IdT*)ids, n, S, rows, slot_offsets, p, g, m, v, row_stride, D, lin_in_row, lin_p, lin_g, lin_m, lin_v,
+        stamp, step_dev, lr_t_dev, 1.f - beta1, 1.f - beta2, eps);
+  });
   DR_CUDA_LAUNCH_CHECK("dr_lazy_adam_rows");
   return DR_OK;
 }

@@ -104,7 +104,8 @@ def test_rows_tf_rejects_bad_arguments():
     assert _rows_call(lib, rs=32, flags=1) == DR_EINVAL      # an in-row weight without its gradient
     assert _rows_call(lib, rs=32, flags=1, lp=P, gl=P, gl_ld=2, gl_slot=1) == DR_EINVAL
     assert _rows_call(lib, hist_len=16) == DR_EINVAL         # a ring length without a ring
-    assert _rows_call(lib, b1=1.0) == DR_EINVAL
+    assert _rows_call(lib, b1=1.0) == DR_EINVAL and b"dr_embed_adam_rows_tf" in lib.dr_last_error()
+    assert _rows_call(lib, n=-1) == DR_EINVAL
     assert _rows_call(lib, ids=None) == DR_EINVAL
     assert _rows_call(lib, state=None) == DR_EINVAL
     assert _rows_call(lib, step=None) == DR_EINVAL
@@ -117,10 +118,13 @@ def test_rows_tf_rejects_bad_arguments():
 def test_catch_up_rejects_bad_arguments():
     from deep_recommenders_b200 import _lib
     lib = _lib.load()
-    call = lambda n=8, S=2, rs=0, flags=0, lp=None, ids=P, state=P, hist=None, hist_len=0, idb=8: \
-        lib.dr_embed_adam_catch_up(ids, idb, n, S, 8, P, P, rs, 0, flags, P, lp, state, P, hist, hist_len, 0.01, 0.9,
+    call = lambda n=8, S=2, rs=0, flags=0, lp=None, ids=P, state=P, hist=None, hist_len=0, idb=8, b1=0.9: \
+        lib.dr_embed_adam_catch_up(ids, idb, n, S, 8, P, P, rs, 0, flags, P, lp, state, P, hist, hist_len, 0.01, b1,
                                    0.999, 1e-8, None)
     assert call(n=7) == DR_EINVAL                            # not whole examples of S slots
+    assert call(S=0) == DR_EINVAL
+    assert call(flags=2) == DR_EINVAL and b"flags=2" in lib.dr_last_error()
+    assert call(b1=1.0) == DR_EINVAL and b"dr_embed_adam_catch_up" in lib.dr_last_error()
     assert call(rs=6) == DR_EINVAL and b"bad strides" in lib.dr_last_error()
     assert call(rs=8, flags=1) == DR_EINVAL
     assert call(rs=32, flags=1, lp=P) == DR_EINVAL

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-DR_EINVAL = -1
+DR_EINVAL, DR_EALIGN = -1, -2
 P = 1 << 12            # a 16-B aligned non-null address: never dereferenced, the checks fail first
 
 
@@ -31,8 +31,11 @@ def test_shard_adam_entries_reject_bad_arguments_without_gpu():
     assert mark(step=None) == DR_EINVAL
     assert mark(idb=2) == DR_EINVAL
     assert mark(n=-1) == DR_EINVAL
-    prep = lambda D=16, rs=32, lin_off=0, flags=1, touch=P, state=P, hist=0, hp=None: lib.dr_shard_adam_prepare(
-        touch, 10, P, P, D, rs, lin_off, flags, P, state, P, hp, hist, 0.01, 0.9, 0.999, 1e-7, None)
+    prep = lambda D=16, rs=32, lin_off=0, flags=1, touch=P, state=P, hist=0, hp=None, local=10, b2=0.999, shard=P: \
+        lib.dr_shard_adam_prepare(touch, local, P, P, D, rs, lin_off, flags, shard, state, P, hp, hist, 0.01, 0.9, b2,
+                                  1e-7, None)
+    assert prep(local=-1) == DR_EINVAL and b"local_rows=-1" in lib.dr_last_error()
+    assert prep(local=1 << 31) == DR_EINVAL
     assert prep(D=6) == DR_EINVAL and b"D=6" in lib.dr_last_error()
     assert prep(D=132) == DR_EINVAL
     assert prep(D=0) == DR_EINVAL
@@ -42,12 +45,17 @@ def test_shard_adam_entries_reject_bad_arguments_without_gpu():
     assert prep(touch=None) == DR_EINVAL
     assert prep(state=None) == DR_EINVAL
     assert prep(hist=16) == DR_EINVAL                        # a ring length without a ring
-    app = lambda D=16, grad=P, lr_t=P, b1=0.9: lib.dr_shard_adam_apply(P, P, 10, D, 32, 0, 1, P, grad, P, P, lr_t, b1,
-                                                                        0.999, 1e-7, None)
+    assert prep(b2=1.0) == DR_EINVAL and b"dr_shard_adam_prepare" in lib.dr_last_error()
+    assert prep(shard=P + 4) == DR_EALIGN
+    assert prep(state=P + 8) == DR_EALIGN
+    app = lambda D=16, grad=P, lr_t=P, b1=0.9, eps=1e-7: lib.dr_shard_adam_apply(P, P, 10, D, 32, 0, 1, P, grad, P, P,
+                                                                                  lr_t, b1, 0.999, eps, None)
     assert app(D=130) == DR_EINVAL
     assert app(grad=None) == DR_EINVAL
     assert app(lr_t=None) == DR_EINVAL
     assert app(b1=1.0) == DR_EINVAL
+    assert app(eps=-1.0) == DR_EINVAL and b"dr_shard_adam_apply" in lib.dr_last_error()
+    assert app(grad=P + 4) == DR_EALIGN
 
 
 @pytest.mark.parametrize("new_world", [2, 5])
