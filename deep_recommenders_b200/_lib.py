@@ -84,6 +84,7 @@ _SIGS = {
     # SURVEY 8(f) "next" rows
     "dr_adam_step": [_p, _p, _p, _p, _i64, _f, _f, _f, _f, _i, _p, _p],
     "dr_adam_advance": [_p, _f, _f, _f, _p, _p],
+    "dr_adam_step_multi": [_i, _p, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p],
     "dr_lazy_adam_rows": [_p, _i, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _p, _p, _p, _p,
                           _f, _f, _f, _p],
     "dr_embed_adam_state_stride": [_i],

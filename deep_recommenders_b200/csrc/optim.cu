@@ -56,6 +56,105 @@ extern "C" int dr_adam_step(float* p, float* g, float* m, float* v, int64_t n, f
   return DR_OK;
 }
 
+// ---- dr_adam_step over a list of tensors in one launch -------------------------------------------------------------
+// tf.keras Adam updates every variable of a model each step; a launch per variable makes a model with many small
+// variables (the Transformer) launch-bound.  The tensor table and its work list travel by value in the kernel's argument
+// block (no host-to-device copy, so the entry can be captured in a CUDA graph): CTA b works on chunk b - chunk0[i] of
+// tensor i, the last i with chunk0[i] <= b.  Kept under the classic 4 KB argument limit: 64 tensors per launch.
+namespace dr {
+constexpr int kMultiTensors = 64;
+constexpr int kMultiChunk = 16384;      // floats per CTA: a multiple of 4, so a 16-B aligned tensor's chunks stay aligned
+
+struct AdamMultiArgs {
+  float* p[kMultiTensors];
+  float* g[kMultiTensors];
+  float* m[kMultiTensors];
+  float* v[kMultiTensors];
+  int64_t n[kMultiTensors];
+  int32_t chunk0[kMultiTensors + 1];   // first CTA of tensor i; chunk0[count] = the grid
+  uint64_t vec;                        // bit i: tensor i's four pointers are 16-B aligned (float4 path)
+  int count;
+};
+
+__global__ void __launch_bounds__(256) adam_multi_kernel(const __grid_constant__ AdamMultiArgs a, float lr_t,
+                                                          float omb1, float omb2, float eps,
+                                                          const float* __restrict__ lr_t_dev) {
+  if (lr_t_dev) lr_t = __ldg(lr_t_dev);
+  const int b = blockIdx.x;
+  int i = 0, hi = a.count - 1;
+  while (i < hi) {
+    const int mid = (i + hi + 1) >> 1;
+    if (a.chunk0[mid] <= b) i = mid;
+    else hi = mid - 1;
+  }
+  float* __restrict__ p = a.p[i];
+  const float* __restrict__ g = a.g[i];
+  float* __restrict__ m = a.m[i];
+  float* __restrict__ v = a.v[i];
+  const int64_t begin = (int64_t)(b - a.chunk0[i]) * kMultiChunk;
+  const int64_t end = min(begin + kMultiChunk, a.n[i]);
+  const int64_t end4 = ((a.vec >> i) & 1) ? (end & ~(int64_t)3) : begin;
+  for (int64_t j = begin + 4 * threadIdx.x; j < end4; j += 4 * blockDim.x) {
+    float4 pp = *reinterpret_cast<const float4*>(p + j);
+    const float4 gg = *reinterpret_cast<const float4*>(g + j);
+    float4 mm = *reinterpret_cast<const float4*>(m + j);
+    float4 vv = *reinterpret_cast<const float4*>(v + j);
+    adam_functor4(pp, gg, mm, vv, lr_t, omb1, omb2, eps);
+    stg4(p + j, pp);
+    stg4(m + j, mm);
+    stg4(v + j, vv);
+  }
+  for (int64_t j = end4 + threadIdx.x; j < end; j += blockDim.x) {
+    float pp = p[j], mm = m[j], vv = v[j];
+    adam_functor(pp, g[j], mm, vv, lr_t, omb1, omb2, eps);
+    p[j] = pp; m[j] = mm; v[j] = vv;
+  }
+}
+}  // namespace dr
+
+extern "C" int dr_adam_step_multi(int n_tensors, float* const* p, float* const* g, float* const* m, float* const* v,
+                                  const int64_t* n, float lr_t, float beta1, float beta2, float eps,
+                                  const float* lr_t_dev, void* stream) {
+  DR_REQUIRE(n_tensors >= 0, DR_EINVAL, "dr_adam_step_multi: n_tensors=%d < 0", n_tensors);
+  if (n_tensors == 0) return DR_OK;
+  DR_REQUIRE(p && g && m && v && n, DR_EINVAL, "dr_adam_step_multi: null pointer array");
+  if (int rc = check_adam_hparams("dr_adam_step_multi", beta1, beta2, eps)) return rc;
+  for (int i = 0; i < n_tensors; ++i) {      // every tensor is checked before the first launch
+    DR_REQUIRE(n[i] >= 0, DR_EINVAL, "dr_adam_step_multi: n[%d]=%lld < 0", i, (long long)n[i]);
+    DR_REQUIRE(n[i] == 0 || (p[i] && g[i] && m[i] && v[i]), DR_EINVAL, "dr_adam_step_multi: null pointer in tensor %d",
+               i);
+    DR_REQUIRE(n[i] / kMultiChunk < INT32_MAX, DR_EINVAL, "dr_adam_step_multi: n[%d]=%lld too large", i,
+               (long long)n[i]);
+  }
+  AdamMultiArgs a;
+  a.count = 0;
+  a.vec = 0;
+  int32_t grid = 0;
+  auto launch = [&]() -> int {
+    a.chunk0[a.count] = grid;
+    adam_multi_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(a, lr_t, 1.f - beta1, 1.f - beta2, eps,
+                                                                        lr_t_dev);
+    DR_CUDA_LAUNCH_CHECK("dr_adam_step_multi");
+    a.count = 0;
+    a.vec = 0;
+    grid = 0;
+    return DR_OK;
+  };
+  for (int i = 0; i < n_tensors; ++i) {
+    if (n[i] == 0) continue;
+    const int32_t chunks = (int32_t)((n[i] + kMultiChunk - 1) / kMultiChunk);
+    if (a.count == kMultiTensors || grid > INT32_MAX - chunks)
+      if (int rc = launch()) return rc;
+    const int k = a.count++;
+    a.p[k] = p[i]; a.g[k] = g[i]; a.m[k] = m[i]; a.v[k] = v[i];
+    a.n[k] = n[i];
+    a.chunk0[k] = grid;
+    if (aligned16(p[i]) && aligned16(g[i]) && aligned16(m[i]) && aligned16(v[i])) a.vec |= 1ull << k;
+    grid += chunks;
+  }
+  return a.count ? launch() : DR_OK;
+}
+
 // ---- step counter on the device: t += 1, lr_t = lr * sqrt(1 - b2^t) / (1 - b1^t) -------------------------------
 // Keras optimizer_v2 Adam._prepare_local: local_step = iterations + 1, beta powers in the variable dtype.  Keeping
 // t and lr_t in device memory lets the whole train step (incl. the optimizer) replay as one CUDA graph.

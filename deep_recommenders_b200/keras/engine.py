@@ -261,6 +261,16 @@ class TrainingLoopMixin:
             raise RuntimeError("call compile() before reading the optimizer")
         return _OptimizerHandle(self)
 
+    def _build_optimizer(self):
+        """A spec with build_for_model (optimizers.KerasAdam) takes the whole model; any other builds a torch optimizer
+        over the trainable parameters, after the tables of an earlier KerasAdam are handed back to it."""
+        spec = self._optimizer_spec
+        if hasattr(spec, "build_for_model"):
+            return spec.build_for_model(self)
+        from ..optimizers import release_row_optimizers
+        release_row_optimizers(self)
+        return spec.build([p for p in self.parameters() if p.requires_grad])
+
     def _step_loss(self, x, y, sample_weight=None):
         """Keras's SUM_OVER_BATCH_SIZE: mean over the rows of w * loss (w = 1 without a sample weight)."""
         pred = self(x)
@@ -336,7 +346,7 @@ class TrainingLoopMixin:
             for batch in itertools.islice(stream, steps_per_epoch):
                 pred, yt, w, loss = self._step_loss(*_unpack(batch))
                 if self._optimizer is None:        # parameters of lazily built layers exist after the first forward
-                    self._optimizer = self._optimizer_spec.build([p for p in self.parameters() if p.requires_grad])
+                    self._optimizer = self._build_optimizer()
                 self._optimizer.zero_grad(set_to_none=True)
                 loss.backward()
                 self._optimizer.step()

@@ -983,6 +983,26 @@ def adam_step_(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tenso
           "dr_adam_step")
 
 
+def adam_step_multi_(params, grads, ms, vs, clock: "AdamClock") -> None:
+    """adam_step_(p, g, m, v, zero_grad=False, lr_t_dev=clock.lr_t) for every (p, g, m, v) of the four lists, in one
+    launch per 64 tensors (dr_adam_step_multi) and bitwise equal to the per-tensor calls.  Every tensor is a contiguous
+    CUDA float32 tensor with as many elements as its p; the gradients are only read."""
+    import ctypes as C
+    lib = _lib.load()
+    k = len(params)
+    if not (len(grads) == len(ms) == len(vs) == k):
+        raise ValueError(f"adam_step_multi_: {k} params, {len(grads)} grads, {len(ms)} m, {len(vs)} v")
+    for i, p in enumerate(params):
+        for name, t in (("p", p), ("g", grads[i]), ("m", ms[i]), ("v", vs[i])):
+            _f32(t, f"{name}[{i}]")
+            if not t.is_contiguous() or t.numel() != p.numel():
+                raise ValueError(f"adam_step_multi_: {name}[{i}] must be contiguous with {p.numel()} elements")
+    ptrs = lambda ts: (C.c_void_p * max(k, 1))(*[t.data_ptr() for t in ts])
+    ns = (C.c_int64 * max(k, 1))(*[p.numel() for p in params])
+    check(lib.dr_adam_step_multi(k, ptrs(params), ptrs(grads), ptrs(ms), ptrs(vs), ns, 0.0, clock.beta1, clock.beta2,
+                                 clock.eps, clock.lr_t.data_ptr(), _stream()), "dr_adam_step_multi")
+
+
 class AdamClock:
     """Device-resident step counter t and bias-corrected rate lr_t = lr * sqrt(1 - b2^t) / (1 - b1^t)
     (Keras optimizer_v2 Adam._prepare_local), advanced by one kernel so a captured train step needs no host scalar."""

@@ -16,6 +16,9 @@ sweep is the step.  RowSparseAdam gives the same numbers while it touches only t
 
 The rates of the replayed steps come from the clock's ring of bias-corrected rates (AdamClock(history=1 << 16)), or are
 recomputed for steps that fell out of it; steps more than kCatchUpMax = 2048 behind only decay m and v, in closed form.
+
+KerasAdam is tf.keras.optimizers.Adam for a whole Keras model (compile(optimizer=KerasAdam())): a RowSparseAdam per
+EmbeddingCollection and every other variable in one multi-tensor dense update (ops.adam_step_multi_), on one clock.
 """
 from __future__ import annotations
 
@@ -154,6 +157,11 @@ class RowSparseAdam:
         B = splits.numel() - 1
         self._pending.append(_Rows(ids, B, 1, splits, int(slot), g, g_off, g_ld, 0, gl, gl_off, gl_ld, 0))
 
+    @property
+    def has_pending(self) -> bool:
+        """Whether a backward recorded lookups since the last step(), i.e. whether step() has anything to apply."""
+        return bool(self._pending)
+
     # ---- the update ---------------------------------------------------------------------------------------------------
     def step(self) -> None:
         """Apply step t (the clock's current step, after its advance) to every row the recorded backwards touched."""
@@ -206,3 +214,111 @@ class RowSparseAdam:
         check(lib.dr_embed_adam_flush(rows.data_ptr(), offs.data_ptr(), c.num_slots, c.dim, c.total_rows, c.row_stride,
                                       c.lin_stride, flags, tp.data_ptr(), ops._ptr(lp), self.state.data_ptr(), step, hist,
                                       hist_len, ck.lr, ck.beta1, ck.beta2, ck.eps, ops._stream()), "dr_embed_adam_flush")
+
+
+class KerasAdam:
+    """tf.keras.optimizers.Adam(learning_rate, beta_1, beta_2, epsilon) for a whole Keras model, with TensorFlow's
+    arithmetic (ApplyAdam: eps is added to sqrt(v), the bias correction is folded into lr_t), where the engine's `Adam`
+    builds torch.optim.Adam.  Use it as `model.compile(optimizer=KerasAdam(...))`; fit() calls build_for_model(model)
+    after the first forward.
+
+    The build walks the model.  tables="rows" (the default) puts every EmbeddingCollection's `weight` (and split
+    `linear`) arena on a RowSparseAdam, all of them and the dense variables on one AdamClock: the same numbers as dense
+    Adam over the tables, at the cost of the rows a batch reads (4 D + 32 floats of state per row, rounded up to 32).
+    Every other trainable parameter -- the collections' `bias`, towers, Cross / CIN / attention weights, `Gather` tables
+    -- is in the dense group, whose m and v are two flat arenas stepped by one ops.adam_step_multi_.  tables="dense" keeps
+    the arenas in the dense group: the same update swept over every row.
+
+    step(): advance the clock with the current learning rate, update the dense variables that have a gradient (as
+    Keras's apply_gradients, a variable without one is left alone), then apply the step to the rows of every collection
+    that a backward read.  A collection that no forward read this step is not stepped; its rows replay the step when
+    they are next read.  param_groups[0]["lr"] (the engine's model.optimizer.lr) takes effect at the next step(), and the
+    clock's ring of rates keeps each step's own lr_t for those replays.
+
+    Rejected: amsgrad=True (NotImplementedError); a collection built with sparse_lr, whose backward applies fused SGD,
+    and a collection already carrying a RowSparseAdam that the user attached (ValueError).  A RowSparseAdam of an
+    earlier KerasAdam build on the same model is flushed and released, so a recompiled model starts from fresh slots at
+    step 1, as a new Keras optimizer does.  Slots are not saved by state_dict().
+    """
+
+    def __init__(self, learning_rate=0.001, beta_1=0.9, beta_2=0.999, epsilon=1e-7, amsgrad=False, tables="rows"):
+        if amsgrad:
+            raise NotImplementedError("KerasAdam: amsgrad=True is not implemented")
+        if tables not in ("rows", "dense"):
+            raise ValueError(f"KerasAdam: tables={tables!r}; expected 'rows' or 'dense'")
+        self.beta_1, self.beta_2, self.epsilon = float(beta_1), float(beta_2), float(epsilon)
+        self.tables = tables
+        # the engine reads and writes the rate as spec.kw["lr"] before the build and param_groups[0]["lr"] after it
+        self.kw = {"lr": float(learning_rate)}
+        self.param_groups = [self.kw]
+        self.clock = None
+        self.dense = []            # (parameter, m, v) of the dense group
+        self.row_optimizers = []   # one RowSparseAdam per collection (tables="rows")
+
+    def build_for_model(self, model) -> "KerasAdam":
+        from .embedding import EmbeddingCollection
+        colls = [mod for mod in model.modules() if isinstance(mod, EmbeddingCollection)]
+        for c in colls:
+            if c.sparse_lr is not None:
+                raise ValueError("KerasAdam: an EmbeddingCollection of the model trains with fused SGD (sparse_lr); "
+                                 "build the model with sparse_lr=None")
+            if c.row_optimizer is not None and not getattr(c.row_optimizer, "_keras_adam", False):
+                raise ValueError("KerasAdam: an EmbeddingCollection of the model already has a RowSparseAdam attached")
+        params = [p for p in model.parameters() if p.requires_grad]
+        if not params:
+            raise ValueError("KerasAdam: the model has no trainable parameters")
+        release_row_optimizers(model)
+        b1, b2, eps, lr = self.beta_1, self.beta_2, self.epsilon, self.kw["lr"]
+        self.clock = ops.AdamClock(lr, b1, b2, eps, device=params[0].device, history=HISTORY)
+        self.row_optimizers, on_rows = [], set()
+        if self.tables == "rows":
+            for c in colls:
+                if not c.weight.requires_grad:
+                    continue
+                ro = RowSparseAdam(c, lr, b1, b2, eps, clock=self.clock)
+                ro._keras_adam = True
+                self.row_optimizers.append(ro)
+                on_rows.update(id(t) for t in (c.weight, c.linear) if t is not None)
+        dense = [p for p in params if id(p) not in on_rows]
+        offsets, total = [], 0
+        for p in dense:
+            if not p.is_contiguous():
+                raise ValueError(f"KerasAdam: a parameter of shape {tuple(p.shape)} is not contiguous")
+            offsets.append(total)
+            total += (p.numel() + 3) // 4 * 4          # every variable's m and v start 16-B aligned
+        m = torch.zeros((total,), dtype=torch.float32, device=params[0].device)
+        v = torch.zeros_like(m)
+        self.dense = [(p, m[o:o + p.numel()].view_as(p), v[o:o + p.numel()].view_as(p)) for p, o in zip(dense, offsets)]
+        return self
+
+    def zero_grad(self, set_to_none: bool = True) -> None:
+        for p, _, _ in self.dense:
+            if p.grad is None:
+                continue
+            if set_to_none:
+                p.grad = None
+            else:
+                p.grad.detach_().zero_()
+
+    def step(self) -> None:
+        if self.clock is None:
+            raise RuntimeError("KerasAdam.step(): build_for_model(model) first")
+        self.clock.lr = float(self.kw["lr"])
+        self.clock.advance()
+        live = [(p, p.grad, m, v) for p, m, v in self.dense if p.grad is not None]
+        if live:
+            ps, gs, ms, vs = zip(*live)
+            ops.adam_step_multi_(ps, [g.contiguous() for g in gs], ms, vs, self.clock)
+        for ro in self.row_optimizers:
+            if ro.has_pending:
+                ro.step()
+
+
+def release_row_optimizers(model) -> None:
+    """Flush the RowSparseAdam a KerasAdam build attached to each EmbeddingCollection of `model` and detach it: the
+    tables then hold what dense Adam would and train with whatever optimizer the model is compiled with next."""
+    from .embedding import EmbeddingCollection
+    for c in model.modules():
+        if isinstance(c, EmbeddingCollection) and getattr(c.row_optimizer, "_keras_adam", False):
+            c.row_optimizer.flush()
+            c.row_optimizer = None

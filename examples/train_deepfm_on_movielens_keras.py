@@ -6,6 +6,9 @@ import lines below; the rest reads like the reference script.  Data: the real TF
 directory is given, else SYNTHETIC MovieLens-1M-shaped batches (no network here).
 
     python examples/train_deepfm_on_movielens_keras.py [--steps-per-epoch N] [--epochs E] [--data DIR]
+                                                        [--optimizer {keras,tf}]
+--optimizer keras (the default) compiles with the engine's Adam (torch.optim.Adam); tf compiles with
+optimizers.KerasAdam(), TensorFlow's Adam arithmetic with the embedding tables trained row-sparse.
 Needs a CUDA device (the layers run in libdeeprec_b200.so; there is no CPU fallback).
 """
 import argparse
@@ -18,6 +21,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from deep_recommenders_b200 import feature_column as fc  # noqa: E402     (tf.feature_column)
 from deep_recommenders_b200.keras import engine as K  # noqa: E402          (tf.keras.losses / optimizers / metrics / callbacks)
 from deep_recommenders.keras.models.ranking import DeepFM  # noqa: E402
+from deep_recommenders_b200.optimizers import KerasAdam  # noqa: E402
 
 NUM_USERS, NUM_MOVIES = 6040, 3952
 GENDER_VOCAB = ["F", "M"]
@@ -59,6 +63,8 @@ def main():
     ap.add_argument("--steps-per-epoch", type=int, default=50)
     ap.add_argument("--validation-steps", type=int, default=10)
     ap.add_argument("--data", default=None, help="MovieLens TFRecord directory (datasets.MovielensRanking); default synthetic")
+    ap.add_argument("--optimizer", choices=["keras", "tf"], default="keras",
+                    help="keras: the engine's Adam (torch.optim.Adam); tf: optimizers.KerasAdam (TensorFlow's Adam)")
     args = ap.parse_args()
     indicator_columns, embedding_columns = build_columns()
     if args.data:
@@ -71,7 +77,7 @@ def main():
 
     model = DeepFM(indicator_columns, embedding_columns, dnn_units_size=[256, 32], seed=0, device="cuda")
     model.compile(loss=K.binary_crossentropy,
-                  optimizer=K.Adam(),
+                  optimizer=K.Adam() if args.optimizer == "keras" else KerasAdam(),
                   metrics=[K.AUC(), K.Precision(), K.Recall()])
     history = model.fit(train,
                         epochs=args.epochs,

@@ -536,6 +536,19 @@ int dr_dcn_head_bce_fwd_bwd(const float* x_cross, const float* deep, const float
 int dr_adam_step(float* p, float* g, float* m, float* v, int64_t n, float lr_t, float beta1, float beta2,
                  float eps, int zero_grad, const float* lr_t_dev, void* stream);
 
+/* dr_adam_step (zero_grad = 0) over n_tensors flat tensors p[i], g[i], m[i], v[i] of n[i] floats each, in one launch
+ * per 64 non-empty tensors: the dense half of tf.keras.optimizers.Adam over a whole model, which the reference compiles
+ * every Keras model with (examples/train_deepfm_on_movielens_keras.py:44 `Adam()`, train_gcn_on_cora_keras.py:29
+ * `Adam(0.01)`, train_transformer_on_imdb_keras.py:45 `Adam(beta_1=0.9, beta_2=0.98, epsilon=1e-9)`).  Every element
+ * is bitwise what dr_adam_step gives it: a tensor whose four pointers are 16-B aligned takes the float4 path, any other
+ * and every tail the scalar one.  The arrays are host memory, read before the call returns; their contents travel in
+ * the kernel's argument block (no copy, no synchronisation: graph-capturable).  lr_t_dev (nullable) overrides lr_t.
+ * n[i] = 0 skips tensor i (its pointers may be NULL); a negative n, a NULL pointer of a non-empty tensor or an
+ * out-of-range beta / eps returns DR_EINVAL before any launch. */
+int dr_adam_step_multi(int n_tensors, float* const* p, float* const* g, float* const* m, float* const* v,
+                       const int64_t* n, float lr_t, float beta1, float beta2, float eps, const float* lr_t_dev,
+                       void* stream);
+
 /* Step counter on the device (Keras optimizer_v2 Adam._prepare_local): *step_dev += 1 and
  * *lr_t_dev = lr * sqrt(1 - beta2^t) / (1 - beta1^t) with t the incremented step (first call: t = 1).         */
 int dr_adam_advance(int64_t* step_dev, float lr, float beta1, float beta2, float* lr_t_dev, void* stream);
