@@ -1,8 +1,7 @@
 // TensorFlow's Adam as the optimizer kernels of optim.cu and embed_adam.cu share it: the ApplyAdam functor, the replay
-// of the steps a row sat out, one lane's share of a row's replay and update, and the host-side argument check and
-// launch dispatch of their entries.
+// of the steps a row sat out, one lane's share of a row's replay and update, and the host-side check of their
+// hyperparameters.
 #pragma once
-#include <type_traits>
 #include "common.cuh"
 
 namespace dr {
@@ -157,40 +156,6 @@ static inline int check_adam_hparams(const char* fn, float beta1, float beta2, f
   DR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, DR_EINVAL,
              "%s: beta1=%g beta2=%g eps=%g out of range", fn, (double)beta1, (double)beta2, (double)eps);
   return DR_OK;
-}
-
-// Lanes per row for `chunks` 16-B chunks: the next power of two.
-static inline int lanes_per_row(int chunks) {
-  int lpr = 1;
-  while (lpr < chunks) lpr <<= 1;
-  return lpr;
-}
-
-// ceil(items / per_cta) CTAs, at most ctas_per_sm per SM
-static inline int64_t capped_grid(int64_t items, int64_t per_cta, int ctas_per_sm) {
-  const int64_t ctas = (items + per_cta - 1) / per_cta, cap = (int64_t)num_sms() * ctas_per_sm;
-  return ctas > cap ? cap : ctas;
-}
-
-// f(std::integral_constant<int, LPR>{}) for lpr in {1, 2, 4, 8, 16}; any other lpr runs as 32.
-template <int LPR = 1, typename F>
-inline void with_lpr(int lpr, F&& f) {
-  if constexpr (LPR == 32) {
-    f(std::integral_constant<int, 32>{});
-  } else {
-    if (lpr == LPR) f(std::integral_constant<int, LPR>{});
-    else with_lpr<2 * LPR>(lpr, f);
-  }
-}
-// f(IdT{}) with IdT = int64_t for id_bytes 8, int32_t otherwise
-template <typename F>
-inline void with_id_type(int id_bytes, F&& f) {
-  if (id_bytes == 8) f(int64_t{});
-  else f(int32_t{});
-}
-template <typename F>
-inline void with_lpr_id(int lpr, int id_bytes, F&& f) {
-  with_lpr(lpr, [&](auto L) { with_id_type(id_bytes, [&](auto id) { f(L, id); }); });
 }
 
 }  // namespace dr

@@ -123,18 +123,15 @@ extern "C" int dr_embed_bag_fwd(const float* table, int64_t rows, int64_t row_st
   DR_REQUIRE(out_stride >= D, DR_EINVAL, "dr_embed_bag_fwd: out_stride=%lld < D=%d", (long long)out_stride, D);
   const bool vec = (D % 4 == 0) && (row_stride % 4 == 0) && (out_stride % 4 == 0) && aligned16(table) && aligned16(out);
   const int group = bag_group(vec ? D / 4 : D);
-  const int per_block = 256 / group;
-  int64_t ctas = (B + per_block - 1) / per_block;
-  if (ctas > num_sms() * 16) ctas = num_sms() * 16;
-  cudaStream_t st = (cudaStream_t)stream;
-#define DR_BAG_FWD(IdT, VEC)                                                                                     \
-  embed_bag_fwd_kernel<IdT, VEC><<<(unsigned)ctas, 256, 0, st>>>(table, rows, row_stride, (const IdT*)ids,        \
-                                                                 row_splits, B, D, combiner, group, out, out_stride)
-  if (id_bytes == 8) { if (vec) DR_BAG_FWD(int64_t, 4); else DR_BAG_FWD(int64_t, 1); }
-  else               { if (vec) DR_BAG_FWD(int32_t, 4); else DR_BAG_FWD(int32_t, 1); }
-#undef DR_BAG_FWD
-  DR_CUDA_LAUNCH_CHECK("embed_bag_fwd");
-  return DR_OK;
+  const int64_t ctas = capped_grid(B, 256 / group, 16);
+  return with_id_type(id_bytes, [&](auto id) {
+    using IdT = decltype(id);
+    auto k = vec ? embed_bag_fwd_kernel<IdT, 4> : embed_bag_fwd_kernel<IdT, 1>;
+    k<<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(table, rows, row_stride, (const IdT*)ids, row_splits, B, D,
+                                                        combiner, group, out, out_stride);
+    DR_CUDA_LAUNCH_CHECK("embed_bag_fwd");
+    return DR_OK;
+  });
 }
 
 extern "C" int dr_embed_bag_bwd(const void* ids, int id_bytes, const int64_t* row_splits, int64_t B, int D,
@@ -146,16 +143,13 @@ extern "C" int dr_embed_bag_bwd(const void* ids, int id_bytes, const int64_t* ro
   DR_REQUIRE(g_stride >= D, DR_EINVAL, "dr_embed_bag_bwd: g_stride=%lld < D=%d", (long long)g_stride, D);
   const bool vec = (D % 4 == 0) && (row_stride % 4 == 0) && (g_stride % 4 == 0) && aligned16(grad_table) && aligned16(g_out);
   const int group = bag_group(vec ? D / 4 : D);
-  const int per_block = 256 / group;
-  int64_t ctas = (B + per_block - 1) / per_block;
-  if (ctas > num_sms() * 16) ctas = num_sms() * 16;
-  cudaStream_t st = (cudaStream_t)stream;
-#define DR_BAG_BWD(IdT, VEC)                                                                                     \
-  embed_bag_bwd_kernel<IdT, VEC><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, row_splits, B, D, combiner,     \
-                                                                 group, g_out, g_stride, rows, row_stride, grad_table, scale)
-  if (id_bytes == 8) { if (vec) DR_BAG_BWD(int64_t, 4); else DR_BAG_BWD(int64_t, 1); }
-  else               { if (vec) DR_BAG_BWD(int32_t, 4); else DR_BAG_BWD(int32_t, 1); }
-#undef DR_BAG_BWD
-  DR_CUDA_LAUNCH_CHECK("embed_bag_bwd");
-  return DR_OK;
+  const int64_t ctas = capped_grid(B, 256 / group, 16);
+  return with_id_type(id_bytes, [&](auto id) {
+    using IdT = decltype(id);
+    auto k = vec ? embed_bag_bwd_kernel<IdT, 4> : embed_bag_bwd_kernel<IdT, 1>;
+    k<<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>((const IdT*)ids, row_splits, B, D, combiner, group, g_out,
+                                                        g_stride, rows, row_stride, grad_table, scale);
+    DR_CUDA_LAUNCH_CHECK("embed_bag_bwd");
+    return DR_OK;
+  });
 }

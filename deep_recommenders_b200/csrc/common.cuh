@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
+#include <type_traits>
 #include "deeprec_b200.h"
 
 #ifndef __CUDA_ARCH_LIST__
@@ -51,6 +52,57 @@ void count_launch(int n = 1);
   } while (0)
 
 __host__ __device__ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// ---- host side of the entries: argument checks and launch dispatch ------------------------------------------------------
+// The shape and id-width checks of the lookup entries, in this order.  `d_join` joins the two conditions of the D
+// message: the embedding entries print " and", the FNN entries ",".
+static inline int check_lookup_dims(const char* fn, int64_t B, int S, int D, int id_bytes, const char* d_join = " and") {
+  DR_REQUIRE(B >= 0, DR_EINVAL, "%s: B=%lld < 0", fn, (long long)B);
+  DR_REQUIRE(S >= 1 && S <= 4096, DR_EINVAL, "%s: S=%d outside [1,4096]", fn, S);
+  DR_REQUIRE(D >= 4 && D <= 128 && (D % 4) == 0, DR_EINVAL,
+             "%s: D=%d unsupported (need D %% 4 == 0%s 4 <= D <= 128)", fn, D, d_join);
+  DR_REQUIRE(id_bytes == 8 || id_bytes == 4, DR_EINVAL, "%s: id_bytes=%d (need 4 or 8)", fn, id_bytes);
+  return DR_OK;
+}
+
+// Lanes per row for `chunks` 16-B chunks: the next power of two.
+static inline int lanes_per_row(int chunks) {
+  int lpr = 1;
+  while (lpr < chunks) lpr <<= 1;
+  return lpr;
+}
+
+// ceil(items / per_cta) CTAs, at most ctas_per_sm per SM
+static inline int64_t capped_grid(int64_t items, int64_t per_cta, int ctas_per_sm) {
+  const int64_t ctas = (items + per_cta - 1) / per_cta, cap = (int64_t)num_sms() * ctas_per_sm;
+  return ctas > cap ? cap : ctas;
+}
+
+// A kernel launched with more than 48 KB of dynamic shared memory has to be allowed that much first.
+template <typename Kernel>
+static inline int allow_dynamic_smem(Kernel* k, size_t smem) {
+  if (smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  return DR_OK;
+}
+
+// f(std::integral_constant<int, LPR>{}) for lpr in {MIN, 2 MIN, ..., MAX}; any other lpr runs as MAX.  Returns f's code,
+// and instantiates f for those lane counts only.
+template <int MAX = 32, int MIN = 1, typename F>
+inline int with_lpr(int lpr, F&& f) {
+  if constexpr (MIN >= MAX) return f(std::integral_constant<int, MAX>{});
+  else if (lpr == MIN) return f(std::integral_constant<int, MIN>{});
+  else return with_lpr<MAX, 2 * MIN>(lpr, f);
+}
+// f(IdT{}) with IdT = int64_t for id_bytes 8, int32_t otherwise
+template <typename F>
+inline int with_id_type(int id_bytes, F&& f) {
+  if (id_bytes == 8) return f(int64_t{});
+  return f(int32_t{});
+}
+template <int MAX = 32, typename F>
+inline int with_lpr_id(int lpr, int id_bytes, F&& f) {
+  return with_lpr<MAX>(lpr, [&](auto L) { return with_id_type(id_bytes, [&](auto id) { return f(L, id); }); });
+}
 
 // ---- device helpers -------------------------------------------------------------------
 #ifdef __CUDACC__

@@ -599,13 +599,13 @@ extern "C" int dr_embed_adam_count(const void* ids, int id_bytes, int64_t B, int
   DR_REQUIRE(ids && rows && slot_offsets && state, DR_EINVAL, "dr_embed_adam_count: null pointer");
   const int64_t n = B * S;
   const int64_t ctas = capped_grid(n, 256, 16);
-  with_id_type(id_bytes, [&](auto id) {
+  return with_id_type(id_bytes, [&](auto id) {
     using IdT = decltype(id);
     embed_adam_count_kernel<IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
         (const IdT*)ids, n, S, rows, slot_offsets, state, adam_state_stride(D), 3 * D + 3);
+    DR_CUDA_LAUNCH_CHECK("dr_embed_adam_count");
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK("dr_embed_adam_count");
-  return DR_OK;
 }
 
 static int embed_fm_bwd_adam_impl(const char* fn, const void* ids, int id_bytes, const int64_t* rows,
@@ -643,13 +643,13 @@ static int embed_fm_bwd_adam_impl(const char* fn, const void* ids, int id_bytes,
   const size_t smem = (size_t)S * (sizeof(void*) * 2 + sizeof(int64_t) * 2);
   const int64_t ctas = capped_grid(B, warps, 8);
   cudaStream_t st = (cudaStream_t)stream;
-  with_lpr_id(lanes_per_row(D / 4), id_bytes, [&](auto L, auto id) {
+  return with_lpr_id(lanes_per_row(D / 4), id_bytes, [&](auto L, auto id) {
     using IdT = decltype(id);
     if (exact) embed_fm_bwd_adam_kernel<L, IdT, true><<<(unsigned)ctas, threads, smem, st>>>(p);
     else embed_fm_bwd_adam_kernel<L, IdT, false><<<(unsigned)ctas, threads, smem, st>>>(p);
+    DR_CUDA_LAUNCH_CHECK(fn);
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK(fn);
-  return DR_OK;
 }
 
 extern "C" int dr_embed_fm_bwd_adam(const void* ids, int id_bytes, const int64_t* rows, const int64_t* slot_offsets,
@@ -703,14 +703,14 @@ extern "C" int dr_embed_adam_prepare(const void* ids, int id_bytes, int64_t B, i
   const int lpr = lanes_per_row(D / 4);
   const int64_t n = B * S;
   const int64_t ctas = capped_grid(n * lpr, 256, 16);
-  with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
+  return with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
     using IdT = decltype(id);
     embed_adam_prepare_kernel<L, IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
         (const IdT*)ids, n, S, D, rows, slot_offsets, table_ptrs, lin_in_row ? nullptr : lin_ptrs, row_stride, lin_stride,
         lin_in_row, state, adam_state_stride(D), step_dev, h, 1.f - beta1, 1.f - beta2, eps);
+    DR_CUDA_LAUNCH_CHECK("dr_embed_adam_prepare");
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK("dr_embed_adam_prepare");
-  return DR_OK;
 }
 
 extern "C" int dr_embed_adam_flush(const int64_t* rows, const int64_t* slot_offsets, int S, int D, int64_t total_rows,
@@ -727,13 +727,13 @@ extern "C" int dr_embed_adam_flush(const int64_t* rows, const int64_t* slot_offs
   const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
   const int lpr = lanes_per_row(D / 4);
   const int64_t ctas = capped_grid(total_rows * lpr, 256, 16);
-  with_lpr(lpr, [&](auto L) {
+  return with_lpr(lpr, [&](auto L) {
     embed_adam_flush_kernel<L><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
         table_ptrs, lin_in_row ? nullptr : lin_ptrs, rows, slot_offsets, S, D, row_stride, lin_stride, lin_in_row, state,
         adam_state_stride(D), total_rows, step_dev, h, 1.f - beta1, 1.f - beta2, eps);
+    DR_CUDA_LAUNCH_CHECK("dr_embed_adam_flush");
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK("dr_embed_adam_flush");
-  return DR_OK;
 }
 
 // ---- tf.keras Adam of the layer API (see embed_adam_catch_up_kernel) --------------------------------------------------
@@ -768,14 +768,14 @@ extern "C" int dr_embed_adam_catch_up(const void* ids, int id_bytes, int64_t n, 
   const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
   const int lpr = lanes_per_row(D / 4);
   const int64_t ctas = capped_grid(n * lpr, 256, 16);
-  with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
+  return with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
     using IdT = decltype(id);
     embed_adam_catch_up_kernel<L, IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
         (const IdT*)ids, n, S, D, rows, slot_offsets, table_ptrs, lin_ptrs, row_stride, lin_stride, lin_in_row, state,
         adam_state_stride(D), step_dev, h, 1.f - beta1, 1.f - beta2, eps);
+    DR_CUDA_LAUNCH_CHECK(fn);
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK(fn);
-  return DR_OK;
 }
 
 extern "C" int dr_embed_adam_rows_tf(const void* ids, int id_bytes, int64_t n, int64_t B, int S,
@@ -816,13 +816,13 @@ extern "C" int dr_embed_adam_rows_tf(const void* ids, int id_bytes, int64_t n, i
   const int lpr = lanes_per_row(D / 4);
   const int64_t ctas = capped_grid(n * lpr, 256, 16);
   cudaStream_t st = (cudaStream_t)stream;
-  with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
+  return with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
     using IdT = decltype(id);
     if (row_splits) embed_adam_rows_tf_kernel<L, IdT, true><<<(unsigned)ctas, 256, 0, st>>>(p);
     else embed_adam_rows_tf_kernel<L, IdT, false><<<(unsigned)ctas, 256, 0, st>>>(p);
+    DR_CUDA_LAUNCH_CHECK(fn);
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK(fn);
-  return DR_OK;
 }
 
 // ---- row-sharded tf.keras Adam (see shard_adam_mark_kernel) -----------------------------------------------------------
@@ -836,13 +836,13 @@ extern "C" int dr_shard_adam_mark(const void* ids, int id_bytes, int64_t n, int 
   DR_REQUIRE(ids && slot_offsets && rows && touch_bases && step_dev, DR_EINVAL, "dr_shard_adam_mark: null pointer");
   if (n == 0) return DR_OK;
   const int64_t ctas = capped_grid(n, 256, 16);
-  with_id_type(id_bytes, [&](auto id) {
+  return with_id_type(id_bytes, [&](auto id) {
     using IdT = decltype(id);
     shard_adam_mark_kernel<IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>((const IdT*)ids, n, S, slot_offsets,
                                                                                  rows, world, touch_bases, step_dev);
+    DR_CUDA_LAUNCH_CHECK("dr_shard_adam_mark");
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK("dr_shard_adam_mark");
-  return DR_OK;
 }
 
 static int shard_adam_layout_check(const char* fn, int64_t local_rows, int D, int64_t row_stride, int64_t lin_offset,
@@ -875,13 +875,13 @@ extern "C" int dr_shard_adam_prepare(int32_t* touch, int64_t local_rows, int32_t
   const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
   const AdamHist h{lr_hist, hist_len, lr, beta1, beta2};
   const int64_t ctas = capped_grid(local_rows, 256, 16);
-  with_lpr(lanes_per_row(D / 4), [&](auto L) {
+  return with_lpr(lanes_per_row(D / 4), [&](auto L) {
     shard_adam_prepare_kernel<L><<<(unsigned)ctas, 256, 0, st>>>(touch, local_rows, list, count, shard, row_stride,
                                                                  lin_offset, lin_in_row, state, adam_state_stride(D), D,
                                                                  step_dev, h, 1.f - beta1, 1.f - beta2, eps);
+    DR_CUDA_LAUNCH_CHECK(fn);
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK(fn);
-  return DR_OK;
 }
 
 extern "C" int dr_shard_adam_apply(const int32_t* list, const int32_t* count, int64_t local_rows, int D,
@@ -898,11 +898,11 @@ extern "C" int dr_shard_adam_apply(const int32_t* list, const int32_t* count, in
   const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
   const int lpr = lanes_per_row(D / 4);
   const int64_t ctas = capped_grid(local_rows * lpr, 256, 16);
-  with_lpr(lpr, [&](auto L) {
+  return with_lpr(lpr, [&](auto L) {
     shard_adam_apply_kernel<L><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
         list, count, shard, grad, row_stride, lin_offset, lin_in_row, state, adam_state_stride(D), D, step_dev, lr_t_dev,
         1.f - beta1, 1.f - beta2, eps);
+    DR_CUDA_LAUNCH_CHECK(fn);
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK(fn);
-  return DR_OK;
 }

@@ -551,80 +551,57 @@ __global__ void __launch_bounds__(256) scatter_add_rows_kernel(float* __restrict
 }
 
 // ---- host-side dispatch -----------------------------------------------------------------
-static int lpr_for(int D, int lin_in_row = 0) {
-  int chunks = D / 4 + (lin_in_row ? 1 : 0), l = 1;
-  while (l < chunks) l <<= 1;
-  return l;
-}
-
 struct LaunchGeom {
   int threads, ctas;
   size_t smem;
 };
 
+// B >= 1: the entries return before a launch at B = 0
 static LaunchGeom geom(int64_t B, int S, int LPR, int id_bytes) {
   LaunchGeom lg;
   lg.threads = g_tune_embed_block;
   if (lg.threads != 128 && lg.threads != 256 && lg.threads != 512) lg.threads = 256;
   const int warps = lg.threads / 32, G = 32 / LPR;
   lg.smem = embed_smem_bytes(S, warps, G, id_bytes);
-  const int64_t ntiles = (B + G - 1) / G;
-  int64_t ctas = (ntiles + warps - 1) / warps;
   int per_sm = 2048 / lg.threads;
   if (g_tune_embed_ctas_per_sm > 0 && g_tune_embed_ctas_per_sm < per_sm) per_sm = g_tune_embed_ctas_per_sm;
-  const int64_t cap = (int64_t)num_sms() * per_sm;
-  if (ctas > cap) ctas = cap;
-  if (ctas < 1) ctas = 1;
-  lg.ctas = (int)ctas;
+  lg.ctas = (int)capped_grid((B + G - 1) / G, warps, per_sm);
   return lg;
+}
+
+template <typename Params>
+static int launch(void (*k)(Params), const LaunchGeom& lg, const Params& p, cudaStream_t st, const char* what) {
+  if (int rc = allow_dynamic_smem(k, lg.smem)) return rc;
+  k<<<lg.ctas, lg.threads, lg.smem, st>>>(p);
+  DR_CUDA_LAUNCH_CHECK(what);
+  return DR_OK;
 }
 
 template <int LPR, typename IdT, int U, bool LINXSEL = false>
 static int launch_fwd_u(const EmbedFwdParams& p, cudaStream_t st) {
+  // experiment instantiations (same arithmetic, same results): narrow rows, U = 8 / 13 only
+  //   MINB 3 / 4: register cap via __launch_bounds__(256, n);  LINX: see the kernel comment
+  constexpr bool kExp = (LPR <= 8) && (U == 8 || U == 13);
+  constexpr int UU = kExp ? U : 8;
+  static_assert(!LINXSEL || kExp, "LINX is instantiated for LPR <= 8 and U in {8, 13} only");
   LaunchGeom lg = geom(p.B, p.S, LPR, sizeof(IdT));
   if (p.shard_world > 0) {
-    if (LINXSEL && LPR <= 8 && U == 8) {
-      auto k = embed_fm_fwd_kernel<LPR, IdT, (LPR <= 8 && U == 8) ? U : 8, true, 0, LINXSEL>;
-      if (lg.smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lg.smem));
-      k<<<lg.ctas, lg.threads, lg.smem, st>>>(p);
-    } else {
-      auto k = embed_fm_fwd_kernel<LPR, IdT, U, true>;
-      if (lg.smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lg.smem));
-      k<<<lg.ctas, lg.threads, lg.smem, st>>>(p);
-    }
-  } else {
-    // experiment instantiations (same arithmetic, same results): narrow rows, U = 8 / 13 only
-    //   MINB 3 / 4: register cap via __launch_bounds__(256, n);  LINX: see the kernel comment
-    constexpr bool kExp = (LPR <= 8) && (U == 8 || U == 13);
-    constexpr int UU = kExp ? U : 8;
-    static_assert(!LINXSEL || kExp, "LINX is instantiated for LPR <= 8 and U in {8, 13} only");
-    const int minb = (kExp && lg.threads <= 256 && lg.smem <= 48 * 1024) ? g_tune_embed_fwd_minblocks : 0;
-    if (kExp && (minb >= 3 || LINXSEL)) {
-      int per_sm = minb >= 4 ? 4 : (minb == 3 ? 3 : 2);
-      per_sm *= (lg.threads <= 256 ? 256 / lg.threads : 1);
-      if (g_tune_embed_ctas_per_sm > 0 && g_tune_embed_ctas_per_sm < per_sm) per_sm = g_tune_embed_ctas_per_sm;
-      const int64_t warps = lg.threads / 32, G = 32 / LPR;
-      int64_t ctas = ((p.B + G - 1) / G + warps - 1) / warps;
-      if (ctas > (int64_t)num_sms() * per_sm) ctas = (int64_t)num_sms() * per_sm;   // one resident wave
-      if (ctas < 1) ctas = 1;
-      if (minb >= 4) {
-        embed_fm_fwd_kernel<LPR, IdT, UU, false, 4, LINXSEL><<<(unsigned)ctas, lg.threads, lg.smem, st>>>(p);
-      } else if (minb == 3) {
-        embed_fm_fwd_kernel<LPR, IdT, UU, false, 3, LINXSEL><<<(unsigned)ctas, lg.threads, lg.smem, st>>>(p);
-      } else {
-        auto k = embed_fm_fwd_kernel<LPR, IdT, UU, false, 0, LINXSEL>;
-        if (lg.smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lg.smem));
-        k<<<(unsigned)ctas, lg.threads, lg.smem, st>>>(p);
-      }
-      DR_CUDA_LAUNCH_CHECK("embed_fm_fwd(linx/capped)");
-      return DR_OK;
-    }
-    auto k = embed_fm_fwd_kernel<LPR, IdT, U, false>;
-    if (lg.smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lg.smem));
-    k<<<lg.ctas, lg.threads, lg.smem, st>>>(p);
+    if (LINXSEL && U == 8) return launch(embed_fm_fwd_kernel<LPR, IdT, 8, true, 0, LINXSEL>, lg, p, st, "embed_fm_fwd");
+    return launch(embed_fm_fwd_kernel<LPR, IdT, U, true>, lg, p, st, "embed_fm_fwd");
   }
-  DR_CUDA_LAUNCH_CHECK("embed_fm_fwd");
-  return DR_OK;
+  const int minb = (kExp && lg.threads <= 256 && lg.smem <= 48 * 1024) ? g_tune_embed_fwd_minblocks : 0;
+  if (kExp && (minb >= 3 || LINXSEL)) {
+    int per_sm = minb >= 4 ? 4 : (minb == 3 ? 3 : 2);
+    per_sm *= (lg.threads <= 256 ? 256 / lg.threads : 1);
+    if (g_tune_embed_ctas_per_sm > 0 && g_tune_embed_ctas_per_sm < per_sm) per_sm = g_tune_embed_ctas_per_sm;
+    const int G = 32 / LPR;
+    lg.ctas = (int)capped_grid((p.B + G - 1) / G, lg.threads / 32, per_sm);   // one resident wave
+    void (*k)(EmbedFwdParams) = minb >= 4    ? embed_fm_fwd_kernel<LPR, IdT, UU, false, 4, LINXSEL>
+                                : minb == 3 ? embed_fm_fwd_kernel<LPR, IdT, UU, false, 3, LINXSEL>
+                                            : embed_fm_fwd_kernel<LPR, IdT, UU, false, 0, LINXSEL>;
+    return launch(k, lg, p, st, "embed_fm_fwd(linx/capped)");
+  }
+  return launch(embed_fm_fwd_kernel<LPR, IdT, U, false>, lg, p, st, "embed_fm_fwd");
 }
 
 template <int LPR, typename IdT>
@@ -635,27 +612,16 @@ static int launch_fwd_linx(const EmbedFwdParams& p, cudaStream_t st) {
 
 // lane group sized for the embedding chunks only (LINX): D <= 32 with the weight in the row
 static int dispatch_fwd_linx(const EmbedFwdParams& p, int id_bytes, cudaStream_t st) {
-  const int lpr = lpr_for(p.D, 0);
-#define DR_LINX(L) (id_bytes == 8 ? launch_fwd_linx<L, int64_t>(p, st) : launch_fwd_linx<L, int32_t>(p, st))
-  switch (lpr) {
-    case 1: return DR_LINX(1);
-    case 2: return DR_LINX(2);
-    case 4: return DR_LINX(4);
-    default: return DR_LINX(8);
-  }
-#undef DR_LINX
+  return with_lpr_id<8>(lanes_per_row(p.D / 4), id_bytes,
+                        [&](auto L, auto id) { return launch_fwd_linx<L, decltype(id)>(p, st); });
 }
 
 // DR_EMBED_NO_FM forward: the default (non-LINX, uncapped) mapping at the default unroll
 template <int LPR, typename IdT>
 static int launch_fwd_nofm(const EmbedFwdParams& p, cudaStream_t st) {
   constexpr int U = (LPR <= 8) ? 8 : 4;
-  LaunchGeom lg = geom(p.B, p.S, LPR, sizeof(IdT));
-  auto k = embed_fm_fwd_kernel<LPR, IdT, U, false, 0, false, true>;
-  if (lg.smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lg.smem));
-  k<<<lg.ctas, lg.threads, lg.smem, st>>>(p);
-  DR_CUDA_LAUNCH_CHECK("embed_fm_fwd(no_fm)");
-  return DR_OK;
+  return launch(embed_fm_fwd_kernel<LPR, IdT, U, false, 0, false, true>, geom(p.B, p.S, LPR, sizeof(IdT)), p, st,
+                "embed_fm_fwd(no_fm)");
 }
 
 template <int LPR, typename IdT>
@@ -674,56 +640,39 @@ static int launch_fwd(const EmbedFwdParams& p, cudaStream_t st) {
 
 template <int LPR, typename IdT, int U>
 static int launch_bwd_u(const EmbedBwdParams& p, cudaStream_t st) {
-  LaunchGeom lg = geom(p.B, p.S, LPR, sizeof(IdT));
-  if (g_tune_embed_bwd_agg) {
-    auto k = embed_fm_bwd_kernel<LPR, IdT, U, true>;
-    if (lg.smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lg.smem));
-    k<<<lg.ctas, lg.threads, lg.smem, st>>>(p);
-  } else {
-    auto k = embed_fm_bwd_kernel<LPR, IdT, U, false>;
-    if (lg.smem > 48 * 1024) DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lg.smem));
-    k<<<lg.ctas, lg.threads, lg.smem, st>>>(p);
-  }
-  DR_CUDA_LAUNCH_CHECK("embed_fm_bwd");
-  return DR_OK;
+  void (*k)(EmbedBwdParams) =
+      g_tune_embed_bwd_agg ? embed_fm_bwd_kernel<LPR, IdT, U, true> : embed_fm_bwd_kernel<LPR, IdT, U, false>;
+  return launch(k, geom(p.B, p.S, LPR, sizeof(IdT)), p, st, "embed_fm_bwd");
 }
 
-template <int LPR, typename IdT, int U, bool LINX = false>
-static int launch_bwd_sp_u(const EmbedBwdParams& p, cudaStream_t st) {
-  const int threads = 256, warps = threads / 32;
+// Slot-parallel backward: a warp per example, at most embed_ctas_per_sm (default 8) CTAs of 256 threads per SM.
+static int launch_bwd_sp(void (*k)(EmbedBwdParams), const EmbedBwdParams& p, cudaStream_t st, const char* what) {
+  const int threads = 256;
   const size_t smem = (size_t)p.S * (sizeof(void*) * 2 + sizeof(int64_t) * 2) + kMaxShardWorld * sizeof(void*);
-  int64_t ctas = (p.B + warps - 1) / warps;
-  int per_sm = g_tune_embed_ctas_per_sm > 0 ? g_tune_embed_ctas_per_sm : 8;
-  if (ctas > (int64_t)num_sms() * per_sm) ctas = (int64_t)num_sms() * per_sm;
-  if (ctas < 1) ctas = 1;
-  void (*k)(EmbedBwdParams) = p.shard_world > 0 ? embed_fm_bwd_sp_kernel<LPR, IdT, U, true>
-                              : (LINX ? embed_fm_bwd_sp_kernel<LPR, IdT, U, false, LINX>
-                                      : embed_fm_bwd_sp_kernel<LPR, IdT, U, false>);
+  const int64_t ctas = capped_grid(p.B, threads / 32, g_tune_embed_ctas_per_sm > 0 ? g_tune_embed_ctas_per_sm : 8);
   // The update runs beside the persistent wgmma weight-gradient GEMM, which configures its SMs with the maximum
   // shared-memory carveout (up to 224 KB of dynamic shared memory).  A kernel that prefers another L1 / shared split cannot
   // become resident on an SM in that configuration, so the update asks for the same carveout (it uses 2 KB either way).
   if (g_tune_embed_bwd_carveout)
     DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, g_tune_embed_bwd_carveout));
   k<<<(unsigned)ctas, threads, smem, st>>>(p);
-  DR_CUDA_LAUNCH_CHECK("embed_fm_bwd_sp");
+  DR_CUDA_LAUNCH_CHECK(what);
   return DR_OK;
+}
+
+template <int LPR, typename IdT, int U, bool LINX = false>
+static int launch_bwd_sp_u(const EmbedBwdParams& p, cudaStream_t st) {
+  static_assert(!LINX || LPR <= 8, "LINX is instantiated for LPR <= 8 only");
+  void (*k)(EmbedBwdParams) = p.shard_world > 0 ? embed_fm_bwd_sp_kernel<LPR, IdT, U, true>
+                              : (LINX ? embed_fm_bwd_sp_kernel<LPR, IdT, U, false, LINX>
+                                      : embed_fm_bwd_sp_kernel<LPR, IdT, U, false>);
+  return launch_bwd_sp(k, p, st, "embed_fm_bwd_sp");
 }
 
 // DR_EMBED_NO_FM backward: the slot-parallel kernel (the default mode) whatever the developer mode knob says
 template <int LPR, typename IdT>
 static int launch_bwd_nofm(const EmbedBwdParams& p, cudaStream_t st) {
-  const int threads = 256, warps = threads / 32;
-  const size_t smem = (size_t)p.S * (sizeof(void*) * 2 + sizeof(int64_t) * 2) + kMaxShardWorld * sizeof(void*);
-  int64_t ctas = (p.B + warps - 1) / warps;
-  int per_sm = g_tune_embed_ctas_per_sm > 0 ? g_tune_embed_ctas_per_sm : 8;
-  if (ctas > (int64_t)num_sms() * per_sm) ctas = (int64_t)num_sms() * per_sm;
-  if (ctas < 1) ctas = 1;
-  auto k = embed_fm_bwd_sp_kernel<LPR, IdT, 2, false, false, true>;
-  if (g_tune_embed_bwd_carveout)
-    DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, g_tune_embed_bwd_carveout));
-  k<<<(unsigned)ctas, threads, smem, st>>>(p);
-  DR_CUDA_LAUNCH_CHECK("embed_fm_bwd_sp(no_fm)");
-  return DR_OK;
+  return launch_bwd_sp(embed_fm_bwd_sp_kernel<LPR, IdT, 2, false, false, true>, p, st, "embed_fm_bwd_sp(no_fm)");
 }
 
 template <int LPR, typename IdT>
@@ -745,39 +694,6 @@ static int launch_bwd(const EmbedBwdParams& p, cudaStream_t st) {
   }
 }
 
-#define DR_DISPATCH_LPR(FN, P, ST)                                      \
-  do {                                                                  \
-    const int lpr__ = lpr_for((P).D, (P).lin_in_row);                   \
-    if (id_bytes == 8) {                                                \
-      switch (lpr__) {                                                  \
-        case 1: return FN<1, int64_t>(P, ST);                           \
-        case 2: return FN<2, int64_t>(P, ST);                           \
-        case 4: return FN<4, int64_t>(P, ST);                           \
-        case 8: return FN<8, int64_t>(P, ST);                           \
-        case 16: return FN<16, int64_t>(P, ST);                         \
-        default: return FN<32, int64_t>(P, ST);                         \
-      }                                                                 \
-    } else {                                                            \
-      switch (lpr__) {                                                  \
-        case 1: return FN<1, int32_t>(P, ST);                           \
-        case 2: return FN<2, int32_t>(P, ST);                           \
-        case 4: return FN<4, int32_t>(P, ST);                           \
-        case 8: return FN<8, int32_t>(P, ST);                           \
-        case 16: return FN<16, int32_t>(P, ST);                         \
-        default: return FN<32, int32_t>(P, ST);                         \
-      }                                                                 \
-    }                                                                   \
-  } while (0)
-
-static int check_dims(const char* fn, int64_t B, int S, int D, int id_bytes) {
-  DR_REQUIRE(B >= 0, DR_EINVAL, "%s: B=%lld < 0", fn, (long long)B);
-  DR_REQUIRE(S >= 1 && S <= 4096, DR_EINVAL, "%s: S=%d outside [1,4096]", fn, S);
-  DR_REQUIRE(D >= 4 && D <= 128 && (D % 4) == 0, DR_EINVAL,
-             "%s: D=%d unsupported (need D %% 4 == 0 and 4 <= D <= 128)", fn, D);
-  DR_REQUIRE(id_bytes == 8 || id_bytes == 4, DR_EINVAL, "%s: id_bytes=%d (need 4 or 8)", fn, id_bytes);
-  return DR_OK;
-}
-
 }  // namespace dr
 
 using namespace dr;
@@ -786,7 +702,7 @@ extern "C" int dr_embed_fm_fwd(const float* const* table_ptrs, const float* cons
                                const int64_t* rows, const void* ids, int id_bytes, const float* bias,
                                int64_t B, int S, int D, int64_t row_stride, int64_t lin_stride, int flags,
                                float* out_stack, float* out_sum, float* out_logit, void* stream) {
-  if (int rc = check_dims("dr_embed_fm_fwd", B, S, D, id_bytes)) return rc;
+  if (int rc = check_lookup_dims("dr_embed_fm_fwd", B, S, D, id_bytes)) return rc;
   if (B == 0) return DR_OK;
   DR_REQUIRE(table_ptrs && rows && ids, DR_EINVAL, "dr_embed_fm_fwd: null table_ptrs/rows/ids");
   DR_REQUIRE(out_stack || out_logit || out_sum, DR_EINVAL, "dr_embed_fm_fwd: no output requested");
@@ -800,16 +716,18 @@ extern "C" int dr_embed_fm_fwd(const float* const* table_ptrs, const float* cons
              "dr_embed_fm_fwd: DR_EMBED_LIN_IN_ROW needs row_stride >= D+4 and D <= 124");
   DR_REQUIRE(!out_stack || aligned16(out_stack), DR_EALIGN, "dr_embed_fm_fwd: out_stack not 16-B aligned");
   DR_REQUIRE(!out_sum || aligned16(out_sum), DR_EALIGN, "dr_embed_fm_fwd: out_sum not 16-B aligned");
-  if (B == 0) return DR_OK;
   EmbedFwdParams p{};
   p.table_ptrs = table_ptrs; p.lin_ptrs = lin_ptrs; p.rows = rows; p.ids = ids; p.bias = bias;
   p.B = B; p.S = S; p.D = D; p.out_stack = out_stack; p.out_sum = out_sum; p.out_logit = out_logit;
   p.row_stride = row_stride; p.lin_stride = lin_stride; p.lin_in_row = lin_in_row;
   p.l2_hints = g_tune_embed_l2_hints;
   cudaStream_t st = (cudaStream_t)stream;
-  if (flags & DR_EMBED_NO_FM) DR_DISPATCH_LPR(launch_fwd_nofm, p, st);
-  if (g_tune_embed_fwd_linx && lin_in_row && out_logit && lpr_for(D, 0) <= 8) return dispatch_fwd_linx(p, id_bytes, st);
-  DR_DISPATCH_LPR(launch_fwd, p, st);
+  const int lpr = lanes_per_row(D / 4 + lin_in_row);
+  if (flags & DR_EMBED_NO_FM)
+    return with_lpr_id(lpr, id_bytes, [&](auto L, auto id) { return launch_fwd_nofm<L, decltype(id)>(p, st); });
+  if (g_tune_embed_fwd_linx && lin_in_row && out_logit && lanes_per_row(D / 4) <= 8)
+    return dispatch_fwd_linx(p, id_bytes, st);
+  return with_lpr_id(lpr, id_bytes, [&](auto L, auto id) { return launch_fwd<L, decltype(id)>(p, st); });
 }
 
 extern "C" int dr_embed_fm_bwd(const void* ids, int id_bytes, const int64_t* rows, const float* stack,
@@ -817,7 +735,7 @@ extern "C" int dr_embed_fm_bwd(const void* ids, int id_bytes, const int64_t* row
                                int64_t B, int S, int D, int64_t row_stride, int64_t lin_stride, int flags,
                                float* const* grad_table_ptrs, float* const* grad_lin_ptrs, float* g_bias,
                                float scale, void* stream) {
-  if (int rc = check_dims("dr_embed_fm_bwd", B, S, D, id_bytes)) return rc;
+  if (int rc = check_lookup_dims("dr_embed_fm_bwd", B, S, D, id_bytes)) return rc;
   if (B == 0) return DR_OK;
   DR_REQUIRE(ids && rows && grad_table_ptrs, DR_EINVAL, "dr_embed_fm_bwd: null ids/rows/grad_table_ptrs");
   DR_REQUIRE(g_logit || g_stack, DR_EINVAL, "dr_embed_fm_bwd: both g_logit and g_stack are NULL");
@@ -832,7 +750,6 @@ extern "C" int dr_embed_fm_bwd(const void* ids, int id_bytes, const int64_t* row
   const int lin_in_row = (flags & DR_EMBED_LIN_IN_ROW) ? 1 : 0;
   DR_REQUIRE(!lin_in_row || (row_stride >= D + 4 && D <= 124), DR_EINVAL,
              "dr_embed_fm_bwd: DR_EMBED_LIN_IN_ROW needs row_stride >= D+4 and D <= 124");
-  if (B == 0) return DR_OK;
   EmbedBwdParams p{};
   p.ids = ids; p.rows = rows; p.stack = stack; p.sum_e = sum_e; p.g_logit = g_logit; p.g_stack = g_stack;
   p.B = B; p.S = S; p.D = D; p.grad_table_ptrs = grad_table_ptrs; p.grad_lin_ptrs = grad_lin_ptrs;
@@ -841,57 +758,48 @@ extern "C" int dr_embed_fm_bwd(const void* ids, int id_bytes, const int64_t* row
   p.l2_hints = g_tune_embed_l2_hints;
   p.mode = g_tune_embed_bwd_mode;
   cudaStream_t st = (cudaStream_t)stream;
-  if (flags & DR_EMBED_NO_FM) DR_DISPATCH_LPR(launch_bwd_nofm, p, st);
-  if (g_tune_embed_bwd_linx && p.mode == 0 && lin_in_row && g_logit && lpr_for(D, 0) <= 8) {
-    const int lpr = lpr_for(D, 0);
-#define DR_BLINX(L) (id_bytes == 8 ? launch_bwd_sp_u<L, int64_t, 2, true>(p, st) : launch_bwd_sp_u<L, int32_t, 2, true>(p, st))
-    switch (lpr) {
-      case 1: return DR_BLINX(1);
-      case 2: return DR_BLINX(2);
-      case 4: return DR_BLINX(4);
-      default: return DR_BLINX(8);
-    }
-#undef DR_BLINX
-  }
-  DR_DISPATCH_LPR(launch_bwd, p, st);
+  const int lpr = lanes_per_row(D / 4 + lin_in_row);
+  if (flags & DR_EMBED_NO_FM)
+    return with_lpr_id(lpr, id_bytes, [&](auto L, auto id) { return launch_bwd_nofm<L, decltype(id)>(p, st); });
+  if (g_tune_embed_bwd_linx && p.mode == 0 && lin_in_row && g_logit && lanes_per_row(D / 4) <= 8)
+    return with_lpr_id<8>(lanes_per_row(D / 4), id_bytes,
+                          [&](auto L, auto id) { return launch_bwd_sp_u<L, decltype(id), 2, true>(p, st); });
+  return with_lpr_id(lpr, id_bytes, [&](auto L, auto id) { return launch_bwd<L, decltype(id)>(p, st); });
 }
 
 extern "C" int dr_gather_fwd(const float* table, int64_t rows, const void* ids, int id_bytes, int64_t n,
                              int D, float* out, void* stream) {
-  if (int rc = check_dims("dr_gather_fwd", n, 1, D, id_bytes)) return rc;
+  if (int rc = check_lookup_dims("dr_gather_fwd", n, 1, D, id_bytes)) return rc;
   if (n == 0) return DR_OK;
   DR_REQUIRE(table && ids && out, DR_EINVAL, "dr_gather_fwd: null pointer");
   DR_REQUIRE(rows >= 0, DR_EINVAL, "dr_gather_fwd: rows < 0");
   DR_REQUIRE(aligned16(table) && aligned16(out), DR_EALIGN, "dr_gather_fwd: table/out not 16-B aligned");
   const int chunks = D / 4;
-  int64_t ctas = (n * chunks + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (id_bytes == 8)
-    gather_rows_kernel<int64_t><<<(unsigned)ctas, 256, 0, st>>>(table, rows, (const int64_t*)ids, n, chunks, out);
-  else
-    gather_rows_kernel<int32_t><<<(unsigned)ctas, 256, 0, st>>>(table, rows, (const int32_t*)ids, n, chunks, out);
-  DR_CUDA_LAUNCH_CHECK("gather_rows");
-  return DR_OK;
+  const int64_t ctas = capped_grid(n * chunks, 256, 8);
+  return with_id_type(id_bytes, [&](auto id) {
+    using IdT = decltype(id);
+    gather_rows_kernel<IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(table, rows, (const IdT*)ids, n, chunks, out);
+    DR_CUDA_LAUNCH_CHECK("gather_rows");
+    return DR_OK;
+  });
 }
 
 extern "C" int dr_scatter_add(float* grad_table, int64_t rows, const void* ids, int id_bytes, int64_t n,
                               int D, const float* g, float scale, void* stream) {
-  if (int rc = check_dims("dr_scatter_add", n, 1, D, id_bytes)) return rc;
+  if (int rc = check_lookup_dims("dr_scatter_add", n, 1, D, id_bytes)) return rc;
   if (n == 0) return DR_OK;
   DR_REQUIRE(grad_table && ids && g, DR_EINVAL, "dr_scatter_add: null pointer");
   DR_REQUIRE(rows >= 0, DR_EINVAL, "dr_scatter_add: rows < 0");
   DR_REQUIRE(aligned16(grad_table) && aligned16(g), DR_EALIGN, "dr_scatter_add: table/g not 16-B aligned");
   const int chunks = D / 4;
-  int64_t ctas = (n * chunks + 255) / 256;
-  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (id_bytes == 8)
-    scatter_add_rows_kernel<int64_t><<<(unsigned)ctas, 256, 0, st>>>(grad_table, rows, (const int64_t*)ids, n, chunks, g, scale);
-  else
-    scatter_add_rows_kernel<int32_t><<<(unsigned)ctas, 256, 0, st>>>(grad_table, rows, (const int32_t*)ids, n, chunks, g, scale);
-  DR_CUDA_LAUNCH_CHECK("scatter_add_rows");
-  return DR_OK;
+  const int64_t ctas = capped_grid(n * chunks, 256, 8);
+  return with_id_type(id_bytes, [&](auto id) {
+    using IdT = decltype(id);
+    scatter_add_rows_kernel<IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(grad_table, rows, (const IdT*)ids, n,
+                                                                                   chunks, g, scale);
+    DR_CUDA_LAUNCH_CHECK("scatter_add_rows");
+    return DR_OK;
+  });
 }
 
 // ---- row-sharded entries: the gather / scatter IS the exchange (NVLink peer memory) -------------------
@@ -899,7 +807,7 @@ extern "C" int dr_embed_fm_fwd_sharded(const float* const* peer_bases, int world
                                        const int64_t* rows, const void* ids, int id_bytes, const float* bias,
                                        int64_t B, int S, int D, int64_t row_stride, int flags, int64_t lin_offset,
                                        float* out_stack, float* out_sum, float* out_logit, void* stream) {
-  if (int rc = check_dims("dr_embed_fm_fwd_sharded", B, S, D, id_bytes)) return rc;
+  if (int rc = check_lookup_dims("dr_embed_fm_fwd_sharded", B, S, D, id_bytes)) return rc;
   DR_REQUIRE(!(flags & DR_EMBED_NO_FM), DR_ENOTSUP, "dr_embed_fm_fwd_sharded: DR_EMBED_NO_FM is not served");
   DR_REQUIRE(lin_offset >= 0 && !((flags & DR_EMBED_LIN_IN_ROW) && lin_offset > 0), DR_EINVAL,
              "dr_embed_fm_fwd_sharded: lin_offset=%lld (must be >= 0 and exclusive with DR_EMBED_LIN_IN_ROW)",
@@ -919,8 +827,10 @@ extern "C" int dr_embed_fm_fwd_sharded(const float* const* peer_bases, int world
   p.row_stride = row_stride; p.lin_stride = row_stride; p.lin_in_row = lin_in_row;
   p.shard_world = world; p.peer_bases = peer_bases; p.slot_offsets = slot_offsets; p.shard_lin_off = lin_offset;
   cudaStream_t st = (cudaStream_t)stream;
-  if (g_tune_embed_fwd_linx_shard && lin_in_row && out_logit && lpr_for(D, 0) <= 8) return dispatch_fwd_linx(p, id_bytes, st);
-  DR_DISPATCH_LPR(launch_fwd, p, st);
+  if (g_tune_embed_fwd_linx_shard && lin_in_row && out_logit && lanes_per_row(D / 4) <= 8)
+    return dispatch_fwd_linx(p, id_bytes, st);
+  return with_lpr_id(lanes_per_row(D / 4 + lin_in_row), id_bytes,
+                     [&](auto L, auto id) { return launch_fwd<L, decltype(id)>(p, st); });
 }
 
 extern "C" int dr_embed_fm_bwd_sharded(float* const* peer_bases, int world, const int64_t* slot_offsets,
@@ -928,7 +838,7 @@ extern "C" int dr_embed_fm_bwd_sharded(float* const* peer_bases, int world, cons
                                        const float* sum_e, const float* g_logit, const float* g_stack, int64_t B,
                                        int S, int D, int64_t row_stride, int flags, int64_t lin_offset, float* g_bias,
                                        float scale, void* stream) {
-  if (int rc = check_dims("dr_embed_fm_bwd_sharded", B, S, D, id_bytes)) return rc;
+  if (int rc = check_lookup_dims("dr_embed_fm_bwd_sharded", B, S, D, id_bytes)) return rc;
   DR_REQUIRE(!(flags & DR_EMBED_NO_FM), DR_ENOTSUP, "dr_embed_fm_bwd_sharded: DR_EMBED_NO_FM is not served");
   DR_REQUIRE(lin_offset >= 0 && !((flags & DR_EMBED_LIN_IN_ROW) && lin_offset > 0), DR_EINVAL,
              "dr_embed_fm_bwd_sharded: lin_offset=%lld (must be >= 0 and exclusive with DR_EMBED_LIN_IN_ROW)",
@@ -949,19 +859,6 @@ extern "C" int dr_embed_fm_bwd_sharded(float* const* peer_bases, int world, cons
   p.shard_world = world; p.peer_bases = peer_bases; p.slot_offsets = slot_offsets; p.shard_lin_off = lin_offset;
   p.mode = 0;                     // only the slot-parallel kernel implements sharded addressing
   cudaStream_t st = (cudaStream_t)stream;
-  int rc;
-  do {
-    const int lpr__ = lpr_for(p.D, p.lin_in_row);
-#define DR_SH(L) (id_bytes == 8 ? launch_bwd<L, int64_t>(p, st) : launch_bwd<L, int32_t>(p, st))
-    switch (lpr__) {
-      case 1: rc = DR_SH(1); break;
-      case 2: rc = DR_SH(2); break;
-      case 4: rc = DR_SH(4); break;
-      case 8: rc = DR_SH(8); break;
-      case 16: rc = DR_SH(16); break;
-      default: rc = DR_SH(32); break;
-    }
-#undef DR_SH
-  } while (0);
-  return rc;
+  return with_lpr_id(lanes_per_row(D / 4 + lin_in_row), id_bytes,
+                     [&](auto L, auto id) { return launch_bwd<L, decltype(id)>(p, st); });
 }

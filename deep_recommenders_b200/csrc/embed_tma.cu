@@ -183,25 +183,15 @@ extern "C" int dr_embed_fm_fwd_tma(const float* arena, int64_t total_rows, const
   p.arena = arena; p.total_rows = total_rows; p.slot_offsets = slot_offsets; p.rows = rows; p.ids = ids; p.bias = bias;
   p.B = B; p.S = S; p.row_stride = row_stride; p.out_stack = out_stack; p.out_sum = out_sum; p.out_logit = out_logit;
   const size_t smem = (size_t)TMA_WARPS * TMA_NBUF * (((size_t)TMA_EX * S * 64 + (size_t)TMA_EX * S * 4 + 127) / 128 * 128);
-  cudaStream_t st = (cudaStream_t)stream;
   const int64_t ntiles = (B + TMA_EX - 1) / TMA_EX;
-  if (id_bytes == 8) {
-    auto k = embed_fm_fwd_tma_kernel<int64_t>;
+  return with_id_type(id_bytes, [&](auto id) {
+    auto k = embed_fm_fwd_tma_kernel<decltype(id)>;
     DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 1;
     DR_CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, TMA_WARPS * 32, smem));
-    int64_t ctas = (int64_t)num_sms() * (occ > 0 ? occ : 1);
-    if (ctas * TMA_WARPS > ntiles) ctas = (ntiles + TMA_WARPS - 1) / TMA_WARPS;
-    k<<<(unsigned)ctas, TMA_WARPS * 32, smem, st>>>(p);
-  } else {
-    auto k = embed_fm_fwd_tma_kernel<int32_t>;
-    DR_CUDA_CALL(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 1;
-    DR_CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, TMA_WARPS * 32, smem));
-    int64_t ctas = (int64_t)num_sms() * (occ > 0 ? occ : 1);
-    if (ctas * TMA_WARPS > ntiles) ctas = (ntiles + TMA_WARPS - 1) / TMA_WARPS;
-    k<<<(unsigned)ctas, TMA_WARPS * 32, smem, st>>>(p);
-  }
-  DR_CUDA_LAUNCH_CHECK("dr_embed_fm_fwd_tma");
-  return DR_OK;
+    const int64_t ctas = capped_grid(ntiles, TMA_WARPS, occ > 0 ? occ : 1);
+    k<<<(unsigned)ctas, TMA_WARPS * 32, smem, (cudaStream_t)stream>>>(p);
+    DR_CUDA_LAUNCH_CHECK("dr_embed_fm_fwd_tma");
+    return DR_OK;
+  });
 }

@@ -136,21 +136,12 @@ __global__ void __launch_bounds__(256) fnn_input_bwd_kernel(const FnnParams p) {
   }
 }
 
-static int fnn_lpr(int D) {
-  int l = 1;
-  while (l * 4 < D) l <<= 1;
-  return l;
-}
-
 template <bool BWD, int LPR, typename IdT>
 static int fnn_launch(const FnnParams& p, cudaStream_t st) {
   constexpr int U = LPR <= 8 ? 8 : 4;
   constexpr int kThreads = 256, G = 32 / LPR;
   const int64_t tiles = ((int64_t)p.n + G * U - 1) / (G * U);
-  int64_t ctas = (tiles + kThreads / 32 - 1) / (kThreads / 32);
-  const int64_t cap = (int64_t)num_sms() * (2048 / kThreads);
-  if (ctas > cap) ctas = cap;
-  if (ctas < 1) ctas = 1;
+  const int64_t ctas = capped_grid(tiles, kThreads / 32, 2048 / kThreads);
   if (BWD) {
     fnn_input_bwd_kernel<LPR, IdT, U><<<(unsigned)ctas, kThreads, 0, st>>>(p);
     DR_CUDA_LAUNCH_CHECK("fnn_input_bwd");
@@ -161,28 +152,12 @@ static int fnn_launch(const FnnParams& p, cudaStream_t st) {
   return DR_OK;
 }
 
-template <bool BWD, typename IdT>
-static int fnn_dispatch_lpr(const FnnParams& p, cudaStream_t st) {
-  switch (fnn_lpr(p.D)) {
-    case 1: return fnn_launch<BWD, 1, IdT>(p, st);
-    case 2: return fnn_launch<BWD, 2, IdT>(p, st);
-    case 4: return fnn_launch<BWD, 4, IdT>(p, st);
-    case 8: return fnn_launch<BWD, 8, IdT>(p, st);
-    case 16: return fnn_launch<BWD, 16, IdT>(p, st);
-    default: return fnn_launch<BWD, 32, IdT>(p, st);
-  }
-}
-
 // The checks both entries share; fills the geometry of p.
 static int fnn_check(const char* fn, const float* const* table_ptrs, const float* const* lin_ptrs,
                      const int64_t* rows, const void* ids, int id_bytes, int64_t row_stride, int64_t lin_stride,
                      int flags, int64_t B, int S, int D, int64_t ld, const float* x, FnnParams& p) {
   DR_REQUIRE(table_ptrs && rows && ids && x, DR_EINVAL, "%s: null table pointers / rows / ids / row buffer", fn);
-  DR_REQUIRE(B >= 0, DR_EINVAL, "%s: B=%lld < 0", fn, (long long)B);
-  DR_REQUIRE(S >= 1 && S <= 4096, DR_EINVAL, "%s: S=%d outside [1,4096]", fn, S);
-  DR_REQUIRE(D >= 4 && D <= 128 && D % 4 == 0, DR_EINVAL, "%s: D=%d unsupported (need D %% 4 == 0, 4 <= D <= 128)",
-             fn, D);
-  DR_REQUIRE(id_bytes == 8 || id_bytes == 4, DR_EINVAL, "%s: id_bytes=%d (need 4 or 8)", fn, id_bytes);
+  if (int rc = check_lookup_dims(fn, B, S, D, id_bytes, ",")) return rc;
   const int P = (1 + S + 3) / 4 * 4;
   DR_REQUIRE(ld == P + (int64_t)S * D, DR_EINVAL, "%s: ld=%lld, the row layout needs P + S*D = %lld", fn,
              (long long)ld, (long long)(P + (int64_t)S * D));
@@ -219,8 +194,9 @@ extern "C" int dr_fnn_input_fwd(const float* const* table_ptrs, const float* con
   DR_REQUIRE(bias, DR_EINVAL, "dr_fnn_input_fwd: null bias");
   if (B == 0) return DR_OK;
   p.bias = bias; p.out = out;
-  cudaStream_t st = (cudaStream_t)stream;
-  return id_bytes == 8 ? fnn_dispatch_lpr<false, int64_t>(p, st) : fnn_dispatch_lpr<false, int32_t>(p, st);
+  return with_lpr_id(lanes_per_row(D / 4), id_bytes, [&](auto L, auto id) {
+    return fnn_launch<false, L, decltype(id)>(p, (cudaStream_t)stream);
+  });
 }
 
 extern "C" int dr_fnn_input_bwd(const void* ids, int id_bytes, const int64_t* rows, const float* g_x, int64_t B,
@@ -233,6 +209,7 @@ extern "C" int dr_fnn_input_bwd(const void* ids, int id_bytes, const int64_t* ro
     return rc;
   if (B == 0) return DR_OK;
   p.g_x = g_x; p.grad_table_ptrs = grad_table_ptrs; p.grad_lin_ptrs = grad_lin_ptrs; p.scale = scale;
-  cudaStream_t st = (cudaStream_t)stream;
-  return id_bytes == 8 ? fnn_dispatch_lpr<true, int64_t>(p, st) : fnn_dispatch_lpr<true, int32_t>(p, st);
+  return with_lpr_id(lanes_per_row(D / 4), id_bytes, [&](auto L, auto id) {
+    return fnn_launch<true, L, decltype(id)>(p, (cudaStream_t)stream);
+  });
 }

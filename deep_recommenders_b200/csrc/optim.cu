@@ -256,12 +256,12 @@ extern "C" int dr_lazy_adam_rows(const void* ids, int id_bytes, int64_t B, int S
   const int lpr = lanes_per_row(D / 4 + lin_in_row);     // the [w | pad] chunk takes a lane of its own
   const int64_t n = B * S;
   const int64_t ctas = capped_grid(n, 256 / lpr, 8);
-  with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
+  return with_lpr_id(lpr, id_bytes, [&](auto L, auto id) {
     using IdT = decltype(id);
     lazy_adam_rows_kernel<L, IdT><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(
         (const IdT*)ids, n, S, rows, slot_offsets, p, g, m, v, row_stride, D, lin_in_row, lin_p, lin_g, lin_m, lin_v,
         stamp, step_dev, lr_t_dev, 1.f - beta1, 1.f - beta2, eps);
+    DR_CUDA_LAUNCH_CHECK("dr_lazy_adam_rows");
+    return DR_OK;
   });
-  DR_CUDA_LAUNCH_CHECK("dr_lazy_adam_rows");
-  return DR_OK;
 }

@@ -103,17 +103,15 @@ extern "C" int dr_shard_bucket_ids(const void* ids, int id_bytes, int64_t n, int
   // here would let a later, well-behaved batch erase the evidence of an earlier truncated one).
   DR_CUDA_CALL(cudaMemsetAsync(send_ids, 0xFF, sizeof(int64_t) * (size_t)G * cap, st));   // all -1
   if (n == 0) return DR_OK;
-  int64_t ctas = (n + 255) / 256;
-  if (ctas > num_sms() * 8) ctas = num_sms() * 8;
-  auto* cur = reinterpret_cast<unsigned long long*>(send_counts);
-  if (id_bytes == 8)
-    shard_bucket_kernel<int64_t><<<(unsigned)ctas, 256, 0, st>>>((const int64_t*)ids, n, S, slot_offsets, rows, G, cap,
-                                                                  cur, send_ids, inv, overflow);
-  else
-    shard_bucket_kernel<int32_t><<<(unsigned)ctas, 256, 0, st>>>((const int32_t*)ids, n, S, slot_offsets, rows, G, cap,
-                                                                  cur, send_ids, inv, overflow);
-  DR_CUDA_LAUNCH_CHECK("shard_bucket");
-  return DR_OK;
+  const int64_t ctas = capped_grid(n, 256, 8);
+  return with_id_type(id_bytes, [&](auto id) {
+    using IdT = decltype(id);
+    shard_bucket_kernel<IdT><<<(unsigned)ctas, 256, 0, st>>>((const IdT*)ids, n, S, slot_offsets, rows, G, cap,
+                                                             reinterpret_cast<unsigned long long*>(send_counts), send_ids,
+                                                             inv, overflow);
+    DR_CUDA_LAUNCH_CHECK("shard_bucket");
+    return DR_OK;
+  });
 }
 
 static int permute_common(const float* in, const int32_t* perm, int64_t n, int D, float* out, void* stream,
@@ -122,8 +120,7 @@ static int permute_common(const float* in, const int32_t* perm, int64_t n, int D
   DR_REQUIRE(n >= 0 && D >= 4 && D % 4 == 0, DR_EINVAL, "dr_permute_rows: bad shape n=%lld D=%d", (long long)n, D);
   DR_REQUIRE(aligned16(in) && aligned16(out), DR_EALIGN, "dr_permute_rows: in/out not 16-B aligned");
   if (n == 0) return DR_OK;
-  int64_t ctas = (n * (D / 4) + 255) / 256;
-  if (ctas > num_sms() * 8) ctas = num_sms() * 8;
+  const int64_t ctas = capped_grid(n * (D / 4), 256, 8);
   if (un) permute_rows_kernel<true><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(in, perm, n, D, out);
   else permute_rows_kernel<false><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(in, perm, n, D, out);
   DR_CUDA_LAUNCH_CHECK("permute_rows");

@@ -148,23 +148,14 @@ static int wide_launch(float* state, int64_t total_rows, const int64_t* rows, co
   if (B == 0 && MODE != kWideFtrl) return DR_OK;
   int lpe = 4;
   while (lpe < S && lpe < 32) lpe <<= 1;
-  const int64_t groups_per_cta = 256 / lpe;
-  int64_t ctas = (B + groups_per_cta - 1) / groups_per_cta;
-  if (ctas > (int64_t)num_sms() * 8) ctas = (int64_t)num_sms() * 8;
-  if (ctas < 1) ctas = 1;
-  cudaStream_t st = (cudaStream_t)stream;
-#define DR_WIDE(L)                                                                                                   \
-  wide_kernel<MODE, L><<<(unsigned)ctas, 256, 0, st>>>(state, total_rows, rows, slot_offsets, ids, B, S, bags, g_logit, \
-                                                       logit, p)
-  switch (lpe) {
-    case 4: DR_WIDE(4); break;
-    case 8: DR_WIDE(8); break;
-    case 16: DR_WIDE(16); break;
-    default: DR_WIDE(32); break;
-  }
-#undef DR_WIDE
-  DR_CUDA_LAUNCH_CHECK(who);
-  return DR_OK;
+  int64_t ctas = capped_grid(B, 256 / lpe, 8);
+  if (ctas < 1) ctas = 1;   // dr_wide_ftrl at B = 0 still updates the bias record
+  return with_lpr<32, 4>(lpe, [&](auto L) {
+    wide_kernel<MODE, L><<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(state, total_rows, rows, slot_offsets, ids, B,
+                                                                          S, bags, g_logit, logit, p);
+    DR_CUDA_LAUNCH_CHECK(who);
+    return DR_OK;
+  });
 }
 
 }  // namespace dr

@@ -167,6 +167,45 @@ def test_c_abi_rejects_bad_wide_arguments():
     assert rc == -1 and b"multi-valued" in lib.dr_last_error()
 
 
+def test_c_abi_wide_rejections_in_order():
+    """Every rejection of the three wide entries, with its code and exact text, in the order the checks run."""
+    from deep_recommenders_b200 import _lib
+    lib = _lib.load()
+    base = 1 << 20          # never dereferenced: validation runs before any launch
+    bs, bi, bp = _ptr_arrays(1)
+    bi[0], bp[0] = base, base
+    entries = {"dr_wide_fwd": lambda st, total, rows, B, S, n, slots, arg: lib.dr_wide_fwd(
+                   st, total, rows, base, base, B, S, n, slots, bi, bp, arg, None),
+               "dr_wide_bwd": lambda st, total, rows, B, S, n, slots, arg: lib.dr_wide_bwd(
+                   st, total, rows, base, base, B, S, n, slots, bi, bp, arg, None),
+               "dr_wide_ftrl": lambda st, total, rows, B, S, n, slots, arg: lib.dr_wide_ftrl(
+                   st, total, rows, base, base, B, S, n, slots, bi, bp, arg, 0.0, 0.0, None)}
+    first = {"dr_wide_fwd": "null logit", "dr_wide_bwd": "null g_logit",
+             "dr_wide_ftrl": "lr=0 l1=0 l2=0 (need lr > 0, l1, l2 >= 0)"}
+    for fn, call in entries.items():
+        ok = 0.1 if fn == "dr_wide_ftrl" else base      # arg: the logit / g_logit pointer, or lr
+        bad = 0.0 if fn == "dr_wide_ftrl" else None
+        for args, msg in [
+            ((base, 10, base, 4, 2, 0, bs, bad), first[fn]),
+            ((base, 10, base, -1, 2, 0, bs, ok), "B=-1 S=2 total_rows=10"),
+            ((base, 10, base, 4, 0, 0, bs, ok), "B=4 S=0 total_rows=10"),
+            ((base, 10, base, 4, 4097, 17, bs, ok), "B=4 S=4097 total_rows=10"),
+            ((base, -1, base, 4, 2, 0, bs, ok), "B=4 S=2 total_rows=-1"),
+            ((None, 10, base, 4, 2, 17, bs, ok), "n_bags=17 (at most 16)"),
+            ((base, 10, base, 4, 2, -1, bs, ok), "n_bags=-1 (at most 16)"),
+            ((base, 10, None, 4, 2, 0, bs, ok), "null pointer"),
+            ((base + 4, 10, base, 4, 2, 1, None, ok), "the state arena is not 16-B aligned"),
+            ((base, 10, base, 4, 2, 1, None, ok), "null bag arrays"),
+        ]:
+            assert call(*args) == -1, (fn, args)
+            assert lib.dr_last_error() == f"{fn}: {msg}".encode(), (fn, args)
+        for slot in (2, -1):
+            bs[0] = slot
+            assert call(base, 10, base, 4, 2, 1, bs, ok) == -1
+            assert lib.dr_last_error() == f"{fn}: bag 0: slot {slot} outside [0, 2) or null arrays".encode()
+        bs[0] = 0
+
+
 @pytest.mark.skipif(not os.path.exists(GOLDEN), reason="golden file not generated")
 def test_oracle_matches_the_reference_model():
     """tests/golden/wdl_golden.npz comes from running the reference's wide_and_deep.py and dnn.py under the numpy
