@@ -143,16 +143,14 @@ class EmbeddingCollection(nn.Module):
             if not second_order:
                 raise ValueError("second_order=False is not served with multi-valued slots (bags)")
             if want_logit and not self.with_linear:
-                raise ValueError("EmbedFMMixed needs a collection with the first-order term (with_linear=True)")
+                raise ValueError("a logit over multi-valued slots (bags) needs a collection with the first-order term "
+                                 "(with_linear=True)")
             bad = [s for s in bags if not (0 <= s < self.num_slots)]
             if bad:
                 raise ValueError(f"bags: slot indices {bad} outside [0, {self.num_slots})")
-            stack, logit = ops.EmbedFMMixed.apply(ids, self.weight, self.linear, self.bias, self, bags)
-            return stack, (logit if want_logit else None)
-        want = want_logit
-        stack, logit = ops.EmbedFM.apply(ids, self.weight, self.linear if want else None,
-                                         self.bias if want else None, self, want, bool(second_order))
-        return stack, (logit if want else None)
+        stack, logit = ops.EmbedFM.apply(ids, self.weight, self.linear, self.bias, self, want_logit,
+                                         bool(second_order), bags)
+        return stack, (logit if want_logit else None)
 
 
 class LinearTable(nn.Module):

@@ -53,40 +53,47 @@ def _ids(t: torch.Tensor, name: str = "ids") -> torch.Tensor:
 # Rows E + L + F: fused multi-slot gather + linear + FM
 # ------------------------------------------------------------------------------------------
 class EmbedFM(torch.autograd.Function):
-    """stack, logit = EmbedFM(ids, weight_arena, linear_arena, bias, meta, want_logit, second_order).
+    """stack, logit = EmbedFM(ids, weight_arena, linear_arena, bias, meta, want_logit, second_order, bags).
 
-    `meta` carries the device pointer arrays (table_ptrs, lin_ptrs, rows) of the collection.
-    Backward either scatter-adds into dense .grad buffers (meta.sparse_lr is None) or applies
-    the fused sparse SGD update in place (meta.sparse_lr = lr) and returns no table gradient.
+    `meta` is the EmbeddingCollection: its device pointer arrays (table_ptrs, lin_ptrs, rows), strides and trainer.
+    want_logit=False: stack only; linear and bias are not read and get no gradient.
     second_order=False (DR_EMBED_NO_FM): the logit is bias + first order only (xDeepFM's linear unit).
+
+    bags {slot: (flat_ids, row_splits[B+1])} serves multi-valued slots (SURVEY 8f #2); the matching columns of ids are
+    ignored.  _reduce_bags reduces each bag slot into a scratch table, so the whole lookup is still ONE
+    dr_embed_fm_fwd.  With bags and first-order weights the logit is computed, and its gradient taken, even when
+    want_logit is False.
+
+    Backward: _route_grads sends the table gradients where the collection trains.
     """
 
     @staticmethod
-    def forward(ctx, ids, weight, linear, bias, meta, want_logit: bool, second_order: bool = True):
+    def forward(ctx, ids, weight, linear, bias, meta, want_logit: bool, second_order: bool = True, bags=None):
         lib = _lib.load()
-        ids = _ids(ids)
+        if _row_opt(meta) is not None:
+            meta.row_optimizer.catch_up(ids, bags)
+        has_logit = bool(want_logit or (bags and meta.with_linear))
+        if not has_logit:
+            linear = bias = None
+        ids, tp, lp, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, linear, meta, bags)
         B, S = ids.shape
         D = meta.dim
-        if _row_opt(meta) is not None:
-            meta.row_optimizer.catch_up(ids)
         stack = torch.empty((B, S, D), device=weight.device, dtype=torch.float32)
-        sum_e = torch.empty((B, D), device=weight.device, dtype=torch.float32) if want_logit else None
-        logit = torch.empty((B,), device=weight.device, dtype=torch.float32) if want_logit else None
-        tp, lp, rows = meta.pointers(weight, linear)
-        has_lin = want_logit and meta.with_linear
-        no_fm = 0 if (second_order or not want_logit) else _DR_EMBED_NO_FM
+        sum_e = torch.empty((B, D), device=weight.device, dtype=torch.float32) if has_logit else None
+        logit = torch.empty((B,), device=weight.device, dtype=torch.float32) if has_logit else None
+        has_lin = has_logit and meta.with_linear
+        no_fm = 0 if (second_order or not has_logit) else _DR_EMBED_NO_FM
         check(lib.dr_embed_fm_fwd(tp.data_ptr(), lp.data_ptr() if has_lin else None,
                                   rows.data_ptr(), ids.data_ptr(), ids.element_size(),
-                                  _ptr(bias) if want_logit else None, B, S, D, meta.row_stride, meta.lin_stride,
+                                  _ptr(bias), B, S, D, meta.row_stride, meta.lin_stride,
                                   (meta.flags if has_lin else 0) | no_fm, stack.data_ptr(), _ptr(sum_e), _ptr(logit),
                                   _stream()), "dr_embed_fm_fwd")
-        ctx.meta = meta
+        ctx.meta, ctx.saved_bags = meta, saved_bags
         ctx.no_fm = no_fm
-        ctx.want_logit = want_logit
+        ctx.has_logit = has_logit
         ctx.has_lin = has_lin
-        ctx.has_bias = bias is not None
-        ctx.save_for_backward(ids, stack, sum_e, weight, linear, bias)
-        if want_logit:
+        ctx.save_for_backward(ids, stack, sum_e, weight, linear, bias, rows)
+        if has_logit:
             return stack, logit
         dummy = stack.new_zeros((0,))
         ctx.mark_non_differentiable(dummy)
@@ -95,64 +102,62 @@ class EmbedFM(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_stack, g_logit):
         lib = _lib.load()
-        ids, stack, sum_e, weight, linear, bias = ctx.saved_tensors
-        meta = ctx.meta
+        ids, stack, sum_e, weight, linear, bias, rows = ctx.saved_tensors
+        meta, bags = ctx.meta, ctx.saved_bags
         B, S = ids.shape
         D = meta.dim
-        want_logit = ctx.want_logit
         g_stack = None if g_stack is None else _f32(g_stack, "g_stack")
-        g_logit = _f32(g_logit, "g_logit") if (want_logit and g_logit is not None) else None
+        g_logit = _f32(g_logit, "g_logit") if (ctx.has_logit and g_logit is not None) else None
         if g_stack is None and g_logit is None:
-            return None, None, None, None, None, None, None
-        if _row_opt(meta) is not None:
-            return EmbedFM._backward_rows(ctx, ids, stack, sum_e, bias, g_stack, g_logit)
-        fused = meta.sparse_lr is not None
-        if fused:
-            gw, gl, gb = weight, linear, bias
-            scale = -float(meta.sparse_lr)
-            tp, lp, rows = meta.pointers(weight, linear)
-        else:
-            gw = torch.zeros_like(weight)
-            gl = torch.zeros_like(linear) if (linear is not None and g_logit is not None) else None
-            gb = torch.zeros_like(bias) if (bias is not None and g_logit is not None) else None
-            scale = 1.0
-            tp, lp, rows = meta.pointers(gw, gl, cache=False)
+            return None, None, None, None, None, None, None, None
+        if g_logit is None and bags and ctx.has_lin:
+            g_logit = torch.zeros((B,), device=stack.device, dtype=torch.float32)
         lin_grad = ctx.has_lin and g_logit is not None
-        with torch.no_grad():
+
+        def fm_bwd(ids, rows, row_stride, lin_stride, flags, tp, lp, gb, scale):
             check(lib.dr_embed_fm_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(),
                                       stack.data_ptr(), _ptr(sum_e), _ptr(g_logit), _ptr(g_stack),
-                                      B, S, D, meta.row_stride, meta.lin_stride,
-                                      (meta.flags if lin_grad else 0) | (ctx.no_fm if g_logit is not None else 0),
-                                      tp.data_ptr(),
-                                      lp.data_ptr() if lin_grad else None,
-                                      _ptr(gb) if g_logit is not None else None, scale, _stream()),
-                  "dr_embed_fm_bwd")
-        if fused:
-            return None, None, None, None, None, None, None
-        return None, gw, gl, gb, None, None, None
+                                      B, S, D, row_stride, lin_stride, flags, tp.data_ptr(), _ptr(lp), _ptr(gb),
+                                      scale, _stream()), "dr_embed_fm_bwd")
 
-    @staticmethod
-    def _backward_rows(ctx, ids, stack, sum_e, bias, g_stack, g_logit):
-        """A RowSparseAdam trains the tables: hand it what its step() needs and return the bias gradient only."""
-        lib = _lib.load()
-        meta = ctx.meta
-        opt = meta.row_optimizer
-        B, S = ids.shape
-        D = meta.dim
-        if g_logit is not None and not ctx.no_fm:
-            opt.record_fm(ids, stack, sum_e, g_logit, g_stack)
-        else:     # no FM term: the stack gradient is the row gradient, g_logit the first-order one
-            g, ld, sl = (g_stack, S * D, D) if g_stack is not None else (stack.new_zeros((D,)), 0, 0)
-            gl, gl_ld = None, 0
-            if meta.with_linear:
-                gl, gl_ld = (g_logit, 1) if (g_logit is not None and ctx.has_lin) else (stack.new_zeros((1,)), 0)
-            opt.record_rows(ids, g, 0, ld, sl, gl, 0, gl_ld, 0)
-        gb = None
-        if ctx.has_bias and g_logit is not None:
-            gb = torch.empty_like(bias)
-            check(lib.dr_act_bwd_colsum(None, g_logit.data_ptr(), B, 1, 0, None, gb.data_ptr(), _stream()),
-                  "dr_act_bwd_colsum")
-        return None, None, None, gb, None, None, None
+        def launch(tp, lp, gb, scale):
+            fm_bwd(ids, rows, meta.row_stride, meta.lin_stride,
+                   (meta.flags if lin_grad else 0) | (ctx.no_fm if g_logit is not None else 0),
+                   tp, lp if lin_grad else None, gb if g_logit is not None else None, scale)
+
+        def record(opt):
+            """Hand the RowSparseAdam what its step() needs; the bias gradient is the only one returned."""
+            if bags and ctx.has_lin:
+                # the FM term: one dr_embed_fm_bwd forms every lookup's gradient rows in [B, S, D] / [B, S] scratch
+                # "tables" that lookup (b, s) reads as row b, and the bias gradient
+                dev = stack.device
+                g = torch.zeros((B, S, D), device=dev, dtype=torch.float32)
+                gl = torch.zeros((B, S), device=dev, dtype=torch.float32)
+                gb = torch.zeros_like(bias)
+                cols = torch.arange(S, device=dev, dtype=torch.int64)
+                rows_b = torch.full((S,), B, device=dev, dtype=torch.int64)
+                ar = torch.arange(B, device=dev, dtype=ids.dtype).unsqueeze(1).expand(B, S).contiguous()
+                with torch.no_grad():
+                    fm_bwd(ar, rows_b, S * D, S, 0, g.data_ptr() + cols * (4 * D), gl.data_ptr() + cols * 4, gb, 1.0)
+                _record_lookups(opt, ids, bags, g, 0, S * D, D, gl, 0, S, 1)
+                return gb
+            if g_logit is not None and not ctx.no_fm:
+                opt.record_fm(ids, stack, sum_e, g_logit, g_stack)
+            else:     # no FM term: the stack gradient is the row gradient, g_logit the first-order one
+                g, ld, sl = (g_stack, S * D, D) if g_stack is not None else (stack.new_zeros((D,)), 0, 0)
+                gl, gl_ld = None, 0
+                if meta.with_linear:
+                    gl, gl_ld = (g_logit, 1) if (g_logit is not None and ctx.has_lin) else (stack.new_zeros((1,)), 0)
+                _record_lookups(opt, ids, bags, g, 0, ld, sl, gl, 0, gl_ld, 0)
+            gb = None
+            if bias is not None and g_logit is not None:
+                gb = torch.empty_like(bias)
+                check(lib.dr_act_bwd_colsum(None, g_logit.data_ptr(), B, 1, 0, None, gb.data_ptr(), _stream()),
+                      "dr_act_bwd_colsum")
+            return gb
+
+        gw, gl, gb = _route_grads(meta, weight, linear, bias, bags, B, lin_grad, launch, record)
+        return None, gw, gl, gb, None, None, None, None
 
 
 def _row_opt(meta):
@@ -1279,14 +1284,18 @@ class EmbedBag(torch.autograd.Function):
 
 
 def _reduce_bags(lib, ids, weight, linear, meta, bags):
-    """Reduce every multi-valued slot of `bags` into a per-batch scratch "table" of B rows in the collection's own
-    row layout: embedding columns = mean of the bag's valid rows and, when the collection has first-order weights,
-    first-order entry = SUM of their weights (the indicator column is a multi-hot count vector).  A fused kernel then
-    reads slot s from that scratch with ids 0..B-1.
+    """The lookup a fused kernel runs: ids [B, S] over the collection's device pointer arrays.
 
-    Returns (ids, table_ptrs, lin_ptrs, rows, saved_bags, scratch): copies of ids and of the collection's device
-    pointer arrays with the bag slots redirected, the (slot, flat ids, row_splits) list the backward needs, and the
-    scratch tensors, which the caller keeps alive until its kernel is enqueued."""
+    Without bags that is ids and meta.pointers(weight, linear) as they are.  With bags, every multi-valued slot is
+    reduced into a per-batch scratch "table" of B rows in the collection's own row layout: embedding columns = mean of
+    the bag's valid rows and, when the collection has first-order weights, first-order entry = SUM of their weights
+    (the indicator column is a multi-hot count vector).  The kernel then reads slot s from that scratch with ids 0..B-1.
+
+    Returns (ids, table_ptrs, lin_ptrs, rows, saved_bags, scratch): with bags, copies of ids and of the pointer arrays
+    with the bag slots redirected, the (slot, flat ids, row_splits) list the backward needs, and the scratch tensors,
+    which the caller keeps alive until its kernel is enqueued."""
+    if not bags:
+        return (_ids(ids), *meta.pointers(weight, linear), [], None)
     ids = _ids(ids).clone()
     B, S = ids.shape
     D, RS = meta.dim, meta.row_stride
@@ -1323,195 +1332,66 @@ def _reduce_bags(lib, ids, weight, linear, meta, bags):
     return ids, tp, lp, rows, saved_bags, (scratch, scratch_lin)
 
 
-def _bag_grad_scratch(meta, tp, lp, saved_bags, B, with_lin, dev):
-    """Backward twin of _reduce_bags: redirect the bag slots of the gradient pointer arrays (tp, lp, modified in
-    place) to zeroed scratch gradient tables of B rows; returns (gscratch, gscratch_lin)."""
+def _route_grads(meta, weight, linear, bias, saved_bags, B, first_order, launch, record):
+    """Send the table gradients of a lookup backward where the collection trains.  Returns (gw, gl, gb) for autograd.
+
+    - A RowSparseAdam (meta.row_optimizer): record(opt) hands it the lookups and returns the bias gradient; the tables
+      get none.
+    - Fused sparse SGD (meta.sparse_lr = lr): launch(tp, lp, gb, scale) enqueues the backward kernel over the
+      parameters themselves with scale = -lr; nothing is returned.
+    - Otherwise zeroed dense gradients, scale = 1; the first-order ones (linear, bias) only when first_order.
+
+    A bag slot of saved_bags (from _reduce_bags) is pointed at a zeroed scratch gradient table of B rows, which
+    dr_embed_bag_bwd then spreads over the bag's rows (embedding / count, first-order x 1)."""
+    opt = _row_opt(meta)
+    if opt is not None:
+        return None, None, record(opt)
+    lib = _lib.load()
+    fused_sgd = meta.sparse_lr is not None
+    if fused_sgd:
+        gw, gl, gb, scale = weight, linear, bias, -float(meta.sparse_lr)
+    else:
+        gw = torch.zeros_like(weight)
+        gl = torch.zeros_like(linear) if (linear is not None and first_order) else None
+        gb = torch.zeros_like(bias) if (bias is not None and first_order) else None
+        scale = 1.0
+    tp, lp, _ = meta.pointers(gw, gl, cache=fused_sgd)
     D, RS = meta.dim, meta.row_stride
     fused_rows = meta.layout == "fused"
-    nb = len(saved_bags)
-    gscratch = torch.zeros((nb, B, RS), device=dev, dtype=torch.float32)
-    gscratch_lin = None if (fused_rows or not with_lin) else torch.zeros((nb, B), device=dev, dtype=torch.float32)
-    for k, (s, _, _) in enumerate(saved_bags):
-        tp[s] = gscratch[k].data_ptr()
-        if with_lin:
-            lp[s] = gscratch[k].data_ptr() + 4 * D if fused_rows else gscratch_lin[k].data_ptr()
-    return gscratch, gscratch_lin
-
-
-def _spread_bag_grads(lib, meta, gw, gl, saved_bags, gscratch, gscratch_lin, B, with_lin):
-    """Spread each bag slot's scratch gradient over the bag's rows of gw (embedding / count) and of the first-order
-    weights (x 1) with dr_embed_bag_bwd.  The scratch already carries the caller's scale: it is spread with 1."""
-    D, RS = meta.dim, meta.row_stride
-    fused_rows = meta.layout == "fused"
-    for k, (s, bid, bsp) in enumerate(saved_bags):
-        off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
-        base = gw.data_ptr() + 4 * off * RS
-        _bag_bwd(lib, bid, bsp, B, D, "mean", gscratch[k].data_ptr(), RS, n_rows, RS, base, 1.0)
-        if not with_lin:
-            continue
-        if fused_rows:
-            _bag_bwd(lib, bid, bsp, B, 1, "sum", gscratch[k].data_ptr() + 4 * D, RS, n_rows, RS, base + 4 * D, 1.0)
-        else:
-            _bag_bwd(lib, bid, bsp, B, 1, "sum", gscratch_lin[k].data_ptr(), 1, n_rows, 1,
-                     gl.data_ptr() + 4 * off, 1.0)
-
-
-class EmbedFMMixed(torch.autograd.Function):
-    """EmbedFM for a collection in which some slots are multi-valued (SURVEY 8f #2).
-
-    Each ragged slot r is first reduced into a per-batch scratch "table" of B rows in the collection's own row
-    layout (embedding columns = mean of the bag's valid rows, first-order entry = SUM of their weights: the
-    indicator column is a multi-hot count vector); the fused gather + FM kernel then reads slot r from that
-    scratch with ids 0..B-1, so the whole model is still ONE dr_embed_fm_fwd launch.  Backward mirrors it: the
-    fused backward accumulates slot r's per-example gradient in a scratch grad table, dr_embed_bag_bwd spreads
-    it over the bag's rows (embedding / count, first-order x 1).  The scratch handling is shared with FnnInputFn
-    (_reduce_bags, _bag_grad_scratch, _spread_bag_grads).
-
-    ids [B, S]: columns of ragged slots are ignored.  bags: {slot: (flat_ids, row_splits[B+1])}.
-    """
-
-    @staticmethod
-    def forward(ctx, ids, weight, linear, bias, meta, bags):
-        lib = _lib.load()
-        if _row_opt(meta) is not None:
-            meta.row_optimizer.catch_up(ids, bags)
-        if not meta.with_linear:
-            return EmbedFMMixed._forward_no_linear(ctx, ids, weight, meta, bags)
-        if bias is None:
-            raise ValueError("EmbedFMMixed needs a collection with the first-order term (with_linear=True)")
-        ids, tp, lp, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, linear, meta, bags)
-        B, S = ids.shape
-        D, RS = meta.dim, meta.row_stride
-        dev = weight.device
-        stack = torch.empty((B, S, D), device=dev, dtype=torch.float32)
-        sum_e = torch.empty((B, D), device=dev, dtype=torch.float32)
-        logit = torch.empty((B,), device=dev, dtype=torch.float32)
-        check(lib.dr_embed_fm_fwd(tp.data_ptr(), lp.data_ptr(), rows.data_ptr(), ids.data_ptr(), ids.element_size(),
-                                  _ptr(bias), B, S, D, RS, meta.lin_stride, meta.flags, stack.data_ptr(),
-                                  sum_e.data_ptr(), logit.data_ptr(), _stream()), "dr_embed_fm_fwd")
-        ctx.meta, ctx.saved_bags = meta, saved_bags
-        ctx.save_for_backward(ids, stack, sum_e, weight, linear, bias, rows)
-        return stack, logit
-
-    @staticmethod
-    def _forward_no_linear(ctx, ids, weight, meta, bags):
-        """Embeddings only (a collection without first-order weights, e.g. WDL's deep half): the bags are
-        mean-reduced into scratch tables and one dr_embed_fm_fwd without a logit gathers the stack."""
-        lib = _lib.load()
-        ids, tp, _, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, None, meta, bags)
-        B, S = ids.shape
-        D, RS = meta.dim, meta.row_stride
-        dev = weight.device
-        stack = torch.empty((B, S, D), device=dev, dtype=torch.float32)
-        check(lib.dr_embed_fm_fwd(tp.data_ptr(), None, rows.data_ptr(), ids.data_ptr(), ids.element_size(), None,
-                                  B, S, D, RS, meta.lin_stride, 0, stack.data_ptr(), None, None, _stream()),
-              "dr_embed_fm_fwd")
-        ctx.meta, ctx.saved_bags = meta, saved_bags
-        ctx.save_for_backward(ids, stack, None, weight, None, None, rows)
-        dummy = stack.new_zeros((0,))
-        ctx.mark_non_differentiable(dummy)
-        return stack, dummy
-
-    @staticmethod
-    def _backward_no_linear(ctx, g_stack):
-        lib = _lib.load()
-        ids, stack, _, weight, _, _, rows = ctx.saved_tensors
-        meta = ctx.meta
-        if g_stack is None:
-            return None, None, None, None, None, None
-        g_stack = _f32(g_stack, "g_stack")
-        B, S = ids.shape
-        D, RS = meta.dim, meta.row_stride
-        fused_sgd = meta.sparse_lr is not None
-        gw, scale = (weight, -float(meta.sparse_lr)) if fused_sgd else (torch.zeros_like(weight), 1.0)
-        tp, lp, _ = meta.pointers(gw, None, cache=False)
-        tp = tp.clone()
-        gscratch, gscratch_lin = _bag_grad_scratch(meta, tp, lp, ctx.saved_bags, B, False, weight.device)
-        with torch.no_grad():
-            check(lib.dr_embed_fm_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(), stack.data_ptr(), None, None,
-                                      g_stack.data_ptr(), B, S, D, RS, meta.lin_stride, 0, tp.data_ptr(), None, None,
-                                      scale, _stream()), "dr_embed_fm_bwd")
-            _spread_bag_grads(lib, meta, gw, None, ctx.saved_bags, gscratch, gscratch_lin, B, False)
-        return None, (None if fused_sgd else gw), None, None, None, None
-
-    @staticmethod
-    def _backward_rows(ctx, g_stack, g_logit):
-        """A RowSparseAdam trains the tables: hand it the per-lookup gradient rows (the bag slots' as their bags' rows)
-        and return the bias gradient only.  Without the FM term they are g_stack itself; with it, one dr_embed_fm_bwd
-        forms them in [B, S, D] / [B, S] scratch "tables" that lookup (b, s) reads as row b."""
-        lib = _lib.load()
-        meta = ctx.meta
-        ids, stack, sum_e, _, _, bias, _ = ctx.saved_tensors
-        B, S = ids.shape
-        D = meta.dim
-        dev = stack.device
-        g_stack = None if g_stack is None else _f32(g_stack, "g_stack")
-        g_logit = None if g_logit is None else _f32(g_logit, "g_logit")
-        if g_stack is None and (g_logit is None or not meta.with_linear):
-            return None, None, None, None, None, None
-        gb, gl, gl_ld, gl_sl = None, None, 0, 0
-        if not meta.with_linear:
-            g, ld, sl = g_stack, S * D, D
-        else:
-            if g_logit is None:
-                g_logit = torch.zeros((B,), device=dev, dtype=torch.float32)
-            g = torch.zeros((B, S, D), device=dev, dtype=torch.float32)
-            gl = torch.zeros((B, S), device=dev, dtype=torch.float32)
-            gb = torch.zeros_like(bias)
-            ld, sl, gl_ld, gl_sl = S * D, D, S, 1
-            cols = torch.arange(S, device=dev, dtype=torch.int64)
-            tp, lp = g.data_ptr() + cols * (4 * D), gl.data_ptr() + cols * 4
-            rows_b = torch.full((S,), B, device=dev, dtype=torch.int64)
-            ar = torch.arange(B, device=dev, dtype=ids.dtype).unsqueeze(1).expand(B, S).contiguous()
-            with torch.no_grad():
-                check(lib.dr_embed_fm_bwd(ar.data_ptr(), ar.element_size(), rows_b.data_ptr(), stack.data_ptr(),
-                                          sum_e.data_ptr(), g_logit.data_ptr(), _ptr(g_stack), B, S, D, ld, S, 0,
-                                          tp.data_ptr(), lp.data_ptr(), gb.data_ptr(), 1.0, _stream()),
-                      "dr_embed_fm_bwd")
-        opt = meta.row_optimizer
-        opt.record_rows(_no_lookup(ids, [s for s, _, _ in ctx.saved_bags]), g, 0, ld, sl, gl, 0, gl_ld, gl_sl)
-        for s, bid, bsp in ctx.saved_bags:
-            opt.record_bag(s, bid, bsp, g, s * sl, ld, gl, s * gl_sl, gl_ld)
-        return None, None, None, gb, None, None
-
-    @staticmethod
-    def backward(ctx, g_stack, g_logit):
-        if _row_opt(ctx.meta) is not None:
-            return EmbedFMMixed._backward_rows(ctx, g_stack, g_logit)
-        if not ctx.meta.with_linear:
-            return EmbedFMMixed._backward_no_linear(ctx, g_stack)
-        lib = _lib.load()
-        ids, stack, sum_e, weight, linear, bias, rows = ctx.saved_tensors
-        meta = ctx.meta
-        B, S = ids.shape
-        D, RS = meta.dim, meta.row_stride
-        dev = weight.device
-        g_stack = None if g_stack is None else _f32(g_stack, "g_stack")
-        g_logit = None if g_logit is None else _f32(g_logit, "g_logit")
-        if g_stack is None and g_logit is None:
-            return None, None, None, None, None, None
-        if g_logit is None:
-            g_logit = torch.zeros((B,), device=dev, dtype=torch.float32)
-        fused_sgd = meta.sparse_lr is not None
-        if fused_sgd:
-            gw, gl, gb, scale = weight, linear, bias, -float(meta.sparse_lr)
-        else:
-            gw = torch.zeros_like(weight)
-            gl = None if linear is None else torch.zeros_like(linear)
-            gb = None if bias is None else torch.zeros_like(bias)
-            scale = 1.0
-        tp, lp, _ = meta.pointers(gw, gl, cache=False)
+    if saved_bags:
         tp, lp = tp.clone(), lp.clone()
-        gscratch, gscratch_lin = _bag_grad_scratch(meta, tp, lp, ctx.saved_bags, B, True, dev)
-        with torch.no_grad():
-            check(lib.dr_embed_fm_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(), stack.data_ptr(),
-                                      sum_e.data_ptr(), g_logit.data_ptr(), _ptr(g_stack), B, S, D, RS,
-                                      meta.lin_stride, meta.flags, tp.data_ptr(), lp.data_ptr(), _ptr(gb), scale,
-                                      _stream()), "dr_embed_fm_bwd")
-            _spread_bag_grads(lib, meta, gw, gl, ctx.saved_bags, gscratch, gscratch_lin, B, True)
-        if fused_sgd:
-            return None, None, None, None, None, None
-        return None, gw, gl, gb, None, None
+        gscratch = torch.zeros((len(saved_bags), B, RS), device=weight.device, dtype=torch.float32)
+        gscratch_lin = (None if (fused_rows or not first_order)
+                        else torch.zeros((len(saved_bags), B), device=weight.device, dtype=torch.float32))
+        for k, (s, _, _) in enumerate(saved_bags):
+            tp[s] = gscratch[k].data_ptr()
+            if first_order:
+                lp[s] = gscratch[k].data_ptr() + 4 * D if fused_rows else gscratch_lin[k].data_ptr()
+    with torch.no_grad():
+        launch(tp, lp, gb, scale)
+        # the scratch already carries the scale: it is spread with 1
+        for k, (s, bid, bsp) in enumerate(saved_bags):
+            off, n_rows = int(meta._offsets[s]), meta.rows_list[s]
+            base = gw.data_ptr() + 4 * off * RS
+            _bag_bwd(lib, bid, bsp, B, D, "mean", gscratch[k].data_ptr(), RS, n_rows, RS, base, 1.0)
+            if not first_order:
+                continue
+            if fused_rows:
+                _bag_bwd(lib, bid, bsp, B, 1, "sum", gscratch[k].data_ptr() + 4 * D, RS, n_rows, RS, base + 4 * D, 1.0)
+            else:
+                _bag_bwd(lib, bid, bsp, B, 1, "sum", gscratch_lin[k].data_ptr(), 1, n_rows, 1,
+                         gl.data_ptr() + 4 * off, 1.0)
+    if fused_sgd:
+        return None, None, None
+    return gw, gl, gb
+
+
+def _record_lookups(opt, ids, saved_bags, g, g_off, g_ld, g_slot, gl, gl_off, gl_ld, gl_slot):
+    """Hand RowSparseAdam `opt` the gradient rows of a lookup: lookup (b, s) at float g_off + b g_ld + s g_slot of g,
+    its first-order gradient likewise in gl.  A bag slot's row is its bag's, given to record_bag."""
+    opt.record_rows(_no_lookup(ids, [s for s, _, _ in saved_bags]), g, g_off, g_ld, g_slot, gl, gl_off, gl_ld, gl_slot)
+    for s, bid, bsp in saved_bags:
+        opt.record_bag(s, bid, bsp, g, g_off + s * g_slot, g_ld, gl, gl_off + s * gl_slot, gl_ld)
 
 
 def fnn_layout(S: int, D: int):
@@ -1526,10 +1406,10 @@ class FnnInputFn(torch.autograd.Function):
     concat([bias, w_1..w_S, e_1..e_S]) in the padded row layout of fnn_layout, written by ONE dr_fnn_input_fwd over
     the collection `meta` (fused or split layout).  `bias` is a device [1] tensor the kernel reads (a constant of
     the model: it gets no gradient).  Multi-valued slots (bags, {slot: (flat_ids, row_splits)}) are reduced first
-    into scratch tables as EmbedFMMixed does (embedding = mean, w = sum).
+    into scratch tables as in EmbedFM (embedding = mean, w = sum).
 
-    Backward: dr_fnn_input_bwd scatter-adds the embedding and w columns of g_x into dense gradients of weight /
-    linear (meta.sparse_lr is None), or applies the fused sparse SGD in place (meta.sparse_lr = lr).
+    Backward: dr_fnn_input_bwd scatter-adds the embedding and w columns of g_x where _route_grads sends them; under a
+    RowSparseAdam g_x itself holds every lookup's gradient row.
     """
 
     @staticmethod
@@ -1542,12 +1422,7 @@ class FnnInputFn(torch.autograd.Function):
             raise ValueError(f"FnnInputFn: bias must have one element, got {tuple(bias.shape)}")
         if _row_opt(meta) is not None:
             meta.row_optimizer.catch_up(ids, bags)
-        if bags:
-            ids, tp, lp, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, linear, meta, bags)
-        else:
-            ids = _ids(ids)
-            tp, lp, rows = meta.pointers(weight, linear)
-            saved_bags = []
+        ids, tp, lp, rows, saved_bags, _scratch = _reduce_bags(lib, ids, weight, linear, meta, bags)
         B, S = ids.shape
         D = meta.dim
         _, ld = fnn_layout(S, D)
@@ -1570,31 +1445,16 @@ class FnnInputFn(torch.autograd.Function):
         B, S = ids.shape
         D = meta.dim
         P, ld = fnn_layout(S, D)
-        opt = _row_opt(meta)
-        if opt is not None:     # a RowSparseAdam trains the tables: g_x holds every lookup's gradient row
-            opt.record_rows(_no_lookup(ids, [s for s, _, _ in ctx.saved_bags]), g_x, P, ld, D, g_x, 1, ld, 1)
-            for s, bid, bsp in ctx.saved_bags:
-                opt.record_bag(s, bid, bsp, g_x, P + s * D, ld, g_x, 1 + s, ld)
-            return None, None, None, None, None, None
-        fused_sgd = meta.sparse_lr is not None
-        if fused_sgd:
-            gw, gl, scale = weight, linear, -float(meta.sparse_lr)
-        else:
-            gw = torch.zeros_like(weight)
-            gl = None if linear is None else torch.zeros_like(linear)
-            scale = 1.0
-        tp, lp, _ = meta.pointers(gw, gl, cache=fused_sgd)
-        if ctx.saved_bags:
-            tp, lp = tp.clone(), lp.clone()
-            gscratch, gscratch_lin = _bag_grad_scratch(meta, tp, lp, ctx.saved_bags, B, True, weight.device)
-        with torch.no_grad():
+
+        def launch(tp, lp, gb, scale):
             check(lib.dr_fnn_input_bwd(ids.data_ptr(), ids.element_size(), rows.data_ptr(), g_x.data_ptr(), B, S, D,
                                        ld, meta.row_stride, meta.lin_stride, meta.flags, tp.data_ptr(), lp.data_ptr(),
                                        scale, _stream()), "dr_fnn_input_bwd")
-            if ctx.saved_bags:
-                _spread_bag_grads(lib, meta, gw, gl, ctx.saved_bags, gscratch, gscratch_lin, B, True)
-        if fused_sgd:
-            return None, None, None, None, None, None
+
+        def record(opt):
+            _record_lookups(opt, ids, ctx.saved_bags, g_x, P, ld, D, g_x, 1, ld, 1)
+
+        gw, gl, _ = _route_grads(meta, weight, linear, None, ctx.saved_bags, B, True, launch, record)
         return None, gw, gl, None, None, None
 
 
